@@ -1,16 +1,15 @@
 #!/usr/bin/env python
 """bench.py -- protein pairs/sec of the IEGMN hot path (IEGMN layers + keypoints + Kabsch).
 
-    python bench.py --gpus N --steps K --warmup W            # B200 engine (this repo)
+    python bench.py --gpus N --steps K --warmup W            # H100 engine (this repo)
     python bench.py --impl reference --gpus N ...            # CPU reference arm (oracle port, rank 0)
     python bench.py --workload {db5-shaped,db5-testset,large,train} ...
 
 Workloads (BASELINE.json configs):
   db5-shaped   (headline, north_star / configs[1] shape) synthetic DB5.5-shaped residue graphs, 200+200 residues, k=10,
-               8-layer IEGMN with the shipped DIPS checkpoint's weights, batched inference, 370 pairs/step/GPU (the batch is
-               sized to the machine: 370 pairs = 1480 attention tiles, 1157 node tiles and 12 334 edge tiles, i.e. 5.00 / 3.91 /
-               41.7 rounds of the 296 resident tile groups of a B200, where 256 pairs left the last attention / node round
-               54 % / 30 % empty: +5.5 % pairs/s).
+               8-layer IEGMN with the shipped DIPS checkpoint's weights, batched inference, 330 pairs/step/GPU (the batch is
+               sized to the machine: 330 pairs = 1320 attention tiles, 1032 node tiles and 11 000 edge tiles, i.e. 10.0 / 7.82 /
+               83.3 rounds of the 132 resident tile groups of an H100, one per SM).
   db5-testset  (configs[1] literally) 25 pairs with the (N_l, N_r) sizes of the DB5.5 test set as ONE ragged batch.
   large        (configs[4]) synthetic 2000+2000-residue complexes, 8 pairs/step/GPU.
   train        (configs[2]/[3]) DIPS-shaped ragged batch of 32 pairs/GPU, 5-layer shared IEGMN, forward + losses
@@ -18,10 +17,14 @@ Workloads (BASELINE.json configs):
 Pairs shard across ranks by estimated cost (equidock_public_b200.sharding) with no data-path collective (weak scaling).
 One step = one pass of the hot path over the rank's batch.  Prints ONE JSON line on rank 0.
 
-Timing protocol: W warm-up steps, then R repetitions (default 5) of EXACTLY K steps, each repetition bracketed by a
-barrier + torch.cuda.synchronize() on both sides and timed with CUDA events on the launching stream; a repetition's
-time is the MAX over ranks; `value` is the MEDIAN repetition (all repetitions are in `rep_ms`).  Clocks are sampled
-in-process through NVML from one second before the first repetition to the end of the last.
+Timing protocol: W warm-up steps, then R repetitions (--reps, default 1: K timed steps in all) of EXACTLY K steps, each
+repetition bracketed by a barrier + torch.cuda.synchronize() on both sides and timed with CUDA events on the launching
+stream; a repetition's time is the MAX over ranks; `value` is the MEDIAN repetition (all repetitions are in `rep_ms`).
+Clocks are sampled in-process through NVML from one second before the first repetition to the end of the last.
+
+--dump-outputs DIR: after the timed steps, rank 0 writes what the timed path returned for its last step (ligand
+coordinates, keypoints, rotations, translations of every pair; the inputs are seeded, identical from run to run) as
+DIR/<name>.npy, so that two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -62,7 +65,7 @@ def db5_test_sizes():
 
 
 WORKLOADS = {
-    'db5-shaped': dict(n_layers=8, ckpt='dips', pairs_per_gpu=370, flop_per_pair=1.781e9, bytes_per_pair=6.20e6,
+    'db5-shaped': dict(n_layers=8, ckpt='dips', pairs_per_gpu=330, flop_per_pair=1.781e9, bytes_per_pair=6.20e6,
                        text='synthetic DB5.5-shaped 200+200 residues k=10, 8-layer IEGMN (DIPS checkpoint weights), '
                             'batched inference'),
     'db5-testset': dict(n_layers=8, ckpt='dips', pairs_per_gpu=25, flop_per_pair=None, bytes_per_pair=None,
@@ -129,10 +132,6 @@ def edge_stage_algorithmic_flops(n_edges: int, dh: int = 64) -> float:
 
 # bf16 FLOPs the tensor-core edge stage really issues per edge: (K 48 x N 64 + K 64 x N 128) MACs x 6 split products
 EDGE_TC_BF16_FLOP_PER_EDGE = 2.0 * (48 * 64 + 64 * 128) * 6
-# dram__bytes_read.sum + dram__bytes_write.sum of one edge_stage_tc_kernel launch of the headline workload
-# (ncu --set full, profiles/): filled from the committed summary of the current round
-EDGE_TC_NCU_TRAFFIC_BYTES = {370: 286.8e6,   # profiles/r02_final_edge_stage_tc_370pairs_ncu_summary.txt: 255.1 MB read + 31.7 MB written
-                             256: 195.3e6}   # profiles/r02_final_edge_stage_tc_ncu_summary.txt: 176.5 MB read + 18.7 MB written
 
 
 def bind_to_gpu_numa(local_rank: int):
@@ -251,15 +250,15 @@ class ClockSampler:
 
 
 def measured_peaks():
-    """(HBM GB/s, dense bf16 TFLOP/s sustained, source).  The edge stage is timed inside a long step, so the sustained
-    tensor figure is the denominator."""
+    """(HBM GB/s, dense bf16 TFLOP/s sustained, source).  The edge stage is timed inside a long step, so a measured
+    sustained tensor figure is the denominator where one exists; otherwise the H100 SXM data sheet (700 W card)."""
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.isfile(p):
         with open(p) as fh:
             d = json.load(fh)
-        return (float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 1380.0))),
+        return (float(d['hbm_gbs']), float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 989.0))),
                 'measured (MEASURED_PEAKS.json)')
-    return 6650.0, 1380.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 989.0, 'H100 SXM data sheet (700 W)'
 
 
 def effective_cores() -> int:
@@ -444,6 +443,8 @@ def run_engine(args, rank, local_rank, world):
     dev = torch.device('cuda', local_rank)
     D = Dist(world, dev, torch)
     wl = WORKLOADS[args.workload]
+    if args.dump_outputs and world > 1:
+        raise SystemExit('--dump-outputs writes one rank\'s outputs: run it with --gpus 1')
     pairs, (lo, hi), sizes = make_pairs(args, rank, world)
     B = len(pairs)
     total_pairs = len(sizes)
@@ -467,6 +468,8 @@ def run_engine(args, rank, local_rank, world):
     else:
         launch = lambda i: model.forward_async(dev_batches[i & 1], 0)
 
+    last = {}
+
     def value_body():
         pending = None
         for i in range(K):          # step i is launched before step i-1's status words are read
@@ -474,7 +477,7 @@ def run_engine(args, rank, local_rank, world):
             if pending is not None:
                 pending.result()
             pending = nxt
-        pending.result()
+        last['out'] = pending.result()
 
     for _ in range(W):
         launch(0).result()
@@ -488,6 +491,8 @@ def run_engine(args, rank, local_rank, world):
     rep_ms, med, per_rank_ms = timed_reps(torch, D, R, value_body)
     ms_total = rep_ms[med]
     value = total_pairs * K / (ms_total * 1e-3)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last['out'])
 
     # ---- instrumented pass: the same K steps on the eager path with CUDA events around every edge / node stage ------
     timer = engine_mod.NativeStageTimer()
@@ -586,14 +591,14 @@ def run_engine(args, rank, local_rank, world):
     ach = alg / (edge_ms * 1e-3) / 1e9
     alg_flops = edge_stage_algorithmic_flops(n_edges)
     step_ms = ms_total / K
-    sm_mhz = (clocks or {}).get('sm_mhz') or 1965.0
-    fp32_peak = 148 * 128 * 2 * sm_mhz * 1e6 / 1e12
+    sm_mhz = (clocks or {}).get('sm_mhz') or 1980.0
+    fp32_peak = 132 * 128 * 2 * sm_mhz * 1e6 / 1e12      # H100 SXM: 132 SMs x 128 FP32 lanes
     line = {
         'metric': METRIC[args.workload], 'value': value, 'unit': 'pairs/s', 'n_gpus': world,
         'steps': K, 'warmup': W, 'ms_per_step': step_ms, 'higher_is_better': True,
         'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
         'config': workload_config(args, world),
-        'notes': {'l2': f'per-step working set {(n_edges * 108 + n_nodes * 3880) / 1e6:.0f} MB vs 126 MB L2; two device '
+        'notes': {'l2': f'per-step working set {(n_edges * 108 + n_nodes * 3880) / 1e6:.0f} MB vs 50 MB L2; two device '
                         f'batches alternate',
                   'coords_and_head_dtype': 'f64',
                   'value_protocol': f'median of {R} repetitions of the {K}-step loop, each bracketed by barrier+sync, CUDA '
@@ -610,8 +615,7 @@ def run_engine(args, rank, local_rank, world):
         'clocks': {**clocks, 'per_rank_sm_mhz': rank_clocks},
         'roofline': {'kernel': 'edge_stage_tc_kernel', 'bound': 'tensor', 'achieved': alg_flops / (edge_ms * 1e-3) / 1e12,
                      'peak': tc_peak, 'unit': 'TFLOP/s', 'frac': alg_flops / (edge_ms * 1e-3) / 1e12 / tc_peak,
-                     'traffic': EDGE_TC_NCU_TRAFFIC_BYTES.get(B) if args.workload == 'db5-shaped' else None,
-                     'peak_source': peak_src + ', sustained bf16',
+                     'peak_source': peak_src + ', bf16',
                      'algorithmic_flops_per_launch': alg_flops, 'launch_ms': edge_ms,
                      'launch_ms_source': f'CUDA events recorded by eqd_iegmn_forward around every edge-stage launch over an '
                                          f'instrumented (eager) pass of the same {K} steps, {instr_ms / K:.3f} ms/step',
@@ -621,9 +625,9 @@ def run_engine(args, rank, local_rank, world):
                              'algorithmic_bytes_per_launch': alg},
                      'share_of_step': timer.total_ms('edge_stage') / K / step_ms,
                      'share_of_instrumented_step': timer.total_ms('edge_stage') / instr_ms,
-                     'note': 'fp32-accurate GEMMs as 6 bf16 split products on tcgen05 (bf16x6): the tensor ceiling in '
+                     'note': 'fp32-accurate GEMMs as 6 bf16 split products on wgmma (bf16x6): the tensor ceiling in '
                              'algorithmic fp32 FLOPs is peak x 38272 / 135168 = 0.283 x peak; AI ~290 FLOP/B, so the HBM '
-                             'fraction (north star) is small by construction'},
+                             'fraction is small by construction'},
         'kernels_ms': {'edge_stage': edge_ms, 'node_stage': node_ms,
                        'edge_share': timer.total_ms('edge_stage') / K / step_ms,
                        'node_share': timer.total_ms('node_stage') / K / step_ms},
@@ -639,6 +643,20 @@ def run_engine(args, rank, local_rank, world):
         line['cpu_baseline'] = cpu_baseline(pairs, args.cpu_seconds, args.workload)
     print(json.dumps(line), flush=True)
     return D
+
+
+def dump_outputs(out_dir, result):
+    """The 5-tuple of Rigid_Body_Docking_Net.forward (per-pair lists) -> out_dir/<name>.npy, pairs concatenated in batch
+    order: ligand_coors (sum N_l, 3), keypts_ligand / keypts_receptor (B, K, 3), rotation (B, 3, 3), translation (B, 3)."""
+    os.makedirs(out_dir, exist_ok=True)
+    coors, kp_l, kp_r, rot, trans = result
+    arrays = {'ligand_coors': [c.reshape(-1, 3) for c in coors], 'keypts_ligand': kp_l, 'keypts_receptor': kp_r,
+              'rotation': rot, 'translation': [t.reshape(3) for t in trans]}
+    for name, parts in arrays.items():
+        a = np.stack([p.detach().cpu().numpy() for p in parts]) if name != 'ligand_coors' else \
+            np.concatenate([p.detach().cpu().numpy() for p in parts])
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32)
+        np.save(os.path.join(out_dir, f'{name}.npy'), a)
 
 
 def cpu_baseline(pairs, budget_s, workload):
@@ -664,7 +682,7 @@ def main():
     ap.add_argument('--gpus', type=int, default=1)
     ap.add_argument('--steps', type=int, default=10)
     ap.add_argument('--warmup', type=int, default=3)
-    ap.add_argument('--reps', type=int, default=5, help='repetitions of the K-step timed loop (value = median)')
+    ap.add_argument('--reps', type=int, default=1, help='repetitions of the K-step timed loop (value = median)')
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
     ap.add_argument('--workload', default='db5-shaped', choices=sorted(WORKLOADS))
     ap.add_argument('--pairs-per-gpu', type=int, default=0, help='0 = the workload\'s default')
@@ -678,6 +696,8 @@ def main():
     ap.add_argument('--no-cuda-graph', action='store_true')
     ap.add_argument('--no-numa-bind', action='store_true')
     ap.add_argument('--no-residue-e2e', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the last timed step\'s outputs as DIR/<name>.npy (inference workloads, one GPU)')
     ap.add_argument('--watchdog-seconds', type=int, default=1500,
                     help='abort (with a stack dump) instead of stalling forever if the run has not finished by then')
     args = ap.parse_args()
@@ -693,6 +713,8 @@ def main():
         run_reference(args, rank, world)
         return
     if args.workload == 'train':
+        if args.dump_outputs:
+            raise SystemExit('--dump-outputs is supported by the inference workloads')
         import bench_train
         D = bench_train.run(args, rank, local_rank, world, sys.modules[__name__])
     else:

@@ -1,4 +1,4 @@
-"""equidock_public_b200 -- B200-native (sm_100a) engine for EquiDock's IEGMN forward hot path.
+"""equidock_public_b200 -- H100-native (sm_90a) engine for EquiDock's IEGMN forward hot path.
 
     from equidock_public_b200.rigid_docking_model import Rigid_Body_Docking_Net   # reference API
     from equidock_public_b200 import hetero_graph                                  # DGL-free input container

@@ -1,14 +1,15 @@
 // Segmented cross attention of a 64-wide IEGMN layer (rigid_docking_model.py:46-64, 247-256) on the tensor
-// cores (tcgen05, bf16x6):   mu_i = sum_j softmax_j(q_i . k_j) v_j   over the partner protein's nodes j
+// cores (wgmma, bf16x6):   mu_i = sum_j softmax_j(q_i . k_j) v_j   over the partner protein's nodes j
 // (the per-pair block of the reference's dense masked softmax; no 1/sqrt(d)).
 //
-// A tile = 128 query nodes of one protein; two tile groups of 256 threads per CTA (2 threads per query row).
-// K and V of every node arrive as bf16x3 8-node blocks (written by the projection kernel), so a run of
-// 8 blocks (64 keys) is TMA-bulk-copied straight into shared memory as a UMMA B operand:
-//   S = Q K^T   : A = Q (TMEM, bf16x3), B = K blocks, K-major  (n = key, k = d)
-//   O += P V    : A = P (TMEM, bf16x3), B = V blocks, MN-major (k = key, n = d)
+// A tile = 128 query nodes of one protein; one CTA of 256 threads (2 threads per query row, two 64-row warpgroup
+// slabs in the GEMMs).  K and V of every node arrive as bf16x3 8-node blocks (written by the projection kernel), so a
+// run of 8 blocks (64 keys) is TMA-bulk-copied straight into shared memory as a wgmma B operand:
+//   S = Q K^T   : A = Q (smem, bf16x3), B = K blocks, K-major  (n = key, k = d)
+//   O += P V    : A = P (smem, bf16x3), B = V blocks, MN-major (k = key, n = d)
+// The P region also holds the fp32 S and O tiles between the MMAs and the threads that read them.
 // Two passes over the keys (row maxima first, then exp / P.V) instead of an online softmax: the extra S GEMMs
-// are cheap on the tensor pipe and O never has to be rescaled in TMEM.
+// are cheap on the tensor pipe and O never has to be rescaled.
 #include "tc_common.cuh"
 
 namespace eqd {
@@ -21,9 +22,11 @@ __device__ long long g_attn_prof[16];
 #define PROF_MARK(k) do { } while (0)
 #endif
 
-#define AT_THREADS 512
+#define AT_THREADS 256
 #define AT_KEYS 64            // keys per chunk = 8 blocks
 #define AT_CHUNK_BYTES 8192   // per split
+#define AT_A_SPLIT 16384      // Q and P operands: 128 rows x 64 bf16 per split
+#define AT_LD 68              // fp32 row stride of the S / O tiles
 
 // X5 = the 69-wide layer 0: the tensor cores handle channels 0..63 exactly as in a 64-wide layer; channels 64..68 of
 // Q, K, V (fp32 in x5[n][16] = [K64..67 | V64..67 | K68 V68 | Q64..68 | 0], written by the layer-0 projection) are a
@@ -38,9 +41,10 @@ struct AtGroupSmem {
 };
 template <bool X5>
 struct AtSmem {
-  AtGroupSmem<X5> grp[2];
-  unsigned long long k_bar[2][2], v_bar[2][2], mma_bar[2];
-  unsigned int tmem_base;
+  unsigned char qa[3 * AT_A_SPLIT];   // Q (A of S = Q K^T)
+  unsigned char pa[3 * AT_A_SPLIT];   // P (A of O = P V), or the fp32 S / O tile [128][AT_LD]
+  AtGroupSmem<X5> grp;
+  unsigned long long k_bar[2], v_bar[2];
 };
 
 template <bool X5>
@@ -49,36 +53,23 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
                     long kv_split_stride, const float* __restrict__ x5, float* __restrict__ mu, int ldmu) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   AtSmem<X5>& S = *reinterpret_cast<AtSmem<X5>*>(smem_raw);
-  const int tid = threadIdx.x, wg = tid >> 8, q = tid & 255, half = q >> 7, r = q & 127, warp = tid >> 5;
-  AtGroupSmem<X5>& G = S.grp[wg];
+  const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, wgi = tid >> 7;
+  AtGroupSmem<X5>& G = S.grp;
   TRACE_START(1);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&S.mma_bar[a], 1);
-      for (int b = 0; b < 2; ++b) {
-        mbar_init(&S.k_bar[a][b], 1);
-        mbar_init(&S.v_bar[a][b], 1);
-      }
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(&S.k_bar[b], 1);
+      mbar_init(&S.v_bar[b], 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, 0, 14);
-  tc_fence_before();
+  if (q == 0) TRACE_PHASE(1, blockIdx.x, 0, 14);
   __syncthreads();
-  tc_fence_after();
-  if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, 0, 13);
-  const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int wg_u = warp_u >> 3;
-  const bool issuer_warp = (warp_u & 7) == 0;
-  const unsigned tmem_wg = __shfl_sync(0xffffffffu, S.tmem_base, 0) + (unsigned)wg_u * 256;
-  const unsigned tmem = tmem_wg + ((unsigned)((warp & 3) * 32) << 16);
-  // columns: Q (A) 0..95 | S (fp32, 64) / P (A, 3x32) 96..191 | O 192..255
-  const unsigned k_saddr = smem_u32(S.grp[wg_u].k), v_saddr = smem_u32(S.grp[wg_u].v);
-  unsigned kph[2] = {0, 0}, vph[2] = {0, 0}, mph = 0;
+  if (q == 0) TRACE_PHASE(1, blockIdx.x, 0, 13);
+  const unsigned k_saddr = smem_u32(G.k), v_saddr = smem_u32(G.v);
+  const unsigned qa_saddr = smem_u32(S.qa), pa_saddr = smem_u32(S.pa);
+  float* const dtile = reinterpret_cast<float*>(S.pa);
+  unsigned kph[2] = {0, 0}, vph[2] = {0, 0};
   const int B = g.n_pairs;
   const unsigned char* k_g = kv;                              // which = 0
   const unsigned char* v_g = kv + 3 * kv_split_stride;        // which = 1
@@ -104,55 +95,25 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
       s[i] += q5[0] * k4.x + q5[1] * k4.y + q5[2] * k4.z + q5[3] * k4.w + q5[4] * k8;
     }
   };
-  // S = Q K^T for one 64-key chunk in K buffer `kb_`.  hi_only: just the leading bf16 x bf16 product (4 MMAs instead
-  // of 24) -- enough for pass 1, which only needs each row's maximum to within a few units to keep exp() in range; the
-  // softmax result does not depend on which shift is subtracted.
-  auto issue_s = [&](int kb_, bool hi_only) {
-    if (issuer_warp) {
-      tc_fence_after();
-      if (elect_one()) {
-        const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
-        unsigned accum = 0;
-#pragma unroll
-        for (int pr = 0; pr < 6; ++pr) {
-          if (hi_only && pr < 5) continue;
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            umma_ts(tmem_wg + 96, tmem_wg + pa[pr] * 32 + kk * 8,
-                    b_desc_ex(k_saddr + (kb_ * 3 + pb[pr]) * AT_CHUNK_BYTES + kk * 256, 128, 1024), accum);
-            accum = 1;
-          }
-        }
-        umma_commit(&S.mma_bar[wg_u]);
-      }
-      __syncwarp();
-    }
+  // S = Q K^T for one 64-key chunk in K buffer `kb_` -> the fp32 tile in the P region.  hi_only: just the leading
+  // bf16 x bf16 product (4 MMAs instead of 24) -- enough for pass 1, which only needs each row's maximum to within a few
+  // units to keep exp() in range; the softmax result does not depend on which shift is subtracted.  The caller makes
+  // sure nobody still reads the P region.
+  auto gemm_s = [&](int kb_, bool hi_only) {
+    float d[32];
+    wg_gemm6<64>(d, [&](int sp, int kb) { return a_desc_at<EQD_TM>(qa_saddr, AT_A_SPLIT, wgi, sp, kb); },
+                 [&](int sp, int kk) { return b_desc_ex(k_saddr + (kb_ * 3 + sp) * AT_CHUNK_BYTES + kk * 256, 128, 1024); },
+                 4, false, hi_only);
+    wg_store_d<64>(dtile + wgi * 64 * AT_LD, AT_LD, d, tid & 127);
   };
-  // O (+)= P V for one chunk in V buffer `vb_`
-  auto issue_pv = [&](int vb_, unsigned accum0) {
-    if (issuer_warp) {
-      tc_fence_after();
-      if (elect_one()) {
-        const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
-        const unsigned idesc = umma_idesc(64, 1);  // B is MN-major: [key][d]
-        unsigned accum = accum0;
-#pragma unroll
-        for (int pr = 0; pr < 6; ++pr)
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            umma_ts_i(tmem_wg + 192, tmem_wg + 96 + pa[pr] * 32 + kk * 8,
-                      b_desc_ex(v_saddr + (vb_ * 3 + pb[pr]) * AT_CHUNK_BYTES + kk * 2048, 1024, 128), idesc, accum);
-            accum = 1;
-          }
-        umma_commit(&S.mma_bar[wg_u]);
-      }
-      __syncwarp();
-    }
-  };
-  auto wait_mma = [&]() {
-    mbar_wait(&S.mma_bar[wg], mph);
-    mph ^= 1;
-    tc_fence_after();
+  // O = P V for one chunk in V buffer `vb_` -> the fp32 tile in the P region (once every MMA has read P)
+  auto gemm_pv = [&](int vb_) {
+    float d[32];
+    wg_gemm6<64, 1>(d, [&](int sp, int kb) { return a_desc_at<EQD_TM>(pa_saddr, AT_A_SPLIT, wgi, sp, kb); },
+                    [&](int sp, int kk) { return b_desc_ex(v_saddr + (vb_ * 3 + sp) * AT_CHUNK_BYTES + kk * 2048, 1024, 128); },
+                    4, false);
+    __syncthreads();
+    wg_store_d<64>(dtile + wgi * 64 * AT_LD, AT_LD, d, tid & 127);
   };
 
 #ifdef ATTN_PROF
@@ -161,9 +122,9 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
   if (tid == 0)
     for (int k = 0; k < 16; ++k) prof_acc[k] = 0;
 #endif
-  for (int tile = blockIdx.x * 2 + wg; tile < g.n_node_tiles; tile += gridDim.x * 2) {
+  for (int tile = blockIdx.x; tile < g.n_node_tiles; tile += gridDim.x) {
     PROF_MARK(15);
-    if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, tile, 1);
+    if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, 1);
     const int seg = g.node_tiles[2 * tile], node0 = g.node_tiles[2 * tile + 1];
     const int nvalid = min(EQD_TM, g.seg_ptr[seg + 1] - node0);
     const int pseg = seg < B ? seg + B : seg - B;
@@ -173,13 +134,13 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
     const int node = node0 + r;
     const bool valid = r < nvalid;
     PROF_MARK(0);   // tile metadata (dependent global loads)
-    if (nchunks > 0) load_chunk(k_g, G.k[0], &S.k_bar[wg][0], blk_lo, 0);
+    if (nchunks > 0) load_chunk(k_g, G.k[0], &S.k_bar[0], blk_lo, 0);
     float q5[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
     if (X5 && valid) {
 #pragma unroll
       for (int e = 0; e < 5; ++e) q5[e] = x5[(long)node * 16 + 10 + e];
     }
-    {  // Q row -> bf16x3 -> TMEM
+    {  // Q row -> bf16x3 -> A
       float v[32];
       const float4* sp = reinterpret_cast<const float4*>(proj + (long)node * pw + 128 + half * 32);
 #pragma unroll
@@ -187,28 +148,28 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
         float4 t = valid ? sp[c4] : make_float4(0.f, 0.f, 0.f, 0.f);
         v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
       }
-      store_half_split3(tmem + half * 16, v);
+      store_half_split3<EQD_TM>(S.qa, AT_A_SPLIT, r, half * 32, v);
     }
     tc_fence_before();
-    wg_barrier(wg);
-    PROF_MARK(1);   // Q row -> TMEM + barrier
+    __syncthreads();
+    PROF_MARK(1);   // Q row -> A + barrier
     // ---------------- pass 1: row maxima ----------------------------------------------------------------
     float mx = -INFINITY;
     for (int c = 0; c < nchunks; ++c) {
       const int kb_ = c & 1;
-      if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, tile, (c << 4) | 2);
-      mbar_wait(&S.k_bar[wg][kb_], kph[kb_]);
+      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 2);
+      mbar_wait(&S.k_bar[kb_], kph[kb_]);
       kph[kb_] ^= 1;
       PROF_MARK(2);   // pass 1: K chunk wait
-      issue_s(kb_, true);
-      // the other K buffer was last read by the S GEMM of chunk c-1, already waited for: prefetch into it
-      if (c + 1 < nchunks) load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[wg][kb_ ^ 1], blk_lo + 8 * (c + 1), kb_ ^ 1);
-      else load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[wg][kb_ ^ 1], blk_lo, kb_ ^ 1);   // first chunk of pass 2
-      if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, tile, (c << 4) | 3);
-      wait_mma();
-      PROF_MARK(3);   // pass 1: issue + S(hi) MMA wait
+      // the other K buffer was last read by the S GEMM of chunk c-1, complete before the last barrier: prefetch into it
+      if (c + 1 < nchunks) load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[kb_ ^ 1], blk_lo + 8 * (c + 1), kb_ ^ 1);
+      else load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[kb_ ^ 1], blk_lo, kb_ ^ 1);   // first chunk of pass 2
+      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 3);
+      gemm_s(kb_, true);
+      __syncthreads();
+      PROF_MARK(3);   // pass 1: S(hi) MMAs
       float s[32];
-      tmem_ld32f(tmem + 96 + half * 32, s);
+      tile_ld32f(dtile, AT_LD, r, half * 32, s);
       if (X5) add_s5(s, G.x5c[kb_], q5);
       const int key0 = (blk_lo + 8 * c) * 8 + half * 32;
 #pragma unroll
@@ -216,36 +177,35 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
         int kn = key0 + i;
         mx = fmaxf(mx, (kn >= j0 && kn < j1) ? s[i] : -INFINITY);
       }
-      tc_fence_before();
-      wg_barrier(wg);  // S drained before the next S GEMM overwrites it
+      __syncthreads();  // S drained before the next S GEMM overwrites it
       PROF_MARK(4);   // pass 1: ld + max + barrier
     }
     G.red[r * 2 + half] = mx;
-    wg_barrier(wg);
+    __syncthreads();
     mx = fmaxf(G.red[r * 2], G.red[r * 2 + 1]);
     // ---------------- pass 2: P = exp(S - max), O += P V ----------------------------------------------------
     float l = 0.f;
     float o_acc[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
-    if (nchunks > 0) load_chunk(v_g, G.v[0], &S.v_bar[wg][0], blk_lo, -1);
+    if (nchunks > 0) load_chunk(v_g, G.v[0], &S.v_bar[0], blk_lo, -1);
     float o5[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
     for (int c = 0; c < nchunks; ++c) {
       const int kb_ = (nchunks + c) & 1, vb_ = c & 1;   // K buffers keep alternating after pass 1
-      if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, tile, (c << 4) | 4);
-      mbar_wait(&S.k_bar[wg][kb_], kph[kb_]);
+      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 4);
+      mbar_wait(&S.k_bar[kb_], kph[kb_]);
       kph[kb_] ^= 1;
       PROF_MARK(5);   // pass 2: K chunk wait (+ row-max exchange on the first chunk)
-      issue_s(kb_, false);
       if (c + 1 < nchunks) {
-        load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[wg][kb_ ^ 1], blk_lo + 8 * (c + 1), kb_ ^ 1);
-        load_chunk(v_g, G.v[vb_ ^ 1], &S.v_bar[wg][vb_ ^ 1], blk_lo + 8 * (c + 1), -1);   // its last reader (P V of c-1) is done
+        load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[kb_ ^ 1], blk_lo + 8 * (c + 1), kb_ ^ 1);
+        load_chunk(v_g, G.v[vb_ ^ 1], &S.v_bar[vb_ ^ 1], blk_lo + 8 * (c + 1), -1);   // its last reader (P V of c-1) is done
       }
-      if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, tile, (c << 4) | 5);
-      wait_mma();
-      PROF_MARK(6);   // pass 2: issue + S MMA wait
+      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 5);
+      gemm_s(kb_, false);
+      __syncthreads();
+      PROF_MARK(6);   // pass 2: S MMAs
       float s[32];
-      tmem_ld32f(tmem + 96 + half * 32, s);
+      tile_ld32f(dtile, AT_LD, r, half * 32, s);
       if (X5) add_s5(s, G.x5c[kb_], q5);
       const int key0 = (blk_lo + 8 * c) * 8 + half * 32;
       float l4[4] = {0.f, 0.f, 0.f, 0.f};
@@ -266,36 +226,32 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
         }
       }
       l += (l4[0] + l4[1]) + (l4[2] + l4[3]);
-      tc_fence_before();
       PROF_MARK(7);   // pass 2: ld + exp
-      wg_barrier(wg);  // every S value is in registers: the P splits may overwrite the S columns
+      __syncthreads();  // every S value is in registers: the P splits may overwrite the S tile
       PROF_MARK(8);   // pass 2: barrier 1
-      store_half_split3(tmem + 96 + half * 16, s);
+      store_half_split3<EQD_TM>(S.pa, AT_A_SPLIT, r, half * 32, s);
       tc_fence_before();
-      wg_barrier(wg);
+      __syncthreads();
       PROF_MARK(9);   // pass 2: P split/store + barrier 2
-      if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, tile, (c << 4) | 6);
-      mbar_wait(&S.v_bar[wg][vb_], vph[vb_]);
+      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 6);
+      mbar_wait(&S.v_bar[vb_], vph[vb_]);
       vph[vb_] ^= 1;
-      issue_pv(vb_, 0u);
-      if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, tile, (c << 4) | 7);
-      wait_mma();      // P (= the S region) and this V buffer are free again
-      PROF_MARK(10);  // pass 2: V wait + issue + P.V MMA wait
+      gemm_pv(vb_);
+      __syncthreads();
+      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 7);
+      PROF_MARK(10);  // pass 2: V wait + P.V MMAs
       // The tensor core truncates (round-toward-zero) every time it adds into an fp32 accumulator, a systematic
       // bias that grows with the number of accumulation steps; each 64-key chunk is therefore accumulated on its
       // own (4 full-magnitude steps) and the chunks are summed here with round-to-nearest FADDs.
       {
         float oc[32];
-        tmem_ld32f(tmem + 192 + half * 32, oc);
+        tile_ld32f(dtile, AT_LD, r, half * 32, oc);
 #pragma unroll
         for (int i = 0; i < 32; ++i) o_acc[i] += oc[i];
       }
-      // Every thread must have OBSERVED this chunk's v_bar and P.V mma_bar phases before the issuing warp may start the
-      // next ones on the same mbarriers (next chunk's S GEMM commit, the V refill two chunks ahead): a warp that is
-      // held up for a microsecond between the barrier above and its try_wait would otherwise be lapped -- two phase
-      // flips look like none -- and spin forever.  (This was a real, rare hang: ~1 in 10^4 launches back to back.)
-      tc_fence_before();
-      wg_barrier(wg);
+      // Every thread has read its O row (the next S tile overwrites it), and has observed this chunk's v_bar phase
+      // before the V refill two chunks ahead re-arms that mbarrier.
+      __syncthreads();
       PROF_MARK(11);  // pass 2: O ld + accumulate + barrier 3
     }
     // ---------------- mu = O / l -----------------------------------------------------------------------------
@@ -304,7 +260,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
 #pragma unroll
       for (int e = 0; e < 5; ++e) G.red5[(r * 2 + half) * 5 + e] = o5[e];
     }
-    wg_barrier(wg);
+    __syncthreads();
     l = G.red[r * 2] + G.red[r * 2 + 1];
     {
       const float inv = l > 0.f ? 1.f / l : 0.f;
@@ -324,19 +280,15 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
           dst[c4] = make_float4(o_acc[c4 * 4] * inv, o_acc[c4 * 4 + 1] * inv, o_acc[c4 * 4 + 2] * inv, o_acc[c4 * 4 + 3] * inv);
       }
     }
-    tc_fence_before();
-    wg_barrier(wg);
+    __syncthreads();
     PROF_MARK(12);  // mu = O / l, stores, barrier
   }
 #ifdef ATTN_PROF
   if (tid == 0 && blockIdx.x == 0)
     for (int k = 0; k < 16; ++k) g_attn_prof[k] = prof_acc[k];
 #endif
-  if (q == 0) TRACE_PHASE(1, blockIdx.x * 2 + wg, 0xffff, 15);
-  tc_fence_before();
-  __syncthreads();
+  if (q == 0) TRACE_PHASE(1, blockIdx.x, 0xffff, 15);
   TRACE_END(1);
-  tmem_release(S.tmem_base, warp);
 }
 
 }  // namespace eqd
@@ -356,8 +308,7 @@ static int launch_attention_tc(const eqd_graph* g, const float* proj, int pw, co
   if (g->n_node_tiles <= 0) return EQD_OK;
   size_t smem = sizeof(eqd::AtSmem<X5>) + 128;
   EQD_SET_SMEM((eqd::attention_tc_kernel<X5>), smem);
-  int grid = (g->n_node_tiles + 1) / 2;
-  if (grid > 148) grid = 148;
+  int grid = g->n_node_tiles < EQD_SMS ? g->n_node_tiles : EQD_SMS;
   long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
   eqd::attention_tc_kernel<X5><<<grid, AT_THREADS, smem, (cudaStream_t)stream>>>(
       *g, proj, pw, reinterpret_cast<const unsigned char*>(kv), split_stride, x5, mu, ldmu);

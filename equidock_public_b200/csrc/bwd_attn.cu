@@ -265,7 +265,7 @@ extern "C" int eqd_bwd_attention(const eqd_graph* g, const eqd_layer* p_l, const
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;
   if (g->n_node_tiles <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  const int grid = g->n_node_tiles < 148 ? g->n_node_tiles : 148;
+  const int grid = g->n_node_tiles < EQD_SMS ? g->n_node_tiles : EQD_SMS;
   if (extra) {
     EQD_SET_SMEM((eqd::bwd_attn_dq_kernel<true>), eqd::AttnBwdCfg<true>::SMEM_DQ);
     eqd::bwd_attn_dq_kernel<true><<<grid, EQD_THREADS, eqd::AttnBwdCfg<true>::SMEM_DQ, st>>>(*g, p->leaky_slope, proj, mu,

@@ -350,7 +350,7 @@ extern "C" int eqd_bwd_edge(const eqd_graph* g, const eqd_layer* p_l, const floa
     return EQD_ERR_BAD_ARG;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;
   const int ntiles = (g->n_edges + EQD_TM - 1) / EQD_TM;
-  int grid = ntiles < 148 ? ntiles : 148;
+  int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   if (n_partials_out) *n_partials_out = grid > 0 ? grid : 0;
   if (g->n_edges <= 0) return EQD_OK;
   size_t smem = sizeof(eqd::EdgeBwdSmem);

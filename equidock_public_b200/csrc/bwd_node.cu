@@ -289,7 +289,7 @@ extern "C" int eqd_bwd_node_mlp(const eqd_graph* g, const eqd_layer* p_l, const 
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;
   if ((ldh & 3) || (ldmu & 3) || ldh < p->dhp || ldmu < p->dhp) return EQD_ERR_BAD_ARG;
   const int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
-  int grid = ntiles < 148 ? ntiles : 148;
+  int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   if (n_partials_out) *n_partials_out = grid > 0 ? grid : 0;
   if (g->n_nodes <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;

@@ -80,7 +80,7 @@ extern "C" int eqd_bwd_project(const eqd_graph* g, const eqd_layer* p_l, const f
   if (!extra && !(p->dh == 64 && p->dhp == 64)) return EQD_ERR_UNSUPPORTED;
   if (g->n_nodes <= 0) return EQD_OK;
   const int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
-  const int grid = ntiles < 148 * 2 ? ntiles : 148 * 2;
+  const int grid = ntiles < EQD_SMS * 2 ? ntiles : EQD_SMS * 2;
   const size_t smem = (size_t)(EQD_TM * 68 + 2 * EQD_WCHUNK * EQD_WLD) * sizeof(float);
   if (extra) {
     EQD_SET_SMEM((eqd::bwd_proj_kernel<true>), smem);

@@ -168,7 +168,7 @@ extern "C" size_t eqd_tn_partial_floats(int64_t nrows, int32_t K, int32_t ncols,
     return 0;
   }
   const int blocks = ((K + 63) / 64) * ((ncols + 63) / 64);
-  long target = (148 * 4 + blocks - 1) / blocks;               // ~4 CTAs per SM over the whole launch
+  long target = (EQD_SMS * 4 + blocks - 1) / blocks;               // ~4 CTAs per SM over the whole launch
   long rpc = (nrows + target - 1) / target;
   rpc = ((rpc + 63) / 64) * 64;
   if (rpc < 256) rpc = 256;

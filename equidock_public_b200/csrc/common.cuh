@@ -1,4 +1,4 @@
-// Shared device helpers for the IEGMN forward kernels (sm_100a).
+// Shared device helpers for the IEGMN forward kernels (sm_90a).
 //
 // Tile model used by every dense stage: one CTA = 128 threads owns a tile of 128 rows (edges or
 // nodes) x 64 output channels.  Thread (ty = tid>>3, tx = tid&7) holds an 8x8 fp32 micro-tile:
@@ -17,6 +17,8 @@
 
 #define EQD_THREADS 128
 #define EQD_TM 128
+// streaming multiprocessors of an H100 SXM: the grid size of the persistent kernels
+#define EQD_SMS 132
 
 #define EQD_CUDA_LAUNCH_CHECK()                          \
   do {                                                   \

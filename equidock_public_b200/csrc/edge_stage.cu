@@ -195,7 +195,7 @@ extern "C" int eqd_edge_stage_ffma(const eqd_graph* g, const eqd_layer* p_l, con
   int ntiles = (g->n_nodes + tn - 1) / tn;
   size_t smem = sizeof(eqd::EdgeSmem);
   EQD_SET_SMEM((eqd::edge_stage_kernel), smem);
-  int grid = ntiles < 148 * 2 ? ntiles : 148 * 2;
+  int grid = ntiles < EQD_SMS * 2 ? ntiles : EQD_SMS * 2;
   eqd::edge_stage_kernel<<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, proj, x_in, x_orig, aggr, x_out,
                                                                            status, tn);
   EQD_CUDA_LAUNCH_CHECK();

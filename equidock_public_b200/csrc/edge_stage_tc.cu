@@ -1,29 +1,28 @@
-// Edge stage of IEGMN_Layer.forward (rigid_docking_model.py:204-237, 263-292) on the 5th-gen tensor
-// cores (tcgen05 / TMEM), fp32-accurate through a 3-way bf16 split of both operands ("bf16x6":
-// a*w ~ a0w0 + a0w1 + a1w0 + a0w2 + a1w1 + a2w0, fp32 accumulation in TMEM; measured error below a
-// plain fp32 FMA loop, see scripts/tc_probe.cu).
+// Edge stage of IEGMN_Layer.forward (rigid_docking_model.py:204-237, 263-292) on the tensor cores (wgmma),
+// fp32-accurate through a 3-way bf16 split of both operands ("bf16x6": a*w ~ a0w0 + a0w1 + a1w0 + a0w2 + a1w1 + a2w0,
+// fp32 accumulation).
 //
-// One persistent CTA per SM, 2 tile groups of 256 threads; each group owns one tile of <=128 edges at a time
-// (2 threads per edge row: thread (r, half) <-> columns [32 half, +32) of row r <-> TMEM lane r), the two groups run
-// out of phase so one's MMA phases overlap the other's epilogues.  Per tile and group:
+// One persistent CTA of 256 threads per SM owns one tile of <=128 edges at a time (2 threads per edge row:
+// thread (r, half) <-> columns [32 half, +32) of row r; the GEMMs run as two 64-row warpgroup slabs).  Per tile:
 //   he rows (cp.async.bulk -> smem staging, prefetched one tile ahead) + 15 RBFs
-//     -> [he|rbf] bf16x3 -> TMEM (tcgen05.st)                      A operand of GEMM1 (K=48)
-//   GEMM1 (18 tcgen05.mma, B = edge_mlp.0.weight[:, 2dh:] bf16x3 resident in smem)
+//     -> [he|rbf] bf16x3 -> smem                                     A operand of GEMM1 (K=48)
+//   GEMM1 (18 wgmma per warpgroup, B = edge_mlp.0.weight[:, 2dh:] bf16x3 resident in smem)
 //     -> + gathered Psrc[src] + Pdst[dst] (cp.async into smem), LeakyReLU, LayerNorm (the two halves of a row
-//        combine their statistics through smem) -> bf16x3 -> TMEM
-//   GEMM2 and GEMM3 on that one A operand (2 x 24 mma, N=64 halves of the stacked panel [W2 ; W3 W2])
+//        combine their statistics through smem) -> bf16x3 -> smem
+//   GEMM2 and GEMM3 on that one A operand (2 x 24 wgmma, N=64 halves of the stacked panel [W2 ; W3 W2])
 //     -> msg (+bias) -> fp32 tile in smem (mean aggregation at the destination nodes)
 //     -> coordinate MLP hidden layer -> LeakyReLU, dot w4 -> phi ; x' = eta x0 + (1-eta) x + mean(x_rel phi) in fp64.
-// Per-edge activations never leave the SM; weights are read from HBM/L2 once per CTA.
-// The kernel is bound by the dependent chain of a tile group, not by a pipe (profiles/r02_edge_variants.txt): the serial tail of
-// a tile is kept short (a tile whose nodes all have 10 in-edges -- a k-NN graph -- needs no row_ptr lookups; the next tile's
-// coordinate gathers leave two GEMMs early; the coordinate update runs on threads that do no aggregation) and the fp32
-// epilogue arithmetic is written on lane pairs (add / mul / fma.f32x2: the same IEEE results in half the instructions).
+// Per-edge activations never leave the SM; weights are read from HBM/L2 once per CTA.  The A operand region doubles as
+// the fp32 result tile of GEMM1 and GEMM3 once their MMAs are complete.  A tile whose nodes all have 10 in-edges (a
+// k-NN graph) needs no row_ptr lookups, and the coordinate update runs on threads that do no aggregation.
 #include "tc_common.cuh"
 
 namespace eqd {
-#define TC_THREADS 512
+#define TC_THREADS 256
 __device__ __forceinline__ float2 f2(float a, float b) { return make_float2(a, b); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return f2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return f2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return f2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 #define TC_MAX_TN 32          // destination nodes per tile (Pdst staging rows)
 #define TC_LD 68              // fp32 row stride of the staging / msg tile
 #define TC_W_BYTES 67584      // 3 splits x (6144 + 8192 + 8192)
@@ -31,8 +30,9 @@ __device__ __forceinline__ float2 f2(float a, float b) { return make_float2(a, b
 #define TC_W23_BASE 18432    // [W2 ; W3 W2] stacked, N = 128
 #define TC_W23_SPLIT 16384
 #define TC_HE_STAGE_FLOATS (EQD_TM * EQD_EDGE_FEATS + 16)
+#define TC_A_SPLIT 16384      // A operand: 128 rows x K <= 64 bf16 per split
 
-struct TcWgSmem {                         // per warpgroup
+struct TcWgSmem {
   float stage[EQD_TM * TC_LD];            // gathered Psrc rows, later the fp32 msg tile
   float pdst[2][TC_MAX_TN * TC_LD];       // Pdst rows of the tile's destination nodes (prefetched one tile ahead)
   float he[TC_HE_STAGE_FLOATS];           // raw he rows of the tile (bulk-copied, 16B-aligned chunks)
@@ -45,68 +45,45 @@ struct TcWgSmem {                         // per warpgroup
 };
 
 struct TcSmem {
-  unsigned char w[TC_W_BYTES];            // bf16x3 weights, canonical K-major no-swizzle UMMA layout
-  TcWgSmem wg[2];
-  unsigned long long w_bar, mma_bar[2], mma2_bar[2], he_bar[2], a_bar[2];
-  unsigned int tmem_base;
+  unsigned char w[TC_W_BYTES];            // bf16x3 weights, canonical K-major no-swizzle layout
+  unsigned char a[3 * TC_A_SPLIT];        // A operand (bf16x3), or the fp32 result tile [128][TC_LD] of GEMM1 / GEMM3
+  TcWgSmem wg;
+  unsigned long long w_bar, he_bar;
 };
 
 struct EdgeConsts {                       // per-layer vectors, passed by value (constant bank operands)
   float ln_g[64], ln_b[64], b2[64], b3[64], w4[64];
 };
 
-// 512 threads = 2 tile groups x 256; in a group, thread (r = q & 127, half = q >> 7) owns columns
-// [32*half, 32*half+32) of edge row r (TMEM lane r): two threads per row keep the per-thread register
-// footprint <= 128 so that 16 warps (4 per scheduler) hide each other's latencies.
+// thread (r = q & 127, half = q >> 7) owns columns [32*half, 32*half+32) of edge row r
 __global__ void __launch_bounds__(TC_THREADS, 1)
 edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ EdgeConsts cst,
                      const float* __restrict__ proj, const double* __restrict__ x_in, const double* __restrict__ x_orig,
                      float* __restrict__ aggr, double* __restrict__ x_out, int* __restrict__ status, int tn) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   TcSmem& S = *reinterpret_cast<TcSmem*>(smem_raw);
-  const int tid = threadIdx.x, wg = tid >> 8, q = tid & 255, half = q >> 7, r = q & 127, warp = tid >> 5;
-  TcWgSmem& W = S.wg[wg];
+  const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, warp = tid >> 5, wgi = tid >> 7;
+  TcWgSmem& W = S.wg;
   const int pw = 128 + 3 * p.dhp;
   const int ntiles = (g.n_nodes + tn - 1) / tn;
   const float slope = p.leaky_slope;
 
   TRACE_START(0);
-  // ---- one-time setup: TMEM, barriers, weights (one TMA bulk copy) -------------------------------
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
+  // ---- one-time setup: barriers, weights (one TMA bulk copy) -------------------------------------
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
-    mbar_init(&S.mma_bar[0], 1);
-    mbar_init(&S.mma_bar[1], 1);
-    mbar_init(&S.he_bar[0], 1);
-    mbar_init(&S.he_bar[1], 1);
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&S.mma2_bar[a], 1);
-      mbar_init(&S.a_bar[a], 8);      // one arrival per warp of the tile group: "my part of the A operand is in TMEM"
-    }
+    mbar_init(&S.he_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     mbar_expect_tx(&S.w_bar, TC_W_BYTES);
     bulk_g2s(S.w, p.w_edge_tc, TC_W_BYTES, &S.w_bar);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  // warp-uniform copies for the MMA issue path: operands the compiler can prove uniform go straight to uniform
-  // registers (UTCHMMA takes UR operands); anything else costs a per-MMA waterfall loop (ELECT / R2UR / BRA.U.ANY)
-  const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int wg_u = warp_u >> 3;
-  const bool issuer_warp = (warp_u & 7) == 0;
-  const unsigned tmem_base_u = __shfl_sync(0xffffffffu, S.tmem_base, 0);
-  const unsigned tmem_wg = tmem_base_u + (unsigned)wg_u * 256;                   // lane 0 (MMA issuer's view)
-  const unsigned tmem = tmem_wg + ((unsigned)((warp & 3) * 32) << 16);           // my lane quarter
-  const unsigned d_col = tmem + half * 32;                                         // my half of D (64 columns)
-  const unsigned a_col = tmem + 128;                                               // A: 3 splits x 32 columns (D: 0..127)
-  if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, 0, 1);
+  if (q == 0) TRACE_PHASE(0, blockIdx.x, 0, 1);
   mbar_wait(&S.w_bar, 0);
-  unsigned mma_phase = 0, mma2_phase = 0, he_phase = 0, a_phase = 0;
-  const unsigned w_saddr = smem_u32(S.w);
+  unsigned he_phase = 0;
+  const unsigned w_saddr = smem_u32(S.w), a_saddr = smem_u32(S.a);
+  float* const dtile = reinterpret_cast<float*>(S.a);          // fp32 result tile over the A region
+  auto a_desc = [&](int sp, int kb) { return a_desc_at<EQD_TM>(a_saddr, TC_A_SPLIT, wgi, sp, kb); };
 
   // Prefetch of a tile's indices, Pdst rows and he rows.
   auto prefetch = [&](int tile, int buf, int& e0_out, int& ne_out, int& off_l, int& n_l, int& off_r) {
@@ -147,10 +124,10 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
         cp_async16(&W.pdst[buf][row * TC_LD + c4 * 4], proj + (long)(n0 + row) * pw + 64 + c4 * 4, true);
       }
       if (q == 0) {
-        mbar_expect_tx(&S.he_bar[wg], bl + br);
-        if (bl) bulk_g2s(W.he, reinterpret_cast<const unsigned char*>(g.he_lig) + sl, bl, &S.he_bar[wg]);
+        mbar_expect_tx(&S.he_bar, bl + br);
+        if (bl) bulk_g2s(W.he, reinterpret_cast<const unsigned char*>(g.he_lig) + sl, bl, &S.he_bar);
         if (br) bulk_g2s(reinterpret_cast<unsigned char*>(W.he) + dst_r_off, reinterpret_cast<const unsigned char*>(g.he_rec) + sr, br,
-                         &S.he_bar[wg]);
+                         &S.he_bar);
       }
     }
     cp_async_commit();
@@ -165,16 +142,16 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     cp_async_commit();
   };
 
-  int tile = blockIdx.x * 2 + wg;
-  const int tstride = gridDim.x * 2;
+  int tile = blockIdx.x;
+  const int tstride = gridDim.x;
   const int lane = tid & 31, wrow0 = 32 * (warp & 3);
-  const int pair_id = 3 + wg * 4 + (warp & 3);   // named barrier of the two warps that hold rows [wrow0, wrow0 + 32)
+  const int pair_id = 3 + (warp & 3);   // named barrier of the two warps that hold rows [wrow0, wrow0 + 32)
   int buf = 0;
   int e0 = 0, ne = 0, off_l = 0, n_l = 0, off_r = 0;
   if (tile < ntiles) {
     prefetch(tile, buf, e0, ne, off_l, n_l, off_r);
     cp_async_wait<0>();
-    wg_barrier(wg);
+    __syncthreads();
     prefetch_x(buf, ne);
   }
 
@@ -185,32 +162,30 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     if (ne > EQD_TM) {  // in-degree bound violated: flag, skip (uniform per tile group)
       if (q == 0) atomicOr(status + g.n_pairs, EQD_STATUS_DEGREE_OVERFLOW);
       cp_async_wait<0>();
-      wg_barrier(wg);
+      __syncthreads();
       if (has_next) {
         prefetch(tile + tstride, buf ^ 1, e0n, nen, off_ln, n_ln, off_rn);
         cp_async_wait<0>();
-        wg_barrier(wg);
+        __syncthreads();
         prefetch_x(buf ^ 1, nen);
       }
       e0 = e0n; ne = nen; off_l = off_ln; n_l = n_ln; off_r = off_rn; buf ^= 1;
       continue;
     }
-    // ---- S0/S1: indices + coordinates ready; geometry; [he|rbf] -> TMEM ---------------------------------------
-    // Synchronisation inside a tile: two full group barriers (here and before the aggregation).  Everything else is
-    // point to point -- each warp announces its part of an A operand on an mbarrier that only the MMA-issuing warp
-    // waits for, every warp gathers exactly the Psrc rows it will read itself (warp-local visibility), and the two
-    // column halves of a row exchange their LayerNorm statistics through a 64-thread named barrier.
-    if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 2);
+    // ---- S0/S1: indices + coordinates ready; geometry; [he|rbf] -> A ------------------------------------------
+    // Every warp gathers exactly the Psrc rows it will read itself (warp-local visibility), and the two column halves
+    // of a row exchange their LayerNorm statistics through a 64-thread named barrier.
+    if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 2);
     cp_async_wait<0>();
-    wg_barrier(wg);
-    if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 3);
+    __syncthreads();
+    if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 3);
     const bool valid = r < ne;
     const int dn = valid ? W.dst[buf][r] : 0;
     {
       float a1v[24];  // half 0: he[0..23];  half 1: he[24..26], 15 RBFs, 6 zeros
-      mbar_wait(&S.he_bar[wg], he_phase);
+      mbar_wait(&S.he_bar, he_phase);
       he_phase ^= 1;
-      if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 4);
+      if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 4);
       const float* hrow = W.he + (r < n_l ? off_l + r * EQD_EDGE_FEATS : off_r + (r - n_l) * EQD_EDGE_FEATS);
       if (half == 0) {
 #pragma unroll
@@ -243,29 +218,13 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
       unsigned p0[12], p1[12], p2[12];
 #pragma unroll
       for (int c = 0; c < 12; ++c) split3_pair(a1v[2 * c], a1v[2 * c + 1], p0[c], p1[c], p2[c]);
-      const unsigned ab = a_col + half * 12;
-      tmem_st8(ab, p0);      tmem_st4(ab + 8, p0 + 8);
-      tmem_st8(ab + 32, p1); tmem_st4(ab + 40, p1 + 8);
-      tmem_st8(ab + 64, p2); tmem_st4(ab + 72, p2 + 8);
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+#pragma unroll
+      for (int j = 0; j < 3; ++j) a_store8<EQD_TM>(S.a, TC_A_SPLIT, r, half * 24 + 8 * j, p0 + 4 * j, p1 + 4 * j, p2 + 4 * j);
     }
     tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&S.a_bar[wg]);
-    // ---- GEMM1: [he|rbf] (K=48) x W1e ---------------------------------------------------------------
-    if (issuer_warp) {
-      if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 5);
-      mbar_wait(&S.a_bar[wg_u], a_phase);   // all 8 warps' A columns are in TMEM (and they are done with the he staging)
-      a_phase ^= 1;
-      if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 6);
-      tc_fence_after();
-      if (elect_one()) {
-        issue_gemm(tmem_wg, tmem_wg + 128, 32, w_saddr, TC_W1_SPLIT, 3);
-        umma_commit(&S.mma_bar[wg_u]);
-      }
-      __syncwarp();
-    }
-    // Psrc[src] of MY warp's 32 rows x MY column half -> smem (8 lanes per row: 128 contiguous bytes), behind GEMM1
+    __syncthreads();   // the A operand is complete (and every thread is done with the he staging)
+    if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 5);
+    // Psrc[src] of MY warp's 32 rows x MY column half -> smem (8 lanes per row: 128 contiguous bytes), under GEMM1
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int grow = wrow0 + i * 4 + (lane >> 3);
@@ -276,35 +235,39 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     cp_async_commit();
     // he staging and the other index / Pdst buffers are free now: prefetch the next tile behind the MMAs
     if (has_next) prefetch(tile + tstride, buf ^ 1, e0n, nen, off_ln, n_ln, off_rn);
-    if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 7);
-    mbar_wait(&S.mma_bar[wg], mma_phase);
-    mma_phase ^= 1;
-    tc_fence_after();
-    if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 8);
-    // ---- epilogue 1: + Psrc[src] + Pdst[dst], LeakyReLU, LayerNorm -> bf16x3 -> TMEM ----------------
+    // ---- GEMM1: [he|rbf] (K=48) x W1e ---------------------------------------------------------------
+    {
+      float d[32];
+      wg_gemm6<64>(d, a_desc, [&](int sp, int kb) { return b_desc_ex(w_saddr + sp * TC_W1_SPLIT + kb * 2048, 1024, 128); }, 3,
+                   false);
+      __syncthreads();   // both warpgroups' MMAs have read A: its region takes the result tile
+      wg_store_d<64>(dtile + wgi * 64 * TC_LD, TC_LD, d, tid & 127);
+    }
+    __syncthreads();
+    if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 8);
+    // ---- epilogue 1: + Psrc[src] + Pdst[dst], LeakyReLU, LayerNorm -> bf16x3 -> A ------------------
     {
       float v[32];
-      tmem_ld32f(d_col, v);
+      tile_ld32f(dtile, TC_LD, r, half * 32, v);
       if (has_next) cp_async_wait<1>(); else cp_async_wait<0>();  // my gathers landed (the newest group is the prefetch)
       __syncwarp();                                                  // ... and so did the rest of my warp's
       const int dloc = valid ? dn - n0 : 0;
       const float4* ps = reinterpret_cast<const float4*>(&W.stage[r * TC_LD + half * 32]);
       const float4* pd = reinterpret_cast<const float4*>(&W.pdst[buf][dloc * TC_LD + half * 32]);
       float s4[4] = {0.f, 0.f, 0.f, 0.f};
-      {   // The fp32 epilogue arithmetic is written on lane PAIRS (add.f32x2 / mul.f32x2 / fma.f32x2 of sm_100: one instruction,
-          // two IEEE results -- bitwise the scalar sequence, ~5 % fewer instructions in this latency-bound kernel)
+      {   // the fp32 epilogue arithmetic runs on lane pairs (two independent chains per accumulator)
         float2 s01 = f2(0.f, 0.f), s23 = f2(0.f, 0.f);
         const float2 sl2 = f2(slope, slope);
 #pragma unroll
         for (int c4 = 0; c4 < 8; ++c4) {
           float4 a = ps[c4], b = pd[c4];
-          float2 x01 = __fadd2_rn(__fadd2_rn(f2(v[c4 * 4 + 0], v[c4 * 4 + 1]), f2(a.x, a.y)), f2(b.x, b.y));
-          float2 x23 = __fadd2_rn(__fadd2_rn(f2(v[c4 * 4 + 2], v[c4 * 4 + 3]), f2(a.z, a.w)), f2(b.z, b.w));
-          float2 y01 = __fmul2_rn(x01, sl2), y23 = __fmul2_rn(x23, sl2);
+          float2 x01 = add2(add2(f2(v[c4 * 4 + 0], v[c4 * 4 + 1]), f2(a.x, a.y)), f2(b.x, b.y));
+          float2 x23 = add2(add2(f2(v[c4 * 4 + 2], v[c4 * 4 + 3]), f2(a.z, a.w)), f2(b.z, b.w));
+          float2 y01 = mul2(x01, sl2), y23 = mul2(x23, sl2);
           float2 t01 = f2(fmaxf(x01.x, y01.x), fmaxf(x01.y, y01.y)), t23 = f2(fmaxf(x23.x, y23.x), fmaxf(x23.y, y23.y));
           v[c4 * 4 + 0] = t01.x; v[c4 * 4 + 1] = t01.y; v[c4 * 4 + 2] = t23.x; v[c4 * 4 + 3] = t23.y;
-          s01 = __fadd2_rn(s01, t01);
-          s23 = __fadd2_rn(s23, t23);
+          s01 = add2(s01, t01);
+          s23 = add2(s23, t23);
         }
         s4[0] = s01.x; s4[1] = s01.y; s4[2] = s23.x; s4[3] = s23.y;
       }
@@ -317,16 +280,16 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
         const float2 nmh = f2(-mh, -mh);
 #pragma unroll
         for (int c = 0; c < 32; c += 4) {
-          float2 d01 = __fadd2_rn(f2(v[c], v[c + 1]), nmh), d23 = __fadd2_rn(f2(v[c + 2], v[c + 3]), nmh);
-          q01 = __ffma2_rn(d01, d01, q01);
-          q23 = __ffma2_rn(d23, d23, q23);
+          float2 d01 = add2(f2(v[c], v[c + 1]), nmh), d23 = add2(f2(v[c + 2], v[c + 3]), nmh);
+          q01 = fma2(d01, d01, q01);
+          q23 = fma2(d23, d23, q23);
         }
         q4[0] = q01.x; q4[1] = q01.y; q4[2] = q23.x; q4[3] = q23.y;
       }
       float* redf = reinterpret_cast<float*>(W.red);
       redf[(r * 2 + half) * 2 + 0] = mh;
       redf[(r * 2 + half) * 2 + 1] = (q4[0] + q4[1]) + (q4[2] + q4[3]);
-      if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 9);
+      if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 9);
       pair_barrier(pair_id);   // only the warp that owns the other half of these 32 rows
       const float m0 = redf[r * 4 + 0], m1 = redf[r * 4 + 2];
       const float mean = 0.5f * (m0 + m1);
@@ -337,16 +300,16 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
         const float2 nm = f2(-mean, -mean), rs2 = f2(rstd, rstd);
 #pragma unroll
         for (int c = 0; c < 32; c += 2) {
-          float2 t = __fmul2_rn(__fadd2_rn(f2(v[c], v[c + 1]), nm), rs2);
-          t = __ffma2_rn(t, f2(cst.ln_g[half * 32 + c], cst.ln_g[half * 32 + c + 1]), f2(cst.ln_b[half * 32 + c], cst.ln_b[half * 32 + c + 1]));
+          float2 t = mul2(add2(f2(v[c], v[c + 1]), nm), rs2);
+          t = fma2(t, f2(cst.ln_g[half * 32 + c], cst.ln_g[half * 32 + c + 1]), f2(cst.ln_b[half * 32 + c], cst.ln_b[half * 32 + c + 1]));
           v[c] = t.x; v[c + 1] = t.y;
         }
       }
-      store_half_split3(a_col + half * 16, v);
+      __syncthreads();   // every row of the GEMM1 result tile has been read
+      store_half_split3<EQD_TM>(S.a, TC_A_SPLIT, r, half * 32, v);
     }
     tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&S.a_bar[wg]);
+    __syncthreads();
     if (has_next) {
       // The next tile's x[src] / x[dst] gathers go out here, two GEMMs before they are needed (issued in the tail of the tile
       // their latency sat in front of the next tile's first barrier).  xs of this tile was consumed in S0 by the half-1 thread of my row, which has since met me at the LayerNorm pair
@@ -357,32 +320,22 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     // ---- GEMM2 and GEMM3 on the same A operand ------------------------------------------------------------------
     // msg = W2 a1 + b2 (edge_mlp.4) and the coordinate MLP's hidden pre-activation W3 msg + b3 =
     // (W3 W2) a1 + (W3 b2 + b3) are both linear in a1: the stacked panel [W2 ; W3 W2] gives them from one A operand
-    // (no bf16x3 split of msg, no second TMEM store).  Issued as two N=64 halves with their own completion barriers so
-    // that the msg epilogue runs under the second half's MMAs.
-    if (issuer_warp) {
-      if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 10);
-      mbar_wait(&S.a_bar[wg_u], a_phase);
-      a_phase ^= 1;
-      tc_fence_after();
-      if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 11);
-      if (elect_one()) {
-        const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
-#pragma unroll
-        for (int hn = 0; hn < 2; ++hn) {
-          unsigned accum = 0;
-#pragma unroll
-          for (int pr = 0; pr < 6; ++pr)
-#pragma unroll
-            for (int kb = 0; kb < 4; ++kb) {
-              umma_ts(tmem_wg + hn * 64, tmem_wg + 128 + pa[pr] * 32 + kb * 8,
-                      b_desc_ex(w_saddr + TC_W23_BASE + pb[pr] * TC_W23_SPLIT + kb * 4096 + hn * 1024, 2048, 128), accum);
-              accum = 1;
-            }
-          umma_commit(hn == 0 ? &S.mma_bar[wg_u] : &S.mma2_bar[wg_u]);
-        }
-      }
-      __syncwarp();
+    // (no bf16x3 split of msg, no second A store), as two N=64 halves.  msg goes straight to the staging tile (its
+    // Psrc rows are consumed), the coordinate-MLP half to the A region once both halves' MMAs are complete.
+    if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 10);
+    {
+      float d[32];
+      auto w23 = [&](int hn) {
+        return [&, hn](int sp, int kb) {
+          return b_desc_ex(w_saddr + TC_W23_BASE + sp * TC_W23_SPLIT + kb * 4096 + hn * 1024, 2048, 128); };
+      };
+      wg_gemm6<64>(d, a_desc, w23(0), 4, false);
+      wg_store_d<64>(W.stage + wgi * 64 * TC_LD, TC_LD, d, tid & 127);
+      wg_gemm6<64>(d, a_desc, w23(1), 4, false);
+      __syncthreads();   // both warpgroups' MMAs have read A
+      wg_store_d<64>(dtile + wgi * 64 * TC_LD, TC_LD, d, tid & 127);
     }
+    __syncthreads();
     // mean aggregation of msg at the destination nodes (:280-283): 4 threads per channel, each a run of nodes
     auto aggregate = [&](bool deg10) {
       const int c = q & 63, part = q >> 6;
@@ -417,49 +370,41 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
         }
       }
     };
-    if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 12);
-    mbar_wait(&S.mma_bar[wg], mma_phase);
-    mma_phase ^= 1;
-    tc_fence_after();
-    if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 13);
+    if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 13);
     {
       float v[32];
-      tmem_ld32f(d_col, v);                       // msg half row -> my own row of the (warp-private until now) tile
+      tile_ld32f(W.stage, TC_LD, r, half * 32, v);   // msg half row (+ bias below, in place)
 #pragma unroll
       for (int c = 0; c < 32; c += 2) {
-        const float2 t = __fadd2_rn(f2(v[c], v[c + 1]), f2(cst.b2[half * 32 + c], cst.b2[half * 32 + c + 1]));
+        const float2 t = add2(f2(v[c], v[c + 1]), f2(cst.b2[half * 32 + c], cst.b2[half * 32 + c + 1]));
         v[c] = t.x; v[c + 1] = t.y;
       }
       float4* ms = reinterpret_cast<float4*>(&W.stage[r * TC_LD + half * 32]);
 #pragma unroll
       for (int c4 = 0; c4 < 8; ++c4) ms[c4] = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
-      mbar_wait(&S.mma2_bar[wg], mma2_phase);
-      mma2_phase ^= 1;
-      if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 14);
-      tc_fence_after();
-      tmem_ld32f(d_col + 64, v);                  // coordinate-MLP hidden half row
+      if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 14);
+      tile_ld32f(dtile, TC_LD, r, half * 32, v);  // coordinate-MLP hidden half row
       float ph4[4] = {0.f, 0.f, 0.f, 0.f};        // 4 independent chains; the two halves are combined in fp64
       {
         float2 p01 = f2(0.f, 0.f), p23 = f2(0.f, 0.f);
         const float2 sl2 = f2(slope, slope);
 #pragma unroll
         for (int c = 0; c < 32; c += 4) {
-          float2 x01 = __fadd2_rn(f2(v[c], v[c + 1]), f2(cst.b3[half * 32 + c], cst.b3[half * 32 + c + 1]));
-          float2 x23 = __fadd2_rn(f2(v[c + 2], v[c + 3]), f2(cst.b3[half * 32 + c + 2], cst.b3[half * 32 + c + 3]));
-          float2 y01 = __fmul2_rn(x01, sl2), y23 = __fmul2_rn(x23, sl2);
-          p01 = __ffma2_rn(f2(fmaxf(x01.x, y01.x), fmaxf(x01.y, y01.y)), f2(cst.w4[half * 32 + c], cst.w4[half * 32 + c + 1]), p01);
-          p23 = __ffma2_rn(f2(fmaxf(x23.x, y23.x), fmaxf(x23.y, y23.y)), f2(cst.w4[half * 32 + c + 2], cst.w4[half * 32 + c + 3]), p23);
+          float2 x01 = add2(f2(v[c], v[c + 1]), f2(cst.b3[half * 32 + c], cst.b3[half * 32 + c + 1]));
+          float2 x23 = add2(f2(v[c + 2], v[c + 3]), f2(cst.b3[half * 32 + c + 2], cst.b3[half * 32 + c + 3]));
+          float2 y01 = mul2(x01, sl2), y23 = mul2(x23, sl2);
+          p01 = fma2(f2(fmaxf(x01.x, y01.x), fmaxf(x01.y, y01.y)), f2(cst.w4[half * 32 + c], cst.w4[half * 32 + c + 1]), p01);
+          p23 = fma2(f2(fmaxf(x23.x, y23.x), fmaxf(x23.y, y23.y)), f2(cst.w4[half * 32 + c + 2], cst.w4[half * 32 + c + 3]), p23);
         }
         ph4[0] = p01.x; ph4[1] = p01.y; ph4[2] = p23.x; ph4[3] = p23.y;
       }
       W.red[r * 2 + half] = ((double)ph4[0] + (double)ph4[1]) + ((double)ph4[2] + (double)ph4[3]);
     }
     cp_async_wait<0>();  // next tile's indices have landed (issued behind GEMM1)
-    tc_fence_before();
     // msg tile, phi halves, x_rel complete; next tile's indices visible.  The barrier also tells whether every node of the tile
     // has exactly 10 in-edges (the k-NN graphs of protein_utils.py:339-346): the tail then runs without row_ptr lookups.
-    const bool deg10 = wg_barrier_and(wg, q >= nn || W.rp[buf][q + 1] - W.rp[buf][q] == 10);
-    if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, tile, 15);
+    const bool deg10 = __syncthreads_and(q >= nn || W.rp[buf][q + 1] - W.rp[buf][q] == 10) != 0;
+    if (q == 0) TRACE_PHASE(0, blockIdx.x, tile, 15);
     // coordinate update :264, 274-277, 286-292 on the LAST threads of the group (warp 0 also issues the MMAs; the threads
     // 192..255 take no aggregation work below when all 3 nn outputs fit there)
     for (int o = 255 - q; o < nn * 3; o += 256) {
@@ -488,12 +433,10 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     aggregate(deg10);
     e0 = e0n; ne = nen; off_l = off_ln; n_l = n_ln; off_r = off_rn; buf ^= 1;
   }
-  if (q == 0) TRACE_PHASE(0, blockIdx.x * 2 + wg, 0xffff, 16);
+  if (q == 0) TRACE_PHASE(0, blockIdx.x, 0xffff, 16);
   cp_async_wait<0>();
-  tc_fence_before();
   __syncthreads();
   TRACE_END(0);
-  tmem_release(S.tmem_base, warp);
 }
 
 }  // namespace eqd
@@ -518,8 +461,7 @@ extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const fl
   memcpy(&cst, p_l->consts.edge, sizeof(cst));
   size_t smem = sizeof(eqd::TcSmem) + 128;
   EQD_SET_SMEM((eqd::edge_stage_tc_kernel), smem);
-  int grid = (ntiles + 1) / 2;
-  if (grid > 148) grid = 148;
+  int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   eqd::edge_stage_tc_kernel<<<grid, TC_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, cst, proj, x_in, x_orig, aggr, x_out,
                                                                              status, tn);
   EQD_CUDA_LAUNCH_CHECK();

@@ -98,7 +98,7 @@ extern "C" int eqd_project(const eqd_graph* g, const eqd_layer* p_l, const float
   if (g->n_nodes <= 0) return EQD_OK;
   int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
   size_t smem = (size_t)(EQD_TM * (p->dhp + 4) + 2 * EQD_WCHUNK * EQD_WLD) * sizeof(float);
-  int grid = ntiles < 148 * 4 ? ntiles : 148 * 4;
+  int grid = ntiles < EQD_SMS * 4 ? ntiles : EQD_SMS * 4;
   if (p->dhp == 72) {
     EQD_SET_SMEM((eqd::project_kernel<true>), smem);
     eqd::project_kernel<true><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, h, ldh, proj);

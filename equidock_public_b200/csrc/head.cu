@@ -403,7 +403,7 @@ extern "C" int eqd_keypoints(const eqd_graph* g, const eqd_head_params* hp, cons
   {
     size_t smem = (size_t)(EQD_TM * 68 + 2 * EQD_WCHUNK * EQD_WLD) * sizeof(float);
     EQD_SET_SMEM((eqd::head_mean_kernel), smem);
-    int grid = g->n_node_tiles < 148 * 2 ? g->n_node_tiles : 148 * 2;
+    int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
     eqd::head_mean_kernel<<<grid, EQD_THREADS, smem, st>>>(*g, *hp, h, part);
     EQD_CUDA_LAUNCH_CHECK();
   }

@@ -170,8 +170,6 @@ __device__ __forceinline__ void warp_argmin(double& v, int& k) {
 //     offset, so their contribution to the initial sink distances, base[k] = min_i (C_ik - u_i), changes only when the
 //     minimiser leaves the excess set.
 //   * All minima are lexicographic in (value, index): the plan does not depend on list or lane order.
-// (Round 2 first shipped the same algorithm with the sources expanded one by one inside warp 0: 39.5 ms for the `train` bench
-// batch, ~55 k cycles per augmentation in dependent shared-memory loads; see profiles/r02_ot_emd_*.)
 // The final flows are written to flow[(p0 + i) * 50 + k] (int32, global).
 __global__ void __launch_bounds__(LOSS_THREADS)
 ot_emd_kernel(int n_pairs, int cap, const int* __restrict__ pocket_ptr, const float* __restrict__ pocket_lig,

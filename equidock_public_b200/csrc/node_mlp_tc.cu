@@ -1,16 +1,19 @@
-// Node MLP of a 64-wide IEGMN layer (rigid_docking_model.py:319-337) on the tensor cores (tcgen05, bf16x6):
+// Node MLP of a 64-wide IEGMN layer (rigid_docking_model.py:319-337) on the tensor cores (wgmma, bf16x6):
 //   h' = skip( W6 . LayerNorm(LeakyReLU(W5 . [h | aggr_msg | mu | h0] + b5)) + b6 )
-// Weight-stationary (W5: 64x272, W6: 64x64 as bf16x3 UMMA panels, 126 KB in shared memory), two tile groups of
-// 256 threads (2 threads per node row) running out of phase.  The 272-wide input is fed in 5 K-pieces.
+// Weight-stationary (W5: 64x272, W6: 64x64 as bf16x3 panels, 126 KB in shared memory); one tile of 128 node rows per
+// CTA of 256 threads at a time (2 threads per node row, two 64-row warpgroup slabs in the GEMMs).  The 272-wide input
+// is fed in 5 K-pieces; the A operand region takes each piece's fp32 result tile once its MMAs are complete.
 #include "tc_common.cuh"
 
 namespace eqd {
 
-#define NM_THREADS 512
+#define NM_THREADS 256
 #define NM_W5_SPLIT 34816   // 64 x 272 bf16
 #define NM_W6_BASE 104448
 #define NM_W6_SPLIT 8192
 #define NM_W_BYTES 129024
+#define NM_A_SPLIT 16384    // A operand: 128 rows x 64 bf16 per split
+#define NM_LD 68            // fp32 row stride of the result tile
 
 struct NmConsts { float b5[64], ln_g[64], ln_b[64], b6[64]; };
 
@@ -18,10 +21,10 @@ struct NmConsts { float b5[64], ln_g[64], ln_b[64], b6[64]; };
 
 struct NmSmem {
   unsigned char w[NM_W_BYTES];
+  unsigned char a[3 * NM_A_SPLIT];
   float sc[NM_THREADS / 32][32 * NM_SC_LD];   // one 32-row x 128-byte scratch per warp (its rows x its column half)
-  float red[2][EQD_TM * 4];
-  unsigned long long w_bar, a_bar[2][2];
-  unsigned int tmem_base;
+  float red[EQD_TM * 4];
+  unsigned long long w_bar;
 };
 
 __global__ void __launch_bounds__(NM_THREADS, 1)
@@ -30,51 +33,36 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
                    float* __restrict__ h_out) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   NmSmem& S = *reinterpret_cast<NmSmem*>(smem_raw);
-  const int tid = threadIdx.x, wg = tid >> 8, q = tid & 255, half = q >> 7, r = q & 127, warp = tid >> 5;
+  const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, warp = tid >> 5, wgi = tid >> 7;
   const int ntiles = (n_nodes + EQD_TM - 1) / EQD_TM;
   TRACE_START(3);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b) mbar_init(&S.a_bar[a][b], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     mbar_expect_tx(&S.w_bar, NM_W_BYTES);
     bulk_g2s(S.w, p.w_node_tc, NM_W_BYTES, &S.w_bar);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int wg_u = warp_u >> 3;
-  const bool issuer_warp = (warp_u & 7) == 0;
-  const unsigned tmem_wg = __shfl_sync(0xffffffffu, S.tmem_base, 0) + (unsigned)wg_u * 256;
-  const unsigned tmem = tmem_wg + ((unsigned)((warp & 3) * 32) << 16);
-  // columns: D 0..63, A 64..159
-  const unsigned w_saddr = smem_u32(S.w);
+  const unsigned w_saddr = smem_u32(S.w), a_saddr = smem_u32(S.a);
+  float* const dtile = reinterpret_cast<float*>(S.a);
+  auto a_desc = [&](int sp, int kb) { return a_desc_at<EQD_TM>(a_saddr, NM_A_SPLIT, wgi, sp, kb); };
   mbar_wait(&S.w_bar, 0);
-  unsigned ph[2] = {0, 0};
   const float slope = p.leaky_slope;
-  float* red = S.red[wg];
+  float* red = S.red;
 
-  // MMAs of K-blocks [kb0, kb0+nkb) of W5 (or all of W6) reading A buffer `ab`, then arrive on a_bar[ab]
-  auto issue = [&](int ab, unsigned w_off, unsigned w_split, int nkb, unsigned accum0) {
-    if (issuer_warp) {
-      tc_fence_after();
-      if (elect_one()) {
-        issue_gemm(tmem_wg, tmem_wg + 64 + ab * 96, 32, w_saddr + w_off, w_split, nkb, accum0);
-        umma_commit(&S.a_bar[wg_u][ab]);
-      }
-      __syncwarp();
+  // The A operand in place (callers fence + barrier first) times K-blocks [0, nkb) of the panel at w_off -> out (my row
+  // half of the fresh product); on return the A region is free again.
+  auto gemm = [&](unsigned w_off, unsigned w_split, int nkb, float (&out)[32]) {
+    {
+      float d[32];
+      wg_gemm6<64>(d, a_desc, [&](int sp, int kb) { return b_desc_ex(w_saddr + w_off + sp * w_split + kb * 2048, 1024, 128); },
+                   nkb, false);
+      __syncthreads();
+      wg_store_d<64>(dtile + wgi * 64 * NM_LD, NM_LD, d, tid & 127);
     }
-  };
-  auto wait_a = [&](int ab) {
-    mbar_wait(&S.a_bar[wg][ab], ph[ab]);
-    ph[ab] ^= 1;
-    tc_fence_after();
+    __syncthreads();
+    tile_ld32f(dtile, NM_LD, r, half * 32, out);
+    __syncthreads();
   };
 
   // Global rows travel coalesced: the warp's 32 rows x 128 bytes (its column half) are cp.async'ed into its scratch,
@@ -102,78 +90,51 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
     }
     __syncwarp();
   };
-  fetch(h_in, EQD_HID, blockIdx.x * 2 + wg);
-  for (int tile = blockIdx.x * 2 + wg; tile < ntiles; tile += gridDim.x * 2) {
-    if (q == 0) TRACE_PHASE(3, blockIdx.x * 2 + wg, tile, 1);
+  fetch(h_in, EQD_HID, blockIdx.x);
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    if (q == 0) TRACE_PHASE(3, blockIdx.x, tile, 1);
     const int node = tile * EQD_TM + r;
     const bool valid = node < n_nodes;
     // ---- node_mlp.0 over [h | aggr | mu | h0] in 5 K-pieces ---------------------------------------------------
-    // The tensor core truncates (round-toward-zero) on every add into an fp32 accumulator: a bias that grows with
-    // the number of accumulation steps.  Each 64-wide piece is therefore its own accumulation (4 full-magnitude
-    // steps, like the edge-stage GEMMs) and the pieces are summed in registers with round-to-nearest FADDs.
+    // Each 64-wide piece is its own accumulation (4 full-magnitude steps, like the edge-stage GEMMs) and the pieces
+    // are summed in registers with round-to-nearest FADDs.
     float acc[32];
 #pragma unroll
     for (int c = 0; c < 32; ++c) acc[c] = cst.b5[half * 32 + c];
     {
-      float v[32];
-      take(v);
-      fetch(aggr, EQD_HID, tile);
-      store_half_split3(tmem + 64 + half * 16, v);         // piece 0 (h) -> A
-    }
-    tc_fence_before();
-    wg_barrier(wg);
-    issue(0, 0, NM_W5_SPLIT, 4, 0);
-    {
       float v[32], d[32];
-      auto drain = [&]() {                                  // D of the finished piece -> acc
-        wait_a(0);
-        tmem_ld32f(tmem + half * 32, d);
+      auto piece = [&](unsigned w_off, int nkb) {
+        tc_fence_before();
+        __syncthreads();
+        gemm(w_off, NM_W5_SPLIT, nkb, d);
 #pragma unroll
         for (int c = 0; c < 32; ++c) acc[c] += d[c];
       };
       take(v);
+      fetch(aggr, EQD_HID, tile);
+      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 0 (h) -> A
+      piece(0, 4);
+      take(v);
       fetch(mu, EQD_HID, tile);
-      drain();
-      store_half_split3(tmem + 64 + half * 16, v);         // piece 1 (aggr)
-      tc_fence_before();
-      wg_barrier(wg);
-      issue(0, 4 * 2048, NM_W5_SPLIT, 4, 0);
+      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 1 (aggr)
+      piece(4 * 2048, 4);
       take(v);
       fetch(h0, EQD_H0_PAD, tile);
-      drain();
-      store_half_split3(tmem + 64 + half * 16, v);         // piece 2 (mu)
-      tc_fence_before();
-      wg_barrier(wg);
-      issue(0, 8 * 2048, NM_W5_SPLIT, 4, 0);
+      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 2 (mu)
+      piece(8 * 2048, 4);
       take(v);
-      drain();
-      store_half_split3(tmem + 64 + half * 16, v);         // piece 3 (h0[0:64])
-      tc_fence_before();
-      wg_barrier(wg);
-      issue(0, 12 * 2048, NM_W5_SPLIT, 4, 0);
-      drain();
-      // piece 4: h0[64:72] + 8 zero columns (K = 16): the half-0 threads write 8 columns per split
+      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 3 (h0[0:64])
+      piece(12 * 2048, 4);
+      // piece 4: h0[64:72] + 8 zero columns (K = 16): the half-0 threads write the k-block
       if (half == 0) {
-        float t[16];
         const float4* sp = reinterpret_cast<const float4*>(h0 + (long)node * EQD_H0_PAD + 64);
         float4 a = valid ? sp[0] : make_float4(0.f, 0.f, 0.f, 0.f), b = valid ? sp[1] : make_float4(0.f, 0.f, 0.f, 0.f);
-        t[0] = a.x; t[1] = a.y; t[2] = a.z; t[3] = a.w; t[4] = b.x; t[5] = b.y; t[6] = b.z; t[7] = b.w;
-#pragma unroll
-        for (int c = 8; c < 16; ++c) t[c] = 0.f;
-        unsigned p0[8], p1[8], p2[8];
-#pragma unroll
-        for (int c = 0; c < 8; ++c) split3_pair(t[2 * c], t[2 * c + 1], p0[c], p1[c], p2[c]);
-        tmem_st8(tmem + 64, p0);
-        tmem_st8(tmem + 64 + 32, p1);
-        tmem_st8(tmem + 64 + 64, p2);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+        float t[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+        store_extra8_split3<EQD_TM>(S.a, NM_A_SPLIT, r, 0, t);
       }
-      tc_fence_before();
-      wg_barrier(wg);
-      issue(0, 16 * 2048, NM_W5_SPLIT, 1, 0);
-      drain();
+      piece(16 * 2048, 1);
     }
-    // ---- + bias, LeakyReLU, LayerNorm -> bf16x3 -> A1 ; node_mlp.4 ---------------------------------------------
+    // ---- + bias, LeakyReLU, LayerNorm -> bf16x3 -> A ; node_mlp.4 ---------------------------------------------
     {
       float v[32];
       float s4[4] = {0.f, 0.f, 0.f, 0.f};
@@ -191,8 +152,7 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
       }
       red[(r * 2 + half) * 2 + 0] = mh;
       red[(r * 2 + half) * 2 + 1] = (q4[0] + q4[1]) + (q4[2] + q4[3]);
-      tc_fence_before();
-      wg_barrier(wg);
+      __syncthreads();
       const float m0 = red[r * 4 + 0], m1 = red[r * 4 + 2];
       const float mean = 0.5f * (m0 + m1);
       const float dm = m0 - m1;
@@ -200,17 +160,15 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
       const float rstd = 1.f / sqrtf(var + 1e-5f);
 #pragma unroll
       for (int c = 0; c < 32; ++c) v[c] = (v[c] - mean) * rstd * cst.ln_g[half * 32 + c] + cst.ln_b[half * 32 + c];
-      store_half_split3(tmem + 64 + half * 16, v);
+      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);
     }
-    tc_fence_before();
-    wg_barrier(wg);
-    issue(0, NM_W6_BASE, NM_W6_SPLIT, 4, 0);
     fetch(h_in, EQD_HID, tile);   // the skip operand again (an L2 hit) rather than 32 registers held across the tile
-    wait_a(0);
+    tc_fence_before();
+    __syncthreads();
     {
       float v[32], hskip[32];
+      gemm(NM_W6_BASE, NM_W6_SPLIT, 4, v);
       take(hskip);
-      tmem_ld32f(tmem + half * 32, v);
       const float sk = p.skip_weight_h, sk1 = 1.f - p.skip_weight_h;
 #pragma unroll
       for (int c = 0; c < 32; ++c) v[c] = sk * (v[c] + cst.b6[half * 32 + c]) + sk1 * hskip[c];  // :332-334
@@ -228,14 +186,9 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
       }
       __syncwarp();
     }
-    fetch(h_in, EQD_HID, tile + gridDim.x * 2);   // next tile's h rows, behind the end-of-tile barrier
-    tc_fence_before();
-    wg_barrier(wg);  // D and both A buffers are free for the next tile
+    fetch(h_in, EQD_HID, tile + gridDim.x);   // next tile's h rows
   }
-  tc_fence_before();
-  __syncthreads();
   TRACE_END(3);
-  tmem_release(S.tmem_base, warp);
 }
 
 
@@ -247,15 +200,16 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
 #define NM0_W6_BASE 107520
 #define NM0_W6_SPLIT 10240    // 64 x 80 bf16
 #define NM0_W_BYTES 138240
+#define NM0_A_SPLIT 20480     // A operand: 128 rows x 80 bf16 per split
+#define NM0_LD 84             // fp32 row stride of the result tile
 
 struct Nm0Consts { float b5[80], ln_g[80], ln_b[80], b6[64]; };
 
 struct Nm0Smem {
   unsigned char w[NM0_W_BYTES];
-  float sc[NM_THREADS / 32][32 * NM_SC_LD];
-  float red[2][EQD_TM * 4];
-  unsigned long long w_bar, a_bar[2];
-  unsigned int tmem_base;
+  unsigned char a[3 * NM0_A_SPLIT];
+  float red[EQD_TM * 4];
+  unsigned long long w_bar;
 };
 
 __global__ void __launch_bounds__(NM_THREADS, 1)
@@ -263,87 +217,42 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
                     const float* __restrict__ aggr, const float* __restrict__ mu /*[n][72]*/, float* __restrict__ h_out) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Nm0Smem& S = *reinterpret_cast<Nm0Smem*>(smem_raw);
-  const int tid = threadIdx.x, wg = tid >> 8, q = tid & 255, half = q >> 7, r = q & 127, warp = tid >> 5;
+  const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, wgi = tid >> 7;
   const int ntiles = (n_nodes + EQD_TM - 1) / EQD_TM;
   TRACE_START(3);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
-    mbar_init(&S.a_bar[0], 1);
-    mbar_init(&S.a_bar[1], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     mbar_expect_tx(&S.w_bar, NM0_W_BYTES);
     bulk_g2s(S.w, p.w_node_tc, NM0_W_BYTES, &S.w_bar);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int wg_u = warp_u >> 3;
-  const bool issuer_warp = (warp_u & 7) == 0;
-  const unsigned tmem_wg = __shfl_sync(0xffffffffu, S.tmem_base, 0) + (unsigned)wg_u * 256;
-  const unsigned tmem = tmem_wg + ((unsigned)((warp & 3) * 32) << 16);
-  // columns: D 0..79, A 80..199 (3 splits x 40: 32 main + 8 extra)
-  const unsigned a_col = tmem + 80;
-  const unsigned w_saddr = smem_u32(S.w);
+  const unsigned w_saddr = smem_u32(S.w), a_saddr = smem_u32(S.a);
+  float* const dtile = reinterpret_cast<float*>(S.a);
+  auto a_desc = [&](int sp, int kb) { return a_desc_at<EQD_TM>(a_saddr, NM0_A_SPLIT, wgi, sp, kb); };
   mbar_wait(&S.w_bar, 0);
-  unsigned ph = 0;
   const float slope = p.leaky_slope;
-  float* red = S.red[wg];
+  float* red = S.red;
 
-  auto issue_w5 = [&](int kb0, int nkb) {   // k-blocks [kb0, kb0 + nkb) of W5' against the A operand, fresh accumulator
-    if (issuer_warp) {
-      tc_fence_after();
-      if (elect_one()) {
-        issue_gemm_n<80>(tmem_wg, tmem_wg + 80, 40, w_saddr + kb0 * (80 * 32), NM0_W5_SPLIT, nkb);
-        umma_commit(&S.a_bar[wg_u]);
-      }
-      __syncwarp();
-    }
-  };
-  auto wait_a = [&]() {
-    mbar_wait(&S.a_bar[wg], ph);
-    ph ^= 1;
-    tc_fence_after();
-  };
-  const int lane = tid & 31, wrow0 = 32 * (warp & 3);
-  float* sc = S.sc[warp];
-  auto fetch = [&](const float* base, int ld, int t) {
-    if (t >= ntiles) return;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int row = i * 4 + (lane >> 3);
-      const long nd = (long)t * EQD_TM + wrow0 + row;
-      const bool ok = nd < n_nodes;   // src-size 0 zero-fills
-      cp_async16(sc + row * NM_SC_LD + (lane & 7) * 4, base + (ok ? nd : 0) * ld + half * 32 + (lane & 7) * 4, ok);
-    }
-    cp_async_commit();
-  };
-  auto take = [&](float (&v)[32]) {
-    cp_async_wait<0>();
-    __syncwarp();
-#pragma unroll
-    for (int c4 = 0; c4 < 8; ++c4) {
-      float4 t = *reinterpret_cast<const float4*>(sc + lane * NM_SC_LD + c4 * 4);
-      v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
-    }
-    __syncwarp();
-  };
-  fetch(h0, EQD_H0_PAD, blockIdx.x * 2 + wg);
-  for (int tile = blockIdx.x * 2 + wg; tile < ntiles; tile += gridDim.x * 2) {
-    if (q == 0) TRACE_PHASE(3, blockIdx.x * 2 + wg, tile, 1);
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    if (q == 0) TRACE_PHASE(3, blockIdx.x, tile, 1);
     const int node = tile * EQD_TM + r;
     const bool valid = node < n_nodes;
+    auto row32 = [&](const float* base, int ld, float (&v)[32]) {   // my half row of a [n][ld] array
+      const float4* sp = reinterpret_cast<const float4*>(base + (long)node * ld + half * 32);
+#pragma unroll
+      for (int c4 = 0; c4 < 8; ++c4) {
+        float4 t = valid ? sp[c4] : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
+      }
+    };
     // channels [64, 72) of an 72-strided row (zero beyond 69) as the piece's fifth k-block; half-0 threads only
     auto extra8 = [&](const float* base) {
       if (half == 0) {
         const float4* ep = reinterpret_cast<const float4*>(base + (long)node * EQD_H0_PAD + 64);
         float4 a = valid ? ep[0] : make_float4(0.f, 0.f, 0.f, 0.f), b = valid ? ep[1] : make_float4(0.f, 0.f, 0.f, 0.f);
         float t[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        store_extra8_split3(a_col + 32, t, 40);
+        store_extra8_split3<EQD_TM>(S.a, NM0_A_SPLIT, r, 64, t);
       }
     };
     float acc[32], accx[16];   // accx: columns 64..79 (half 0)
@@ -351,43 +260,41 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
     for (int c = 0; c < 32; ++c) acc[c] = cst.b5[half * 32 + c];
 #pragma unroll
     for (int c = 0; c < 16; ++c) accx[c] = cst.b5[64 + c];
-    auto drain = [&]() {   // each piece is its own accumulation (<= 5 full-magnitude steps), summed here with RN adds
-      wait_a();
-      float d[32];
-      tmem_ld32f(tmem + half * 32, d);
-#pragma unroll
-      for (int c = 0; c < 32; ++c) acc[c] += d[c];
-      if (half == 0) {
-        float e[16];
-        tmem_ld16f(tmem + 64, e);
-#pragma unroll
-        for (int c = 0; c < 16; ++c) accx[c] += e[c];
+    // k-blocks [kb0, kb0 + nkb) of W5' against the A operand, a fresh accumulation summed here with RN adds (<= 5
+    // full-magnitude steps each); on return the A region is free again
+    auto piece = [&](int kb0, int nkb) {
+      tc_fence_before();
+      __syncthreads();
+      {
+        float d[40];
+        wg_gemm6<80>(d, a_desc, [&](int sp, int kb) {
+          return b_desc_ex(w_saddr + (kb0 + kb) * (80 * 32) + sp * NM0_W5_SPLIT, 80 * 16, 128); }, nkb, false);
+        __syncthreads();
+        wg_store_d<80>(dtile + wgi * 64 * NM0_LD, NM0_LD, d, tid & 127);
       }
+      __syncthreads();
+      const float* dr = dtile + r * NM0_LD;
+#pragma unroll
+      for (int c = 0; c < 32; ++c) acc[c] += dr[half * 32 + c];
+      if (half == 0) {
+#pragma unroll
+        for (int c = 0; c < 16; ++c) accx[c] += dr[64 + c];
+      }
+      __syncthreads();
     };
     {
       float v[32];
-      take(v);
-      fetch(aggr, EQD_HID, tile);
-      store_half_split3(a_col + half * 16, v, 40);      // piece 0: h0 (80)
+      row32(h0, EQD_H0_PAD, v);
+      store_half_split3<EQD_TM>(S.a, NM0_A_SPLIT, r, half * 32, v);   // piece 0: h0 (80)
       extra8(h0);
-      tc_fence_before();
-      wg_barrier(wg);
-      issue_w5(0, 5);
-      take(v);
-      fetch(mu, EQD_H0_PAD, tile);
-      drain();
-      store_half_split3(a_col + half * 16, v, 40);      // piece 1: aggr (64)
-      tc_fence_before();
-      wg_barrier(wg);
-      issue_w5(5, 4);
-      take(v);
-      drain();
-      store_half_split3(a_col + half * 16, v, 40);      // piece 2: mu (80)
+      piece(0, 5);
+      row32(aggr, EQD_HID, v);
+      store_half_split3<EQD_TM>(S.a, NM0_A_SPLIT, r, half * 32, v);   // piece 1: aggr (64)
+      piece(5, 4);
+      row32(mu, EQD_H0_PAD, v);
+      store_half_split3<EQD_TM>(S.a, NM0_A_SPLIT, r, half * 32, v);   // piece 2: mu (80)
       extra8(mu);
-      tc_fence_before();
-      wg_barrier(wg);
-      issue_w5(9, 5);
-      drain();
+      piece(9, 5);
     }
     // ---- LeakyReLU, LayerNorm over the 69 real channels -> bf16x3 -> A ; node_mlp.4 ---------------------------------
     {
@@ -421,8 +328,7 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
       }
       red[(r * 2 + half) * 2 + 0] = mh;
       red[(r * 2 + half) * 2 + 1] = m2;
-      tc_fence_before();
-      wg_barrier(wg);
+      __syncthreads();
       const float m0 = red[r * 4 + 0], m1 = red[r * 4 + 2];
       const float mean = (37.f * m0 + 32.f * m1) * (1.f / 69.f);
       const float dm = m0 - m1;
@@ -430,52 +336,39 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
       const float rstd = 1.f / sqrtf(var + 1e-5f);
 #pragma unroll
       for (int c = 0; c < 32; ++c) acc[c] = (acc[c] - mean) * rstd * cst.ln_g[half * 32 + c] + cst.ln_b[half * 32 + c];
-      store_half_split3(a_col + half * 16, acc, 40);
+      store_half_split3<EQD_TM>(S.a, NM0_A_SPLIT, r, half * 32, acc);
       if (half == 0) {
         float t[8];
 #pragma unroll
         for (int c = 0; c < 5; ++c) t[c] = (accx[c] - mean) * rstd * cst.ln_g[64 + c] + cst.ln_b[64 + c];
         t[5] = t[6] = t[7] = 0.f;
-        store_extra8_split3(a_col + 32, t, 40);
+        store_extra8_split3<EQD_TM>(S.a, NM0_A_SPLIT, r, 64, t);
       }
     }
     tc_fence_before();
-    wg_barrier(wg);
-    if (issuer_warp) {
-      tc_fence_after();
-      if (elect_one()) {
-        issue_gemm_n<64>(tmem_wg, tmem_wg + 80, 40, w_saddr + NM0_W6_BASE, NM0_W6_SPLIT, 5);
-        umma_commit(&S.a_bar[wg_u]);
-      }
-      __syncwarp();
+    __syncthreads();
+    {
+      float d[32];
+      wg_gemm6<64>(d, a_desc, [&](int sp, int kb) {
+        return b_desc_ex(w_saddr + NM0_W6_BASE + sp * NM0_W6_SPLIT + kb * 2048, 1024, 128); }, 5, false);
+      __syncthreads();
+      wg_store_d<64>(dtile + wgi * 64 * NM0_LD, NM0_LD, d, tid & 127);
     }
-    wait_a();
+    __syncthreads();
     {
       float v[32];
-      tmem_ld32f(tmem + half * 32, v);
+      tile_ld32f(dtile, NM0_LD, r, half * 32, v);
 #pragma unroll
       for (int c = 0; c < 32; ++c) v[c] += cst.b6[half * 32 + c];
+      if (valid) {
+        float4* o = reinterpret_cast<float4*>(h_out + (long)node * EQD_HID + half * 32);
 #pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4)
-        *reinterpret_cast<float4*>(sc + lane * NM_SC_LD + c4 * 4) = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
-      __syncwarp();
-      float* o = h_out + ((long)tile * EQD_TM + wrow0) * EQD_HID + half * 32 + (lane & 7) * 4;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int row = i * 4 + (lane >> 3);
-        float4 t = *reinterpret_cast<const float4*>(sc + row * NM_SC_LD + (lane & 7) * 4);
-        if ((long)tile * EQD_TM + wrow0 + row < n_nodes) *reinterpret_cast<float4*>(o + (long)row * EQD_HID) = t;
+        for (int c4 = 0; c4 < 8; ++c4) o[c4] = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
       }
-      __syncwarp();
     }
-    fetch(h0, EQD_H0_PAD, tile + gridDim.x * 2);
-    tc_fence_before();
-    wg_barrier(wg);
+    __syncthreads();   // the result tile has been read: the region takes the next tile's A operand
   }
-  tc_fence_before();
-  __syncthreads();
   TRACE_END(3);
-  tmem_release(S.tmem_base, warp);
 }
 
 }  // namespace eqd
@@ -495,8 +388,7 @@ extern "C" int eqd_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const f
   int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
   size_t smem = sizeof(eqd::NmSmem) + 128;
   EQD_SET_SMEM((eqd::node_mlp_tc_kernel), smem);
-  int grid = (ntiles + 1) / 2;
-  if (grid > 148) grid = 148;
+  int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   eqd::node_mlp_tc_kernel<<<grid, NM_THREADS, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h_in, aggr, mu, h0, h_out);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
@@ -515,8 +407,7 @@ extern "C" int eqd_node_mlp_tc0(const eqd_graph* g, const eqd_layer* p_l, const 
   int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
   size_t smem = sizeof(eqd::Nm0Smem) + 128;
   EQD_SET_SMEM((eqd::node_mlp0_tc_kernel), smem);
-  int grid = (ntiles + 1) / 2;
-  if (grid > 148) grid = 148;
+  int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   eqd::node_mlp0_tc_kernel<<<grid, NM_THREADS, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h0, aggr, mu, h_out);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;

@@ -194,13 +194,13 @@ extern "C" int eqd_node_stage(const eqd_graph* g, const eqd_layer* p_l, const eq
   if (extra) {
     size_t smem = eqd::NodeCfg<true>::SMEM;
     EQD_SET_SMEM((eqd::node_stage_kernel<true>), smem);
-    int grid = g->n_node_tiles < 148 * 2 ? g->n_node_tiles : 148 * 2;
+    int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
     eqd::node_stage_kernel<true><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr,
                                                                   h_out, proj_next);
   } else {
     size_t smem = eqd::NodeCfg<false>::SMEM;
     EQD_SET_SMEM((eqd::node_stage_kernel<false>), smem);
-    int grid = g->n_node_tiles < 148 * 2 ? g->n_node_tiles : 148 * 2;
+    int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
     eqd::node_stage_kernel<false><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr,
                                                                    h_out, proj_next);
   }

@@ -1,28 +1,30 @@
-// Node projections of a layer on the tensor cores (tcgen05, bf16x6; att_mlp_Q/K/V :130-140 and the [h_src|h_dst]
+// Node projections of a layer on the tensor cores (wgmma, bf16x6; att_mlp_Q/K/V :130-140 and the [h_src|h_dst]
 // columns of edge_mlp.0 :120, applied per node):
 //   proj[n] = [Psrc | Pdst | Q | K | V] = act(h[n] . Wp + b)      (groups of 64 columns, see eqd_layer_params)
 // plus, for the tensor-core attention of the same layer, K and V of every node as bf16x3 in 8-node blocks
-//   kv[which][split][n/8][d/8][n%8][d%8]   (1 KB per 8 nodes; a run of blocks is a ready UMMA B operand).
+//   kv[which][split][n/8][d/8][n%8][d%8]   (1 KB per 8 nodes; a run of blocks is a ready wgmma B operand).
 // Weight-stationary: the bf16x3 panels (120 KB; 158 KB for the K = 80 layer 0) sit in shared memory for the life of
-// the CTA; two tile groups of 256 threads (2 threads per node row) ping-pong two TMEM accumulators.
+// the CTA next to the tile's A operand and its fp32 result tile; 2 threads per node row, one 64-row warpgroup slab per
+// 128 threads (layer 0 takes 64-row tiles: its larger panels leave room for no more).
 #include "tc_common.cuh"
 
 namespace eqd {
 
-#define PJ_THREADS 512
-#define PJ_SC_LD 36   // padded row stride (floats) of a warp's 32 x 32 transposition scratch: conflict-free both ways
+#define PJ_LD 68   // fp32 row stride of the result tile
 
 // Two instances: the 64-wide layers (K = 64, 5 groups) and the 69-wide layer 0 (h = h0, K = 69 padded to 80 = 5 k-blocks;
 // the first 64 channels of Q / K / V go where the 64-wide layers put theirs, channels 64..68 of all three form a sixth
 // N = 16 group written to x5[n][16] = [K64..67 | V64..67 | K68 V68 | Q64..68 | 0], the layout the layer-0 attention reads).
 template <bool L0>
 struct PjCfg {
+  static constexpr int R = L0 ? 64 : 128;                 // rows per tile
+  static constexpr int THREADS = 2 * R;
   static constexpr int KB = L0 ? 5 : 4;                   // k-blocks of 16
-  static constexpr int ASC = L0 ? 40 : 32;                // TMEM columns per A split
   static constexpr int GROUP_BYTES = 64 * KB * 16 * 2 * 3;  // one N = 64 group: 3 splits
   static constexpr int SPLIT_BYTES = 64 * KB * 16 * 2;
   static constexpr int X_SPLIT_BYTES = 16 * KB * 16 * 2;
   static constexpr int W_BYTES = 5 * GROUP_BYTES + (L0 ? 3 * X_SPLIT_BYTES : 0);
+  static constexpr int A_SPLIT_BYTES = R * KB * 32;
   static constexpr int NGROUPS = L0 ? 6 : 5;
 };
 
@@ -31,10 +33,9 @@ struct PjConsts { float b[336]; };
 template <bool L0>
 struct PjSmem {
   unsigned char w[PjCfg<L0>::W_BYTES];
-  // one 32-row x 128-byte scratch per warp (its rows x its column half); layer 0 has no room for it next to its K = 80 panels
-  float sc[L0 ? 1 : PJ_THREADS / 32][32 * PJ_SC_LD];
-  unsigned long long w_bar, d_bar[2][2];
-  unsigned int tmem_base;
+  unsigned char a[3 * PjCfg<L0>::A_SPLIT_BYTES];
+  float d[PjCfg<L0>::R * PJ_LD];
+  unsigned long long w_bar;
 };
 
 // bf16x3 block-layout store of 32 consecutive channels [half*32, +32) of node `node`
@@ -53,126 +54,68 @@ __device__ __forceinline__ void store_kv_blocks(unsigned char* __restrict__ kv, 
 }
 
 template <bool L0>
-__global__ void __launch_bounds__(PJ_THREADS, 1)
+__global__ void __launch_bounds__(PjCfg<L0>::THREADS, 1)
 project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjConsts cst, const float* __restrict__ h, int ldh,
                   float* __restrict__ proj, int pw, unsigned char* __restrict__ kv, long kv_split_stride, float* __restrict__ x5) {
   using C = PjCfg<L0>;
+  constexpr int R = C::R;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   PjSmem<L0>& S = *reinterpret_cast<PjSmem<L0>*>(smem_raw);
-  const int tid = threadIdx.x, wg = tid >> 8, q = tid & 255, half = q >> 7, r = q & 127, warp = tid >> 5;
-  const int ntiles = (n_nodes + EQD_TM - 1) / EQD_TM;
+  const int tid = threadIdx.x, half = tid / R, r = tid % R, warp = tid >> 5, wgi = tid >> 7;
+  const int ntiles = (n_nodes + R - 1) / R;
   TRACE_START(2);
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&S.tmem_base)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
-    for (int a = 0; a < 2; ++a)
-      for (int b = 0; b < 2; ++b) mbar_init(&S.d_bar[a][b], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     mbar_expect_tx(&S.w_bar, C::W_BYTES);
     bulk_g2s(S.w, p.w_proj_tc, C::W_BYTES, &S.w_bar);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const int warp_u = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int wg_u = warp_u >> 3;
-  const bool issuer_warp = (warp_u & 7) == 0;
-  const unsigned tmem_wg = __shfl_sync(0xffffffffu, S.tmem_base, 0) + (unsigned)wg_u * 256;
-  const unsigned tmem = tmem_wg + ((unsigned)((warp & 3) * 32) << 16);
-  const unsigned a_col = tmem + 128;  // D0: 0..63, D1: 64..127, A: 128.. (3 splits x ASC columns)
-  const unsigned w_saddr = smem_u32(S.w);
+  const unsigned w_saddr = smem_u32(S.w), a_saddr = smem_u32(S.a);
+  auto a_desc = [&](int s, int kb) { return a_desc_at<R>(a_saddr, C::A_SPLIT_BYTES, wgi, s, kb); };
+  float* dslab = S.d + wgi * 64 * PJ_LD;   // this warpgroup's 64 result rows
   mbar_wait(&S.w_bar, 0);
-  unsigned ph[2] = {0, 0};
   const float slope = p.leaky_slope;
+  const int lane = tid & 31, wrow0 = (warp * 32) % R;   // the warp's 32 rows (of its column half)
 
-  auto issue = [&](int grp) {  // the 6 KB MMAs of projection group `grp` into D[grp & 1]
-    if (issuer_warp) {
-      tc_fence_after();
-      if (elect_one()) {
-        if (L0 && grp == 5)
-          issue_gemm_n<16>(tmem_wg + 64, tmem_wg + 128, C::ASC, w_saddr + 5 * C::GROUP_BYTES, C::X_SPLIT_BYTES, C::KB);
-        else
-          issue_gemm_n<64>(tmem_wg + (grp & 1) * 64, tmem_wg + 128, C::ASC, w_saddr + grp * C::GROUP_BYTES, C::SPLIT_BYTES, C::KB);
-        umma_commit(&S.d_bar[wg_u][grp & 1]);
-      }
-      __syncwarp();
-    }
-  };
-
-  const int lane = tid & 31, wrow0 = 32 * (warp & 3);
-  float* sc = S.sc[L0 ? 0 : warp];
-  // coalesced cp.async of this warp's 32 rows x [half*32, +32) of tile t into its scratch (zeros past the end)
-  auto load_rows = [&](int t) {
-    if constexpr (!L0) {
-      if (t >= ntiles) return;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int row = i * 4 + (lane >> 3);
-        const long nd = (long)t * EQD_TM + wrow0 + row;
-        float* dst = sc + row * PJ_SC_LD + (lane & 7) * 4;
-        const bool ok = nd < n_nodes;   // src-size 0 zero-fills
-        cp_async16(dst, h + (ok ? nd : 0) * ldh + half * 32 + (lane & 7) * 4, ok);
-      }
-      cp_async_commit();
-    }
-  };
-  load_rows(blockIdx.x * 2 + wg);
-  for (int tile = blockIdx.x * 2 + wg; tile < ntiles; tile += gridDim.x * 2) {
-    if (q == 0) TRACE_PHASE(2, blockIdx.x * 2 + wg, tile, 1);
-    const int node0 = tile * EQD_TM;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    if (tid == 0) TRACE_PHASE(2, blockIdx.x, tile, 1);
+    const int node0 = tile * R;
     const int node = node0 + r;
     const bool valid = node < n_nodes;
     {
       float v[32];
-      if (L0) {   // strided row loads (no scratch) + the 69 - 64 extra channels (h0 is zero-padded to 72) as a fifth k-block
-        const float4* hp = reinterpret_cast<const float4*>(h + (long)node * ldh + half * 32);
+      const float4* hp = reinterpret_cast<const float4*>(h + (long)node * ldh + half * 32);
 #pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          float4 t = valid ? hp[c4] : make_float4(0.f, 0.f, 0.f, 0.f);
-          v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
-        }
-        if (half == 0) {
-          const float4* ep = reinterpret_cast<const float4*>(h + (long)node * ldh + 64);
-          float4 a = valid ? ep[0] : make_float4(0.f, 0.f, 0.f, 0.f), b = valid ? ep[1] : make_float4(0.f, 0.f, 0.f, 0.f);
-          float t[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-          store_extra8_split3(a_col + 32, t, C::ASC);
-        }
-      } else {
-        // the warp's 32 rows x 128 bytes arrive coalesced (8 lanes per row) in its scratch; each thread then reads its row
-        cp_async_wait<0>();
-        __syncwarp();
-#pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          float4 t = *reinterpret_cast<const float4*>(sc + lane * PJ_SC_LD + c4 * 4);
-          v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
-        }
-        __syncwarp();
+      for (int c4 = 0; c4 < 8; ++c4) {
+        float4 t = valid ? hp[c4] : make_float4(0.f, 0.f, 0.f, 0.f);
+        v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
       }
-      store_half_split3(a_col + half * 16, v, C::ASC);
+      if (L0 && half == 0) {   // the 69 - 64 extra channels (h0 is zero-padded to 72) as a fifth k-block
+        const float4* ep = reinterpret_cast<const float4*>(h + (long)node * ldh + 64);
+        float4 a = valid ? ep[0] : make_float4(0.f, 0.f, 0.f, 0.f), b = valid ? ep[1] : make_float4(0.f, 0.f, 0.f, 0.f);
+        float t[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+        store_extra8_split3<R>(S.a, C::A_SPLIT_BYTES, r, 64, t);
+      }
+      store_half_split3<R>(S.a, C::A_SPLIT_BYTES, r, half * 32, v);
     }
     tc_fence_before();
-    wg_barrier(wg);
-    issue(0);
-    issue(1);
+    __syncthreads();
 #pragma unroll 1
     for (int grp = 0; grp < C::NGROUPS; ++grp) {
-      const int d = grp & 1;
-      mbar_wait(&S.d_bar[wg][d], ph[d]);
-      ph[d] ^= 1;
-      tc_fence_after();
       if (L0 && grp == 5) {   // channels 64..68 of K, V, Q -> x5 (half-0 threads own the 16 columns)
-        float e[16];
-        if (half == 0) tmem_ld16f(tmem + 64, e);
-        tc_fence_before();
-        wg_barrier(wg);
+        float d[8];
+        wg_gemm6<16>(d, a_desc, [&](int s, int kb) {
+          return b_desc_ex(w_saddr + 5 * C::GROUP_BYTES + s * C::X_SPLIT_BYTES + kb * 512, 256, 128); }, C::KB, false);
+        wg_store_d<16>(dslab, PJ_LD, d, tid & 127);
+        __syncthreads();
         if (half == 0 && valid) {
+          float e[16];
 #pragma unroll
           for (int c = 0; c < 16; ++c) {
             const bool act = (c < 4) || c == 8 || (c >= 10 && c < 15);   // K and Q carry the LeakyReLU, V does not
-            e[c] = act ? lrelu(e[c], slope) : e[c];
+            const float x = S.d[r * PJ_LD + c];
+            e[c] = act ? lrelu(x, slope) : x;
           }
           float4* o = reinterpret_cast<float4*>(x5 + (long)node * 16);
 #pragma unroll
@@ -180,11 +123,15 @@ project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjCon
         }
         continue;
       }
+      {
+        float d[32];
+        wg_gemm6<64>(d, a_desc, [&](int s, int kb) {
+          return b_desc_ex(w_saddr + grp * C::GROUP_BYTES + s * C::SPLIT_BYTES + kb * 2048, 1024, 128); }, C::KB, false);
+        wg_store_d<64>(dslab, PJ_LD, d, tid & 127);
+      }
+      __syncthreads();
       float v[32];
-      tmem_ld32f(tmem + d * 64 + half * 32, v);
-      tc_fence_before();
-      wg_barrier(wg);                                 // every thread has drained D[d]
-      if (grp + 2 < C::NGROUPS) issue(grp + 2);       // refill it while this group's epilogue runs
+      tile_ld32f(S.d, PJ_LD, r, half * 32, v);
       const bool act = (grp == 2 || grp == 3);        // Q, K carry the LeakyReLU
 #pragma unroll
       for (int c = 0; c < 32; ++c) {
@@ -199,33 +146,28 @@ project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjCon
             for (int c4 = 0; c4 < 8; ++c4) o[c4] = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
           }
         } else {
-          // transpose through the warp's scratch so that 8 lanes write one contiguous 128-byte half row (full sectors)
+          // back through my row of the result tile so that 8 lanes write one contiguous 128-byte half row (full sectors)
+          float* sc = S.d + r * PJ_LD + half * 32;
 #pragma unroll
           for (int c4 = 0; c4 < 8; ++c4)
-            *reinterpret_cast<float4*>(sc + lane * PJ_SC_LD + c4 * 4) = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
+            *reinterpret_cast<float4*>(sc + c4 * 4) = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
           __syncwarp();
           float* o = proj + (long)(node0 + wrow0) * pw + grp * 64 + half * 32 + (lane & 7) * 4;
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const int row = i * 4 + (lane >> 3);
-            float4 t = *reinterpret_cast<const float4*>(sc + row * PJ_SC_LD + (lane & 7) * 4);
+            float4 t = *reinterpret_cast<const float4*>(S.d + (wrow0 + row) * PJ_LD + half * 32 + (lane & 7) * 4);
             if (node0 + wrow0 + row < n_nodes) *reinterpret_cast<float4*>(o + (long)row * pw) = t;
           }
-          __syncwarp();
         }
       }
       if (valid && grp >= 3 && kv != nullptr)
         store_kv_blocks(kv + (long)(grp - 3) * 3 * kv_split_stride, kv_split_stride, node, half, v);
+      __syncthreads();   // the result tile is free for the next group
     }
-    // next tile's rows -> scratch (lands behind the end-of-tile barrier and the other group's work)
-    load_rows(tile + gridDim.x * 2);
-    tc_fence_before();
-    wg_barrier(wg);  // A may be overwritten by the next tile
+    __syncthreads();     // A may be overwritten by the next tile
   }
-  tc_fence_before();
-  __syncthreads();
   TRACE_END(2);
-  tmem_release(S.tmem_base, warp);
 }
 
 // fp32 K / V columns of a projection buffer -> bf16x3 8-node blocks (used after the FFMA layer-0 node stage)
@@ -263,13 +205,12 @@ static int launch_project_tc(const eqd_graph* g, const eqd_layer* p_l, const flo
   eqd::PjConsts cst;
   memset(&cst, 0, sizeof(cst));
   memcpy(&cst, p_l->consts.proj_bias, 320 * sizeof(float));
-  int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
+  int ntiles = (g->n_nodes + eqd::PjCfg<L0>::R - 1) / eqd::PjCfg<L0>::R;
   size_t smem = sizeof(eqd::PjSmem<L0>) + 128;
   EQD_SET_SMEM((eqd::project_tc_kernel<L0>), smem);
-  int grid = (ntiles + 1) / 2;
-  if (grid > 148) grid = 148;
+  int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
-  eqd::project_tc_kernel<L0><<<grid, PJ_THREADS, smem, (cudaStream_t)stream>>>(
+  eqd::project_tc_kernel<L0><<<grid, eqd::PjCfg<L0>::THREADS, smem, (cudaStream_t)stream>>>(
       g->n_nodes, *p, cst, h, ldh, proj, pw, reinterpret_cast<unsigned char*>(kv), split_stride, x5);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;

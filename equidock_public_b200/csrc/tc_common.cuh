@@ -1,16 +1,16 @@
-// tcgen05 / TMEM / TMA / mbarrier primitives shared by the tensor-core kernels (sm_100a inline PTX).
+// wgmma / TMA / mbarrier primitives shared by the tensor-core kernels (sm_90a inline PTX).
 //
 // Numerics: every GEMM runs as "bf16x6": both operands are split into three bf16 terms
 // (v ~ v0 + v1 + v2, round-to-nearest at each level, 24 mantissa bits in total) and the six products
-// a0w0, a0w1, a1w0, a0w2, a1w1, a2w0 are accumulated in fp32 in TMEM, smallest first.  Measured on B200
-// (scripts/tc_probe.cu): max error 6.9e-7 on outputs of magnitude 5.7, below a plain fp32 FMA loop.
+// a0w0, a0w1, a1w0, a0w2, a1w1, a2w0 are accumulated in fp32 registers, smallest first.
 //
-// Operand conventions (M = 128 rows = TMEM lanes, thread r <-> row r):
-//   A : TMEM, K-major, 2 bf16 per 32-bit column (element k in the low half of column k/2 when k even),
-//       split s of a 64-wide operand at columns a + 32*s.  Written with tcgen05.st by the row's threads.
-//   B : shared memory, UMMA canonical no-swizzle layout made of 8x8 "core matrices" (128 contiguous
-//       bytes); descriptor = start address, LBO (stride between core matrices along K), SBO (along N).
-//   D : TMEM fp32, lane = row, column = n.  Read back with tcgen05.ld (32x32b: one row per thread).
+// Operand conventions (a tile of 128 rows = two warpgroups x 64 rows; in the epilogues thread r <-> row r):
+//   A : shared memory, written by the row's threads as bf16x3 (a_store8), canonical K-major no-swizzle layout
+//       of 8x8 "core matrices" (128 contiguous bytes).
+//   B : shared memory, same canonical layout; descriptor = start address, LBO (stride between core matrices
+//       along K), SBO (along N).
+//   D : fp32 accumulator fragments of each warpgroup's 64 rows, stored to a row-major shared-memory tile
+//       (wg_store_d) from which every thread reads its own row.
 #pragma once
 #include "common.cuh"
 
@@ -46,98 +46,101 @@ __device__ __forceinline__ void cp_async8(void* dst, const void* src) {
 __device__ __forceinline__ void cp_async4(void* dst, const void* src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src));
 }
-// barrier among the 256 threads of one tile group (named barriers 1, 2)
-__device__ __forceinline__ void wg_barrier(int wg) { asm volatile("bar.sync %0, 256;" ::"r"(wg + 1) : "memory"); }
-// barrier between the two warps that own the two column halves of the same 32 rows (named barriers 3..10)
-// group barrier + AND-reduction of a predicate over its 256 threads
-__device__ __forceinline__ bool wg_barrier_and(int wg, bool pred) {
-  unsigned r;
-  asm volatile(
-      "{\n\t.reg .pred p, q;\n\tsetp.ne.u32 p, %1, 0;\n\tbar.red.and.pred q, %2, 256, p;\n\tselp.u32 %0, 1, 0, q;\n\t}"
-      : "=r"(r)
-      : "r"((unsigned)pred), "r"(wg + 1)
-      : "memory");
-  return r != 0;
-}
+// barrier between the two warps that own the two column halves of the same 32 rows (named barriers 3..6)
 __device__ __forceinline__ void pair_barrier(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
-__device__ __forceinline__ void mbar_arrive(unsigned long long* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// Generic-proxy shared-memory writes (A operands) made visible to the tensor cores' async proxy; callers follow it
+// with the barrier that hands the operand to the warpgroups issuing the MMAs.
+__device__ __forceinline__ void tc_fence_before() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// No-swizzle canonical B descriptor (version bits for sm_100): lbo / sbo in bytes
+// No-swizzle canonical shared-memory matrix descriptor (sm_90 wgmma): lbo / sbo in bytes
 __device__ __forceinline__ unsigned long long b_desc_ex(unsigned saddr, unsigned lbo, unsigned sbo) {
-  return (unsigned long long)((saddr >> 4) & 0x3FFF) | ((unsigned long long)(lbo >> 4) << 16) |
-         ((unsigned long long)(sbo >> 4) << 32) | (1ull << 46);
-}
-// K-major weight panels [N=64][K]: LBO (K direction) = 1024 B, SBO (N direction) = 128 B
-__device__ __forceinline__ unsigned long long b_desc(unsigned saddr) { return b_desc_ex(saddr, 1024, 128); }
-// D[128x64] (+)= A[tmem, 128x16 bf16] * B[smem desc, 64x16 bf16]^T
-// instruction descriptor: D = f32, A = B = bf16, A K-major, M = 128; b_mn_major selects a [K][N] B operand
-__host__ __device__ constexpr unsigned umma_idesc(unsigned n, unsigned b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (b_mn_major << 16) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
-__device__ __forceinline__ void umma_ts_i(unsigned d_tmem, unsigned a_tmem, unsigned long long bdesc, unsigned idesc,
-                                          unsigned accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc),
-      "r"(accum) : "memory");
-}
-__device__ __forceinline__ void umma_ts(unsigned d_tmem, unsigned a_tmem, unsigned long long bdesc, unsigned accum) {
-  const unsigned idesc = umma_idesc(64, 0);
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc),
-      "r"(accum) : "memory");
-}
-// All 6 cross products of the bf16x3 splits, smallest terms first; A split s at a_base + s*a_split_cols,
-// weight split s at w_saddr + s*w_split_bytes (K-major panel, 2048 B per k-block of 16).
-// accum0 = 0 starts a fresh accumulator, 1 adds to what D already holds.
-__device__ __forceinline__ void issue_gemm(unsigned d_tmem, unsigned a_base, unsigned a_split_cols, unsigned w_saddr,
-                                           unsigned w_split_bytes, int kblocks, unsigned accum0 = 0) {
-  const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
-  unsigned accum = accum0;
-#pragma unroll
-  for (int pr = 0; pr < 6; ++pr)
-    for (int kb = 0; kb < kblocks; ++kb) {
-      umma_ts(d_tmem, a_base + pa[pr] * a_split_cols + kb * 8, b_desc(w_saddr + pb[pr] * w_split_bytes + kb * 2048), accum);
-      accum = 1;
-    }
-}
-// Same for a K-major [N][K] panel of any N (multiple of 16): a k-block of 16 is 32 N bytes, LBO = 16 N, SBO = 128.
-template <int N>
-__device__ __forceinline__ void issue_gemm_n(unsigned d_tmem, unsigned a_base, unsigned a_split_cols, unsigned w_saddr,
-                                             unsigned w_split_bytes, int kblocks, unsigned accum0 = 0) {
-  const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
-  const unsigned idesc = umma_idesc(N, 0);
-  unsigned accum = accum0;
-#pragma unroll
-  for (int pr = 0; pr < 6; ++pr)
-    for (int kb = 0; kb < kblocks; ++kb) {
-      umma_ts_i(d_tmem, a_base + pa[pr] * a_split_cols + kb * 8,
-                b_desc_ex(w_saddr + pb[pr] * w_split_bytes + kb * (N * 32), N * 16, 128), idesc, accum);
-      accum = 1;
-    }
-}
-// End of a kernel that owns tensor memory: every thread has passed its last tcgen05 operation (callers fence + sync
-// first); warp 0, which allocated the 512 columns, releases them.
-__device__ __forceinline__ void tmem_release(unsigned tmem_base, int warp) {
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
-}
-__device__ __forceinline__ bool elect_one() {
-  unsigned pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(unsigned long long* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+  return (unsigned long long)((saddr >> 4) & 0x3FFF) | ((unsigned long long)((lbo >> 4) & 0x3FFF) << 16) |
+         ((unsigned long long)((sbo >> 4) & 0x3FFF) << 32);
 }
 
-// ---- bf16x3 split of register tiles and TMEM stores / loads -------------------------------------
+// wgmma.mma_async m64nNk16, D fp32 in registers (+=), A and B bf16 from shared-memory descriptors;
+// TB = 1 reads B as MN-major ([K][N]).  scale_d = 0 starts a fresh accumulator.
+template <int N, int TB>
+struct Wgmma;
+template <int TB>
+struct Wgmma<16, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[8], unsigned long long a, unsigned long long b, int scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, %11;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TB));
+  }
+};
+template <int TB>
+struct Wgmma<64, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[32], unsigned long long a, unsigned long long b, int scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TB));
+  }
+};
+template <int TB>
+struct Wgmma<80, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[40], unsigned long long a, unsigned long long b, int scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, %43;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+        : "l"(a), "l"(b), "r"(scale_d), "n"(TB));
+  }
+};
+
+// bf16x6 GEMM of one 64-row slab on the calling warpgroup: d (+)= sum over the 6 split products (smallest terms
+// first) and k-blocks [0, kblocks) of A[split][kb] . B[split][kb]^T; a_desc(split, kb) / b_desc(split, kb) give the
+// operand descriptors.  hi_only: just the leading bf16 x bf16 product.  Returns with the MMAs complete.
+template <int N, int TB = 0, class AD, class BD>
+__device__ __forceinline__ void wg_gemm6(float (&d)[N / 2], AD a_desc, BD b_desc, int kblocks, bool accumulate,
+                                         bool hi_only = false) {
+  const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+  int scale_d = accumulate ? 1 : 0;
+#pragma unroll
+  for (int pr = hi_only ? 5 : 0; pr < 6; ++pr)
+    for (int kb = 0; kb < kblocks; ++kb) {
+      Wgmma<N, TB>::mma(d, a_desc(pa[pr], kb), b_desc(pb[pr], kb), scale_d);
+      scale_d = 1;
+    }
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+
+// A operand of a tile of R rows in shared memory, canonical K-major no-swizzle layout of 8 x 16-byte core matrices:
+//   byte offset of (split s, k-block kb, 8-channel half kh, row) = s * split_bytes + kb * 32R + kh * 16R + (row / 8) * 128
+//   + (row % 8) * 16.  The descriptor of warpgroup h's 64-row slab starts 1024 h bytes in (LBO = 16R, SBO = 128).
+template <int R>
+__device__ __forceinline__ unsigned long long a_desc_at(unsigned a_saddr, unsigned split_bytes, int wgi, int s, int kb) {
+  return b_desc_ex(a_saddr + s * split_bytes + kb * (32 * R) + wgi * 1024, 16 * R, 128);
+}
+// 8 consecutive channels [c, c + 8) of `row` (c a multiple of 8), as three packed bf16x3 split rows
+template <int R>
+__device__ __forceinline__ void a_store8(unsigned char* a, unsigned split_bytes, int row, int c, const unsigned* p0,
+                                         const unsigned* p1, const unsigned* p2) {
+  unsigned char* base = a + (c >> 4) * (32 * R) + ((c >> 3) & 1) * (16 * R) + (row >> 3) * 128 + (row & 7) * 16;
+  *reinterpret_cast<uint4*>(base) = make_uint4(p0[0], p0[1], p0[2], p0[3]);
+  *reinterpret_cast<uint4*>(base + split_bytes) = make_uint4(p1[0], p1[1], p1[2], p1[3]);
+  *reinterpret_cast<uint4*>(base + 2 * split_bytes) = make_uint4(p2[0], p2[1], p2[2], p2[3]);
+}
+
+// wgmma m64nN accumulator fragment of warpgroup thread t -> rows [0, 64) of a row-major fp32 tile (ld floats per row)
+template <int N>
+__device__ __forceinline__ void wg_store_d(float* tile, int ld, const float (&d)[N / 2], int t) {
+  const int row = (t >> 5) * 16 + ((t & 31) >> 2), col = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(tile + row * ld + 8 * j + col) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(tile + (row + 8) * ld + 8 * j + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+
+// ---- bf16x3 split of register tiles, A-operand stores, result-tile loads ---------------------------
 __device__ __forceinline__ unsigned cvt_bf16x2(float hi, float lo) {
   unsigned d;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
@@ -146,77 +149,39 @@ __device__ __forceinline__ unsigned cvt_bf16x2(float hi, float lo) {
 // (v0, v1) -> three packed bf16x2 words (v0 in the low half = even k)
 __device__ __forceinline__ void split3_pair(float v0, float v1, unsigned& p0, unsigned& p1, unsigned& p2) {
   p0 = cvt_bf16x2(v1, v0);
-  // v - hi as fma(hi, -1, v) on both lanes at once (fma.f32x2; exact product, same rounding as the subtraction)
-  const float2 m1 = make_float2(-1.f, -1.f);
-  float2 rr = __ffma2_rn(make_float2(__uint_as_float(p0 << 16), __uint_as_float(p0 & 0xFFFF0000u)), m1, make_float2(v0, v1));
-  p1 = cvt_bf16x2(rr.y, rr.x);
-  rr = __ffma2_rn(make_float2(__uint_as_float(p1 << 16), __uint_as_float(p1 & 0xFFFF0000u)), m1, rr);
-  p2 = cvt_bf16x2(rr.y, rr.x);
+  // v - hi, exact: hi is v rounded to bf16
+  const float r0 = v0 - __uint_as_float(p0 << 16), r1 = v1 - __uint_as_float(p0 & 0xFFFF0000u);
+  p1 = cvt_bf16x2(r1, r0);
+  p2 = cvt_bf16x2(r1 - __uint_as_float(p1 & 0xFFFF0000u), r0 - __uint_as_float(p1 << 16));
 }
-__device__ __forceinline__ void tmem_st16(unsigned taddr, const unsigned (&v)[16]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-               "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-               "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_st8(unsigned taddr, const unsigned* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-               "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_nowait(unsigned taddr, unsigned (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-      "%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-// 32 fp32 values (this thread's half of its row) -> bf16x3 -> TMEM: split s lands at a_taddr + 32*s, 16 columns
-// (split_cols: columns between consecutive splits of the A operand, 32 for a 64-wide K, 40 for K = 80)
-__device__ __forceinline__ void store_half_split3(unsigned a_taddr, const float (&v)[32], unsigned split_cols = 32) {
+// 32 fp32 values = channels [c0, c0 + 32) of `row` -> bf16x3 -> A operand
+template <int R>
+__device__ __forceinline__ void store_half_split3(unsigned char* a, unsigned split_bytes, int row, int c0, const float (&v)[32]) {
   unsigned p0[16], p1[16], p2[16];
 #pragma unroll
   for (int c = 0; c < 16; ++c) split3_pair(v[2 * c], v[2 * c + 1], p0[c], p1[c], p2[c]);
-  tmem_st16(a_taddr, p0);
-  tmem_st16(a_taddr + split_cols, p1);
-  tmem_st16(a_taddr + 2 * split_cols, p2);
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+#pragma unroll
+  for (int j = 0; j < 4; ++j) a_store8<R>(a, split_bytes, row, c0 + 8 * j, p0 + 4 * j, p1 + 4 * j, p2 + 4 * j);
 }
-// 8 fp32 values + 8 zeros (one K block of 16) -> bf16x3 -> 8 TMEM columns per split
-__device__ __forceinline__ void store_extra8_split3(unsigned a_taddr, const float (&t)[8], unsigned split_cols) {
+// 8 fp32 values + 8 zeros = channels [c0, c0 + 16) (one k-block) of `row` -> bf16x3 -> A operand
+template <int R>
+__device__ __forceinline__ void store_extra8_split3(unsigned char* a, unsigned split_bytes, int row, int c0, const float (&t)[8]) {
   unsigned p0[8], p1[8], p2[8];
 #pragma unroll
   for (int c = 0; c < 4; ++c) split3_pair(t[2 * c], t[2 * c + 1], p0[c], p1[c], p2[c]);
 #pragma unroll
   for (int c = 4; c < 8; ++c) p0[c] = p1[c] = p2[c] = 0u;
-  tmem_st8(a_taddr, p0);
-  tmem_st8(a_taddr + split_cols, p1);
-  tmem_st8(a_taddr + 2 * split_cols, p2);
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+  a_store8<R>(a, split_bytes, row, c0, p0, p1, p2);
+  a_store8<R>(a, split_bytes, row, c0 + 8, p0 + 4, p1 + 4, p2 + 4);
 }
-__device__ __forceinline__ void tmem_ld16f(unsigned taddr, float (&v)[16]) {
-  unsigned a[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]), "=r"(a[4]), "=r"(a[5]), "=r"(a[6]), "=r"(a[7]), "=r"(a[8]), "=r"(a[9]),
-        "=r"(a[10]), "=r"(a[11]), "=r"(a[12]), "=r"(a[13]), "=r"(a[14]), "=r"(a[15])
-      : "r"(taddr) : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// this thread's 32 channels of its row from a row-major fp32 tile
+__device__ __forceinline__ void tile_ld32f(const float* tile, int ld, int row, int c0, float (&v)[32]) {
+  const float4* s = reinterpret_cast<const float4*>(tile + row * ld + c0);
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(a[i]);
+  for (int c4 = 0; c4 < 8; ++c4) {
+    float4 t = s[c4];
+    v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
+  }
 }
-__device__ __forceinline__ void tmem_st4(unsigned taddr, const unsigned* v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]),
-               "r"(v[3]) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32f(unsigned taddr, float (&v)[32]) {
-  unsigned a[32];
-  tmem_ld32_nowait(taddr, a);
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(a[i]);
-}
-
 
 }  // namespace eqd

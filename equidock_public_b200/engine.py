@@ -1,8 +1,8 @@
-"""Host side of the B200 IEGMN forward engine: weight repacking, batch topology ("plan"), buffer
+"""Host side of the H100 IEGMN forward engine: weight repacking, batch topology ("plan"), buffer
 management and kernel sequencing over the C ABI (``include/eqd_iegmn.h``).
 
 PyTorch is used for device memory, streams and a few index-building ops only; all arithmetic of
-the hot path runs in the hand-written sm_100a kernels of ``csrc/``.  There is no CPU fallback.
+the hot path runs in the hand-written sm_90a kernels of ``csrc/``.  There is no CPU fallback.
 """
 from __future__ import annotations
 
@@ -48,7 +48,7 @@ def _upload_blob(tensors: Dict[str, torch.Tensor], device) -> Dict[str, torch.Te
 
 def umma_bf16x3(w: torch.Tensor) -> torch.Tensor:
     """[N][K] fp32 weight (nn.Linear layout, K % 8 == 0) -> 3 bf16 splits (w ~ w0+w1+w2, round to nearest), each in
-    the UMMA canonical K-major no-swizzle layout: element (n,k) at (k/8)*N*16 + (n/8)*128 + (n%8)*16 + (k%8)*2 bytes.
+    the canonical K-major no-swizzle layout of the wgmma shared-memory operands: element (n,k) at (k/8)*N*16 + (n/8)*128 + (n%8)*16 + (k%8)*2 bytes.
     Returns a flat bf16 tensor [3 * N * K]."""
     n, k = w.shape
     assert n % 8 == 0 and k % 8 == 0

@@ -1,5 +1,5 @@
 """Drop-in replacement for the reference's ``src/model/rigid_docking_model.py`` whose arithmetic
-runs in hand-written sm_100a CUDA kernels (``csrc/``) behind the C ABI of ``include/eqd_iegmn.h``.
+runs in hand-written sm_90a CUDA kernels (``csrc/``) behind the C ABI of ``include/eqd_iegmn.h``.
 
 Same public surface as the reference module (it is star-imported by ``src/utils/train_utils.py:14``,
 which ``train.py`` / ``inference_rigid.py`` star-import in turn, so the module-level names ``nn``,
@@ -248,7 +248,7 @@ class IEGMN_Layer(nn.Module):
         return x_out[:plan.N_l], h_out[:plan.N_l], x_out[plan.N_l:], h_out[plan.N_l:]
 
     def __repr__(self):
-        return 'IEGMN Layer (B200 engine) ' + str({k: v for k, v in self.__dict__.items() if not k.startswith('_')})
+        return 'IEGMN Layer (H100 engine) ' + str({k: v for k, v in self.__dict__.items() if not k.startswith('_')})
 
 
 class IEGMN(nn.Module):
@@ -366,7 +366,7 @@ class IEGMN(nn.Module):
                 list(keyp[:B].unbind(0)), list(keyp[B:].unbind(0))]
 
     def __repr__(self):
-        return 'IEGMN (B200 engine) ' + str({k: v for k, v in self.__dict__.items() if not k.startswith('_')})
+        return 'IEGMN (H100 engine) ' + str({k: v for k, v in self.__dict__.items() if not k.startswith('_')})
 
 
 class Rigid_Body_Docking_Net(nn.Module):
@@ -445,5 +445,5 @@ class Rigid_Body_Docking_Net(nn.Module):
         return ligand_coors, outputs[2], outputs[3], outputs[0], outputs[1]
 
     def __repr__(self):
-        return 'Rigid_Body_Docking_Net (B200 engine) ' + str({k: v for k, v in self.__dict__.items()
+        return 'Rigid_Body_Docking_Net (H100 engine) ' + str({k: v for k, v in self.__dict__.items()
                                                               if not k.startswith('_')})

@@ -1,4 +1,4 @@
-"""Training side of the B200 engine: forward with a layer stash, the hand-written backward (csrc/bwd_*.cu, head.cu,
+"""Training side of the H100 engine: forward with a layer stash, the hand-written backward (csrc/bwd_*.cu, head.cu,
 losses.cu) driven over the C ABI, a ``torch.autograd.Function`` so that the reference's own training loop
 (``loss.backward()``, src/train.py:154) works on the drop-in module unchanged, and a fused data-parallel trainer
 (device losses, flat-gradient NCCL all-reduce overlapped with the tail of backward, clip + Adam in one kernel;
@@ -168,7 +168,7 @@ class BackwardWorkspace:
             need = max(need, int(lib.eqd_tn_partial_floats(rows, K, nc, None, None)))
         self.partial = f(max(need, 1))
         self.colsum = f(4096 * 344)
-        self.vec = f(148 * 256)
+        self.vec = f(132 * 256)   # per-CTA partial sums of bwd_node / bwd_edge (grid <= EQD_SMS)
         self.head_ws_bytes = int(lib.eqd_bwd_head_workspace_bytes(N, plan.n_node_tiles, B))
         self.head_ws = torch.empty(self.head_ws_bytes, dtype=torch.uint8, device=device)
         # edges grouped by SOURCE node (ascending edge id inside a group): the transpose index of the CSR-by-destination

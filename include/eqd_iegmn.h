@@ -1,5 +1,5 @@
 /*
- * eqd_iegmn.h -- C ABI of the B200 (sm_100a) IEGMN forward engine.
+ * eqd_iegmn.h -- C ABI of the H100 (sm_90a) IEGMN forward engine.
  *
  * Drop-in boundary for the ONE hot path of octavian-ganea/equidock_public:
  *   src/model/rigid_docking_model.py  IEGMN_Layer.forward (:189-352), IEGMN.forward (:451-602),
@@ -98,15 +98,15 @@ typedef struct eqd_layer_params {
   const float* b_coor1;       /* [64] */
   const float* w_coor2;       /* [64] coors_mlp.4.weight */
   float b_coor2;              /* coors_mlp.4.bias */
-  /* tensor-core edge stage (tcgen05): the three edge-side weight matrices, each split into 3 bf16 terms
-   * (w ~ w0+w1+w2, round-to-nearest) and stored in the UMMA canonical K-major no-swizzle layout
+  /* tensor-core edge stage (wgmma): the three edge-side weight matrices, each split into 3 bf16 terms
+   * (w ~ w0+w1+w2, round-to-nearest) and stored in the canonical K-major no-swizzle layout of the wgmma shared-memory operands
    *   element (n,k) of split s at  base + s*split_bytes + (k/8)*1024 + (n/8)*128 + (n%8)*16 + (k%8)*2
    * GEMM1 = edge_mlp.0.weight[:, 2dh:] ([64][48], K 42 -> 48, base 0, split 6144 B); GEMM2+3 = the stacked
    * [128][64] panel [edge_mlp.4.weight ; coors_mlp.0.weight @ edge_mlp.4.weight] (base 18432, split 16384 B,
    * k-chunk stride 2048 B): msg and the coordinate MLP's hidden layer are both linear in the LayerNorm output.
    * 67584 B, 16B-aligned. */
   const void* w_edge_tc;
-  /* tensor-core node stage (dh == 64 layers only; NULL for the 69-wide layer 0). Same bf16x3 UMMA panels:
+  /* tensor-core node stage (dh == 64 layers only; NULL for the 69-wide layer 0). Same bf16x3 panels:
    *   w_node_tc : node_mlp.0.weight padded to [64][272] (K order h | aggr | mu | h0(69) | 0) at base 0, split
    *               34816 B; node_mlp.4.weight [64][64] at base 104448, split 8192 B            (129024 B)
    *   w_proj_tc : this layer's projection [Psrc|Pdst|Q|K|V] as 5 groups x 3 splits x 8192 B   (122880 B)
@@ -181,7 +181,7 @@ int eqd_project(const eqd_graph* g, const eqd_layer* p, const float* h, int32_t 
 /* Edge stage of IEGMN_Layer.forward (:204-237, 263-292): RBF, edge MLP, coordinate MLP, mean
  * aggregation at the destination, coordinate update.
  *   aggr[n][64] = mean_e msg_e ;  x_out[n] = eta*x_orig[n] + (1-eta)*x_in[n] + mean_e x_rel*phi
- * Runs on tcgen05 tensor cores (bf16x3 operand split, fp32 accumulation in TMEM).  he_lig / he_rec must be
+ * Runs on the tensor cores with wgmma (bf16x3 operand split, fp32 accumulation).  he_lig / he_rec must be
  * 16-byte aligned and readable up to the next 16-byte boundary past their end (TMA bulk copies).          */
 int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p, const float* proj,
                    const double* x_in, const double* x_orig, float* aggr, double* x_out,
@@ -199,9 +199,9 @@ int eqd_node_stage(const eqd_graph* g, const eqd_layer* p, const eqd_layer* p_ne
                    const float* h_in, int32_t ldh, const float* h0, const float* proj,
                    const float* aggr, float* h_out, float* proj_next, void* stream);
 
-/* ---- tensor-core node stage (tcgen05, layers with dh == 64) ---------------------------------------------
+/* ---- tensor-core node stage (wgmma, layers with dh == 64) ---------------------------------------------
  * K and V of every node travel as bf16x3 "8-node blocks": kv[which 2 (K,V)][split 3][n/8 (+8 zero pad
- * blocks)][d/8][n%8][d%8] bf16 (1 KB per block), so a run of blocks is a ready UMMA B operand for TMA.   */
+ * blocks)][d/8][n%8][d%8] bf16 (1 KB per block), so a run of blocks is a ready wgmma B operand for TMA.   */
 size_t eqd_kv_blocks_bytes(int32_t n_nodes);
 /* proj[n][320] = [Psrc|Pdst|Q|K|V](h[n]) for a dh==64 layer.  With kv != NULL, K and V are written ONLY as
  * bf16x3 blocks into kv and the fp32 columns 192..319 of proj are left untouched (nothing downstream reads them). */

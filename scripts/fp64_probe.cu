@@ -1,5 +1,5 @@
 // Measures the sustained fp64 rates of this GPU: scalar DFMA and mma.sync.m8n8k4.f64 (DMMA).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/fp64_probe scripts/fp64_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/fp64_probe scripts/fp64_probe.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __global__ void dfma_kernel(double* out, int iters, double a, double b) {

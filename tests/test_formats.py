@@ -1,6 +1,5 @@
-"""CPU: the on-disk formats (SURVEY 8f rank 4): flat pair archive round trip incl. labels, PDB writer against the
-reference's shipped output PDB (authoring container only), checkpoint dict compatible with the reference's loader."""
-import os
+"""CPU: the on-disk formats (SURVEY 8f rank 4): flat pair archive round trip incl. labels, PDB writer round trip,
+checkpoint dict compatible with the reference's loader."""
 
 import numpy as np
 import pytest
@@ -48,21 +47,6 @@ def test_pdb_writer_round_trip_and_columns(tmp_path):
     lines, xyz = formats.read_pdb_atoms(str(tmp_path / 'out.pdb'))
     assert len(lines) == 3 and lines[0][:30] == 'ATOM      1  N   MET A   1    ' and lines[0][54:60] == '  1.00'
     assert np.allclose(xyz[0], [-24.430 + 1, 27.340 + 2, 2.614 - 300.5], atol=5e-4)
-
-
-@pytest.mark.skipif(not os.path.isdir('/root/reference/test_sets_pdb'), reason='needs the reference test set (authoring container)')
-def test_pdb_writer_reproduces_shipped_output_pdb(tmp_path):
-    name = 'kq_1kq1.pdb1_2.dill'
-    base = '/root/reference/test_sets_pdb'
-    src = f'{base}/dips_test_random_transformed/random_transformed/{name}_l_b.pdb'
-    shipped = f'{base}/dips_equidock_results/{name}_l_b_EQUIDOCK.pdb'
-    _, allp = gio.load_all('dips')
-    e = allp[name]
-    formats.apply_rigid_to_pdb(src, str(tmp_path / 'o.pdb'), e['ref32']['rotation'], e['ref32']['translation'])
-    l1, x1 = formats.read_pdb_atoms(str(tmp_path / 'o.pdb'))
-    l2, x2 = formats.read_pdb_atoms(shipped)
-    assert len(l1) == len(l2) and np.abs(x1 - x2).max() < 2.1e-3
-    assert all(a[:30] == b[:30] for a, b in zip(l1, l2))
 
 
 def test_checkpoint_dict_has_the_reference_keys(tmp_path):

@@ -1,4 +1,4 @@
-"""GPU (B200) acceptance on ALL 125 shipped test pairs (25 DB5.5 + 100 DIPS), end to end on the device:
+"""GPU (H100) acceptance on ALL 125 shipped test pairs (25 DB5.5 + 100 DIPS), end to end on the device:
 compact all-atom inputs -> GPU graph construction (csrc/graph_build.cu) -> engine forward -> (R, t) -> batched RMSD meter.
   * the GPU-built graphs equal the numpy graph oracle (== the reference's preprocessing on all 125 pairs) on a subset;
   * (R, t) of every pair against the reference's own fp64 run: rotation <= 3e-5, predicted C-alpha coordinates within
@@ -100,7 +100,7 @@ def test_all_shipped_pairs_poses_and_rmsd_table(ds, cuda_device):
     print(f'{ds}: engine vs fp64 oracle on identical (GPU-built) inputs: worst err / bound = {rows[0][3]:.3f}; top 5:',
           [(n, f'{er:.2e}', f'{y:.2e}') for n, er, y, _, _ in rows[:5]])
     # 1 x yardstick + one output ulp per pair; the yardstick is ONE sample of the reference's own fp32 noise (it moves by up
-    # to 2.8 x with the BLAS thread count, profiles/r02_yardstick_spread.txt), so up to 4 % of the pairs may sit within 1.5 x
+    # with the BLAS thread count), so up to 4 % of the pairs may sit within 1.5 x
     over = [r for r in rows if r[3] > 1.0]
     assert all(r[3] <= 1.5 for r in rows) and len(over) <= max(1, len(rows) // 25), over
     assert all(r[4] <= max(3e-5, 0.2 * r[2]) for r in rows), [r for r in rows if r[4] > max(3e-5, 0.2 * r[2])]

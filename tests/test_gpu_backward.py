@@ -1,4 +1,4 @@
-"""GPU (B200): the hand-written CUDA backward (csrc/bwd_*.cu, head.cu) and the device losses / optimiser kernels against
+"""GPU (H100): the hand-written CUDA backward (csrc/bwd_*.cu, head.cu) and the device losses / optimiser kernels against
 the fp64 oracles.  Stage by stage against oracle/backward_manual.py (itself == torch.autograd == the reference's golden
 gradients, tests/test_backward_manual.py), then end to end through ``loss.backward()`` on the drop-in module.
 Tolerance: the backward runs in fp32 (coordinates / head in fp64); gradients are compared relative to the largest entry of
@@ -64,9 +64,9 @@ def _stage_report(model, args, pairs, grad_fns, cuda_device):
     g = gio.make_batch(pairs, cuda_device)
     fwd = eng.forward(g)
     B = len(pairs)
-    if bool(fwd['status_host'][:B].any()):
-        pytest.skip('SVD guard fired (rank-deficient keypoint cloud of a random-init model): the random perturbation '
-                    'branch (:574-584) is not part of the manual oracle')
+    # the random perturbation branch of the SVD guard (:574-584) is not part of the manual oracle: inputs must not reach it
+    assert not bool(fwd['status_host'][:B].any()), ('status flags (SVD guard / NaN / bad residue) on a stage-by-stage case',
+                                                    fwd['status_host'][:B].tolist())
     co_ref = np.concatenate([pp[1]['ligand_coors'] for pp in per_pair])
     assert np.abs(_np(fwd['ligand_coors']) - co_ref).max() < 2e-3 * max(1.0, np.abs(co_ref).max() / 100)
     dco = np.concatenate([pp[2][0] for pp in per_pair])
@@ -139,10 +139,18 @@ def test_backward_stage_by_stage_vs_manual_oracle(ds, cuda_device):
 @pytest.mark.parametrize('kind', ['db5', 'dips', 'random'])
 def test_backward_stage_by_stage_ragged_batch(kind, cuda_device):
     """B = 3 ragged pairs incl. tile boundaries (129 = 128 + 1, 131 = 128 + 3): both checkpoints (5 shared layers / 8
-    layers) and a random-init 3-layer unshared model with non-trivial biases / LayerNorm affine parameters."""
+    layers) and a random-init 3-layer unshared model with non-trivial biases / LayerNorm affine parameters.  The random
+    model's keypoint attention is sharpened: at default init it is nearly uniform, every keypoint sits at the centroid and
+    the reference's SVD guard (:574) fires on all three pairs (the fp64 oracle's own verdict).  Its seed keeps every edge
+    pre-activation of the fp64 oracle >= 1.5e-6 away from the LeakyReLU kink: closer than fp32 resolves, the engine may take
+    the other branch and the derivative there differs by 0.99 x the upstream gradient (seed 5 has one at 1.4e-8)."""
     from test_gpu_parity import _random_model
     if kind == 'random':
-        model, args = _random_model(cuda_device, 3, False, seed=5)
+        model, args = _random_model(cuda_device, 3, False, seed=7)
+        with torch.no_grad():
+            for name, p in model.named_parameters():
+                if name.startswith(('iegmn_original.att_mlp_key_ROT.', 'iegmn_original.att_mlp_query_ROT.')):
+                    p.mul_(8.0)
     else:
         model, args = gio.build_model(kind, cuda_device), gio.load_args(kind)
     model.train()

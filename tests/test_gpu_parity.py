@@ -1,4 +1,4 @@
-"""GPU (B200) parity tests: the CUDA engine, called through the reference-facing module and the C ABI,
+"""GPU (H100) parity tests: the CUDA engine, called through the reference-facing module and the C ABI,
 against (a) outputs of the reference's unmodified module in fp64 on its shipped test inputs/checkpoints
 (tests/golden), (b) the numpy fp64 oracle on seeded synthetic / ragged / edge-case graphs, and
 (c) size-independent properties at the bench's full size.
@@ -8,10 +8,8 @@ Tolerance (north_star: 1e-4 on predicted coordinates; SURVEY 7's definition): pe
 i.e. no worse than the reference's own fp32 evaluation of itself on that pair (SURVEY 0, 7 'hard parts': the
 layer-evolved coordinates reach 1e3 A, one fp32 ulp = 6e-5 A).  Both quantities being compared are fp32 OUTPUT
 coordinates (|coords| up to 64 A -> one ulp = 3.8e-6 A), so each is only known to one output ulp: that ulp is the
-additive term.  The per-pair errors of the shipped build are written by scripts/parity_table.py
-(profiles/r02_parity_table.txt): 8 of 9 fixtures are at 0.03 .. 0.54 of their yardstick, 1QA9 at 1.17e-4 vs 1.13e-4 (exactly
-one output ulp above).  The yardstick itself is one sample of fp32 rounding noise: the reference's fp32 evaluation of 1QA9
-errs by 4.0e-5 / 5.2e-5 / 1.13e-4 A with 2 / 1 / 8 BLAS threads (profiles/r02_yardstick_spread.txt).
+additive term.  The per-pair errors of a build are written by scripts/parity_table.py.  The yardstick itself is one
+sample of fp32 rounding noise: the reference's fp32 evaluation of a pair changes with the BLAS thread count.
 """
 import ctypes as C
 
