@@ -6,7 +6,8 @@
 //
 // Operand conventions (a tile of 128 rows = two warpgroups x 64 rows; in the epilogues thread r <-> row r):
 //   A : shared memory, written by the row's threads as bf16x3 (a_store8), canonical K-major no-swizzle layout
-//       of 8x8 "core matrices" (128 contiguous bytes).
+//       of 8x8 "core matrices" (128 contiguous bytes); or registers (RS form): an fp32 accumulator fragment split into
+//       bf16x3 A fragments in place (acc_to_a_split3), so a GEMM can consume the previous one's epilogue directly.
 //   B : shared memory, same canonical layout; descriptor = start address, LBO (stride between core matrices
 //       along K), SBO (along N).
 //   D : fp32 accumulator fragments of each warpgroup's 64 rows, stored to a row-major shared-memory tile
@@ -46,8 +47,6 @@ __device__ __forceinline__ void cp_async8(void* dst, const void* src) {
 __device__ __forceinline__ void cp_async4(void* dst, const void* src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(dst)), "l"(src));
 }
-// barrier between the two warps that own the two column halves of the same 32 rows (named barriers 3..6)
-__device__ __forceinline__ void pair_barrier(int id) { asm volatile("bar.sync %0, 64;" ::"r"(id) : "memory"); }
 // Generic-proxy shared-memory writes (A operands) made visible to the tensor cores' async proxy; callers follow it
 // with the barrier that hands the operand to the warpgroups issuing the MMAs.
 __device__ __forceinline__ void tc_fence_before() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -93,12 +92,28 @@ struct Wgmma<80, TB> {
   }
 };
 
+// RS form: A from registers (4 x bf16x2 per thread per k16 block, the m16n8k16 A-fragment layout of the warp's 16 rows),
+// B from a shared-memory descriptor.
+template <int N, int TB>
+struct WgmmaRS;
+template <int TB>
+struct WgmmaRS<64, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[32], const unsigned (&a)[4], unsigned long long b, int scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d), "n"(TB));
+  }
+};
+
 // bf16x6 GEMM of one 64-row slab on the calling warpgroup: d (+)= sum over the 6 split products (smallest terms
 // first) and k-blocks [0, kblocks) of A[split][kb] . B[split][kb]^T; a_desc(split, kb) / b_desc(split, kb) give the
-// operand descriptors.  hi_only: just the leading bf16 x bf16 product.  Returns with the MMAs complete.
+// operand descriptors.  hi_only: just the leading bf16 x bf16 product.  The _issue form returns with the MMAs in flight
+// (one commit group; wg_mma_wait completes them), wg_gemm6 with the MMAs complete.
 template <int N, int TB = 0, class AD, class BD>
-__device__ __forceinline__ void wg_gemm6(float (&d)[N / 2], AD a_desc, BD b_desc, int kblocks, bool accumulate,
-                                         bool hi_only = false) {
+__device__ __forceinline__ void wg_gemm6_issue(float (&d)[N / 2], AD a_desc, BD b_desc, int kblocks, bool accumulate,
+                                               bool hi_only = false) {
   const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
   int scale_d = accumulate ? 1 : 0;
@@ -109,7 +124,35 @@ __device__ __forceinline__ void wg_gemm6(float (&d)[N / 2], AD a_desc, BD b_desc
       scale_d = 1;
     }
   asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+}
+// waits for every MMA group of the warpgroup; the accumulators handed in are not touched before it
+template <int M>
+__device__ __forceinline__ void wg_mma_wait(float (&d)[M]) {
   asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+#pragma unroll
+  for (int i = 0; i < M; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+template <int N, int TB = 0, class AD, class BD>
+__device__ __forceinline__ void wg_gemm6(float (&d)[N / 2], AD a_desc, BD b_desc, int kblocks, bool accumulate,
+                                         bool hi_only = false) {
+  wg_gemm6_issue<N, TB>(d, a_desc, b_desc, kblocks, accumulate, hi_only);
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+}
+// wg_gemm6_issue with A from registers: a[split][kb] are the bf16x3 A fragments (acc_to_a_split3), same product order.
+// Returns with the MMAs in flight (wg_mma_wait).
+template <int N, int KB, int TB = 0, class BD>
+__device__ __forceinline__ void wg_gemm6_rs_issue(float (&d)[N / 2], const unsigned (&a)[3][KB][4], BD b_desc, bool accumulate) {
+  constexpr int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+  int scale_d = accumulate ? 1 : 0;
+#pragma unroll
+  for (int pr = 0; pr < 6; ++pr)
+#pragma unroll
+    for (int kb = 0; kb < KB; ++kb) {
+      WgmmaRS<N, TB>::mma(d, a[pa[pr]][kb], b_desc(pb[pr], kb), scale_d);
+      scale_d = 1;
+    }
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
 
 // A operand of a tile of R rows in shared memory, canonical K-major no-swizzle layout of 8 x 16-byte core matrices:
@@ -173,6 +216,26 @@ __device__ __forceinline__ void store_extra8_split3(unsigned char* a, unsigned s
   for (int c = 4; c < 8; ++c) p0[c] = p1[c] = p2[c] = 0u;
   a_store8<R>(a, split_bytes, row, c0, p0, p1, p2);
   a_store8<R>(a, split_bytes, row, c0 + 8, p0 + 4, p1 + 4, p2 + 4);
+}
+// m64nN fp32 accumulator fragment (N = 16 KB columns) -> bf16x3 A fragments of an RS wgmma whose K runs over those
+// columns.  The accumulator's (row, column) ownership is the A fragment's (row, k) ownership: d[8kb + 2i], d[8kb + 2i + 1]
+// hold (row g + 8 (i & 1), k = 16 kb + 8 (i >> 1) + 2 (lane & 3) + {0, 1}) = A register i of k-block kb.
+template <int KB>
+__device__ __forceinline__ void acc_to_a_split3(const float (&v)[8 * KB], unsigned (&a)[3][KB][4]) {
+#pragma unroll
+  for (int kb = 0; kb < KB; ++kb)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) split3_pair(v[8 * kb + 2 * i], v[8 * kb + 2 * i + 1], a[0][kb][i], a[1][kb][i], a[2][kb][i]);
+}
+// barrier of one warpgroup (128 threads) on named barrier `id`; the _and form also returns whether pred holds on all
+__device__ __forceinline__ void wg_barrier(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ bool wg_barrier_and(int id, bool pred) {
+  unsigned all;
+  asm volatile(
+      "{\n\t.reg .pred p, q;\n\tsetp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.and.pred q, %2, 128, p;\n\tselp.u32 %0, 1, 0, q;\n\t}"
+      : "=r"(all) : "r"((unsigned)pred), "r"(id) : "memory");
+  return all != 0;
 }
 // this thread's 32 channels of its row from a row-major fp32 tile
 __device__ __forceinline__ void tile_ld32f(const float* tile, int ld, int row, int c0, float (&v)[32]) {

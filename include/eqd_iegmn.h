@@ -181,7 +181,8 @@ int eqd_project(const eqd_graph* g, const eqd_layer* p, const float* h, int32_t 
 /* Edge stage of IEGMN_Layer.forward (:204-237, 263-292): RBF, edge MLP, coordinate MLP, mean
  * aggregation at the destination, coordinate update.
  *   aggr[n][64] = mean_e msg_e ;  x_out[n] = eta*x_orig[n] + (1-eta)*x_in[n] + mean_e x_rel*phi
- * Runs on the tensor cores with wgmma (bf16x3 operand split, fp32 accumulation).  he_lig / he_rec must be
+ * Runs on the tensor cores with wgmma (bf16x3 operand split, fp32 accumulation) when max_in_degree <= 64 (a node's
+ * in-edges fit one 64-row tile); for 64 < max_in_degree <= 128 it runs eqd_edge_stage_ffma.  he_lig / he_rec must be
  * 16-byte aligned and readable up to the next 16-byte boundary past their end (TMA bulk copies).          */
 int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p, const float* proj,
                    const double* x_in, const double* x_orig, float* aggr, double* x_out,
