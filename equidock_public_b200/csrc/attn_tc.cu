@@ -1,15 +1,17 @@
-// Segmented cross attention of a 64-wide IEGMN layer (rigid_docking_model.py:46-64, 247-256) on the tensor
-// cores (wgmma, bf16x6):   mu_i = sum_j softmax_j(q_i . k_j) v_j   over the partner protein's nodes j
+// Segmented cross attention of an IEGMN layer (rigid_docking_model.py:46-64, 247-256) on the tensor cores (wgmma,
+// bf16x6):   mu_i = sum_j softmax_j(q_i . k_j) v_j   over the partner protein's nodes j
 // (the per-pair block of the reference's dense masked softmax; no 1/sqrt(d)).
 //
-// A tile = 128 query nodes of one protein; one CTA of 256 threads (2 threads per query row, two 64-row warpgroup
-// slabs in the GEMMs).  K and V of every node arrive as bf16x3 8-node blocks (written by the projection kernel), so a
-// run of 8 blocks (64 keys) is TMA-bulk-copied straight into shared memory as a wgmma B operand:
-//   S = Q K^T   : A = Q (smem, bf16x3), B = K blocks, K-major  (n = key, k = d)
-//   O += P V    : A = P (smem, bf16x3), B = V blocks, MN-major (k = key, n = d)
-// The P region also holds the fp32 S and O tiles between the MMAs and the threads that read them.
+// K and V of every node arrive as bf16x3 8-node blocks (written by the projection kernel), so a run of 8 blocks (64 keys)
+// is TMA-bulk-copied straight into shared memory as a wgmma B operand:
+//   S = Q K^T   : A = Q (bf16x3), B = K blocks, K-major  (n = key, k = d)
+//   O += P V    : A = P (bf16x3), B = V blocks, MN-major (k = key, n = d)
 // Two passes over the keys (row maxima first, then exp / P.V) instead of an online softmax: the extra S GEMMs
 // are cheap on the tensor pipe and O never has to be rescaled.
+//
+// Layer 0 (attention0_tc_kernel): a tile = 128 query nodes of one protein; one CTA of 256 threads (2 threads per query
+// row, two 64-row warpgroup slabs in the GEMMs); A operands in shared memory, the P region also holds the fp32 S and O
+// tiles between the MMAs and the threads that read them.  The 64-wide layers: attention64_tc_kernel below.
 #include "tc_common.cuh"
 
 namespace eqd {
@@ -28,33 +30,30 @@ __device__ long long g_attn_prof[16];
 #define AT_A_SPLIT 16384      // Q and P operands: 128 rows x 64 bf16 per split
 #define AT_LD 68              // fp32 row stride of the S / O tiles
 
-// X5 = the 69-wide layer 0: the tensor cores handle channels 0..63 exactly as in a 64-wide layer; channels 64..68 of
+// The 69-wide layer 0: the tensor cores handle channels 0..63 exactly as in a 64-wide layer; channels 64..68 of
 // Q, K, V (fp32 in x5[n][16] = [K64..67 | V64..67 | K68 V68 | Q64..68 | 0], written by the layer-0 projection) are a
 // rank-5 update of the scores and five extra output columns, done with plain FMAs next to the exp().
-template <bool X5>
 struct AtGroupSmem {
   unsigned char k[2][3][AT_CHUNK_BYTES];  // double-buffered K chunks (3 splits)
   unsigned char v[2][3][AT_CHUNK_BYTES];
   float red[EQD_TM * 2];
-  float x5c[X5 ? 2 : 1][X5 ? AT_KEYS * 16 : 4];   // x5 rows of the K chunk in flight (same double buffering as k)
-  float red5[X5 ? EQD_TM * 2 * 5 : 4];
+  float x5c[2][AT_KEYS * 16];   // x5 rows of the K chunk in flight (same double buffering as k)
+  float red5[EQD_TM * 2 * 5];
 };
-template <bool X5>
 struct AtSmem {
   unsigned char qa[3 * AT_A_SPLIT];   // Q (A of S = Q K^T)
   unsigned char pa[3 * AT_A_SPLIT];   // P (A of O = P V), or the fp32 S / O tile [128][AT_LD]
-  AtGroupSmem<X5> grp;
+  AtGroupSmem grp;
   unsigned long long k_bar[2], v_bar[2];
 };
 
-template <bool X5>
 __global__ void __launch_bounds__(AT_THREADS, 1)
-attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const unsigned char* __restrict__ kv,
+attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const unsigned char* __restrict__ kv,
                     long kv_split_stride, const float* __restrict__ x5, float* __restrict__ mu, int ldmu) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  AtSmem<X5>& S = *reinterpret_cast<AtSmem<X5>*>(smem_raw);
+  AtSmem& S = *reinterpret_cast<AtSmem*>(smem_raw);
   const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, wgi = tid >> 7;
-  AtGroupSmem<X5>& G = S.grp;
+  AtGroupSmem& G = S.grp;
   TRACE_START(1);
   if (tid == 0) {
     for (int b = 0; b < 2; ++b) {
@@ -78,7 +77,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
   auto load_chunk = [&](const unsigned char* src, unsigned char (*dst)[AT_CHUNK_BYTES], unsigned long long* bar, int blk0,
                         int x5buf) {
     if (q == 0) {
-      const bool with5 = X5 && x5buf >= 0;
+      const bool with5 = x5buf >= 0;
       mbar_expect_tx(bar, 3 * AT_CHUNK_BYTES + (with5 ? AT_KEYS * 64 : 0));
 #pragma unroll
       for (int s = 0; s < 3; ++s) bulk_g2s(dst[s], src + s * kv_split_stride + (long)blk0 * 1024, AT_CHUNK_BYTES, bar);
@@ -136,7 +135,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
     PROF_MARK(0);   // tile metadata (dependent global loads)
     if (nchunks > 0) load_chunk(k_g, G.k[0], &S.k_bar[0], blk_lo, 0);
     float q5[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    if (X5 && valid) {
+    if (valid) {
 #pragma unroll
       for (int e = 0; e < 5; ++e) q5[e] = x5[(long)node * 16 + 10 + e];
     }
@@ -170,7 +169,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
       PROF_MARK(3);   // pass 1: S(hi) MMAs
       float s[32];
       tile_ld32f(dtile, AT_LD, r, half * 32, s);
-      if (X5) add_s5(s, G.x5c[kb_], q5);
+      add_s5(s, G.x5c[kb_], q5);
       const int key0 = (blk_lo + 8 * c) * 8 + half * 32;
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
@@ -206,7 +205,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
       PROF_MARK(6);   // pass 2: S MMAs
       float s[32];
       tile_ld32f(dtile, AT_LD, r, half * 32, s);
-      if (X5) add_s5(s, G.x5c[kb_], q5);
+      add_s5(s, G.x5c[kb_], q5);
       const int key0 = (blk_lo + 8 * c) * 8 + half * 32;
       float l4[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
@@ -215,7 +214,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
         float pj = (kn >= j0 && kn < j1) ? expf(s[i] - mx) : 0.f;
         s[i] = pj;
         l4[i & 3] += pj;
-        if (X5) {   // the five extra output columns: o5 += p V5[key]
+        {   // the five extra output columns: o5 += p V5[key]
           const float* row = G.x5c[kb_] + (half * 32 + i) * 16;
           const float4 v4 = *reinterpret_cast<const float4*>(row + 4);
           o5[0] = fmaf(pj, v4.x, o5[0]);
@@ -256,7 +255,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
     }
     // ---------------- mu = O / l -----------------------------------------------------------------------------
     G.red[r * 2 + half] = l;
-    if (X5) {
+    {
 #pragma unroll
       for (int e = 0; e < 5; ++e) G.red5[(r * 2 + half) * 5 + e] = o5[e];
     }
@@ -264,7 +263,7 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
     l = G.red[r * 2] + G.red[r * 2 + 1];
     {
       const float inv = l > 0.f ? 1.f / l : 0.f;
-      if (X5 && valid && half == 0) {   // mu[64..68], then zeros up to the row stride
+      if (valid && half == 0) {   // mu[64..68], then zeros up to the row stride
         float e8[8];
 #pragma unroll
         for (int e = 0; e < 5; ++e) e8[e] = (G.red5[r * 10 + e] + G.red5[r * 10 + 5 + e]) * inv;
@@ -291,6 +290,233 @@ attention_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const u
   TRACE_END(1);
 }
 
+// ---- the 64-wide layers ---------------------------------------------------------------------------------------------
+// One persistent CTA of two warpgroups per SM.  Each warpgroup runs its own chain of 64-row query tiles (the halves of
+// the 128-row node_tiles entries; empty halves are skipped) and synchronises only inside itself: its named barrier, its
+// own double-buffered K / V chunks and their mbarriers.  While one chain runs its exp / split epilogue, the other's MMAs
+// use the tensor pipe.  Every GEMM is an RS wgmma whose accumulator stays in registers:
+//   S = Q K^T : A = Q fragments (bf16x3, built once per tile from the staged Q rows), B = K chunk
+//   O = P V   : A = P fragments (exp(S - max) of the S accumulator, split in place), B = V chunk (MN-major)
+// The K chunks of both passes and the V chunks form two streams that run one chunk ahead of their use across tile
+// boundaries, so the next tile's first K and V chunks land during this tile's last chunk.  The next tile's Q rows are
+// cp.async'ed into the staging buffer during this tile.  The chunk walk (8-node blocks from the partner's first block)
+// does not depend on the query tile: every per-element sum has the order of the 128-row kernel it replaces.
+#define AT_CHAINS 2
+
+struct __align__(128) AtChainSmem {
+  unsigned char k[2][3][AT_CHUNK_BYTES];   // double-buffered K chunks (3 splits)
+  unsigned char v[2][3][AT_CHUNK_BYTES];
+  float qs[64 * 64];                       // Q rows of the next tile (16-byte chunks swizzled, staged_rows_to_a_split3)
+  unsigned long long k_bar[2], v_bar[2];
+};
+
+struct AtTile {        // one 64-row query tile
+  int node0, nvalid;   // first query node, valid rows (> 0)
+  int j0, j1;          // partner key range
+  int blk_lo, nchunks; // first 8-node block of the walk, 64-key chunks
+};
+
+__global__ void __launch_bounds__(AT_CHAINS * 128, 1)
+attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigned char* __restrict__ kv,
+                      long kv_split_stride, float* __restrict__ mu) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  AtChainSmem& W = reinterpret_cast<AtChainSmem*>(smem_raw)[threadIdx.x >> 7];
+  const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, lane = t & 31;
+  const int bar = 1 + wgi;   // this chain's named barrier
+  TRACE_START(1);
+  if (t == 0) {
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(&W.k_bar[b], 1);
+      mbar_init(&W.v_bar[b], 1);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  wg_barrier(bar);
+  const unsigned k_saddr = smem_u32(W.k), v_saddr = smem_u32(W.v);
+  const int B = g.n_pairs, nht = 2 * g.n_node_tiles, hstride = gridDim.x * AT_CHAINS;
+  const unsigned char* k_g = kv;                              // which = 0
+  const unsigned char* v_g = kv + 3 * kv_split_stride;        // which = 1
+
+  // The k-th tile of this chain is the half (chain + k hstride) ^ (k & 1): hstride is even, so without the swap a chain
+  // would always take the same half of the 128-row tiles, and only second halves can be empty.
+  const int chain = blockIdx.x * AT_CHAINS + wgi;
+  // the chain's first non-empty tile from its k-th on: returns its k (-1 if none) and its metadata
+  auto find_tile = [&](int k, AtTile& m) {
+    for (; chain + k * hstride < nht; ++k) {
+      const int ht = (chain + k * hstride) ^ (k & 1);
+      const int seg = __ldg(g.node_tiles + 2 * (ht >> 1));
+      m.node0 = __ldg(g.node_tiles + 2 * (ht >> 1) + 1) + 64 * (ht & 1);
+      m.nvalid = min(64, __ldg(g.seg_ptr + seg + 1) - m.node0);
+      if (m.nvalid <= 0) continue;
+      const int pseg = seg < B ? seg + B : seg - B;
+      m.j0 = __ldg(g.seg_ptr + pseg);
+      m.j1 = __ldg(g.seg_ptr + pseg + 1);
+      m.blk_lo = m.j0 >> 3;
+      m.nchunks = (((m.j1 + 7) >> 3) - m.blk_lo + 7) >> 3;
+      return k;
+    }
+    return -1;
+  };
+  // K (V) chunk stream: the n-th chunk filled / consumed uses buffer n & 1, mbarrier phase (n >> 1) & 1.  A chunk is filled
+  // into the buffer that the chunk before it has left, and only after a chain barrier that follows every thread's wait on
+  // that chunk: so a K / V mbarrier is re-armed only after all 128 threads of the chain have observed its previous phase.
+  unsigned kfill = 0, kcons = 0, vfill = 0, vcons = 0;
+  auto fill = [&](unsigned char (*dst)[3][AT_CHUNK_BYTES], unsigned long long* bars, unsigned& n, const unsigned char* src,
+                  int blk0) {
+    if (t == 0) {
+      unsigned long long* b = &bars[n & 1];
+      mbar_expect_tx(b, 3 * AT_CHUNK_BYTES);
+#pragma unroll
+      for (int s = 0; s < 3; ++s) bulk_g2s(dst[n & 1][s], src + s * kv_split_stride + (long)blk0 * 1024, AT_CHUNK_BYTES, b);
+    }
+    ++n;
+  };
+  auto consume = [&](unsigned long long* bars, unsigned& n) {
+    mbar_wait(&bars[n & 1], (n >> 1) & 1);
+    return (int)((n++) & 1);
+  };
+  auto stage_q = [&](const AtTile& m) { stage_rows64(W.qs, proj, 320, 128, m.node0, m.nvalid, t); };
+
+  // accumulator-fragment rows of this thread: fr0 and fr0 + 8; columns (keys, channels) 8 j + fc + {0, 1}, j = 0..7
+  const int fr0 = (t >> 5) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+  AtTile cur, nxt;
+  int kt = find_tile(0, cur);
+  bool k_ahead = false, v_ahead = false;   // the current tile's first K / V chunk is already in flight
+  if (kt >= 0) stage_q(cur);
+  while (kt >= 0) {
+    if (t == 0) TRACE_PHASE(1, chain, kt, 1);
+    // The next tile's metadata (dependent global loads) and Q rows are fetched once the first S GEMM of pass 1 is in flight.
+    int ktn = -1;
+    bool looked = false;
+    auto look_ahead = [&]() {
+      if (looked) return;
+      looked = true;
+      ktn = find_tile(kt + 1, nxt);
+      if (ktn >= 0) stage_q(nxt);   // the staging buffer is free
+    };
+    if (cur.nchunks > 0 && !k_ahead) fill(W.k, W.k_bar, kfill, k_g, cur.blk_lo);
+    // this tile's Q rows have landed (every thread's own copies, then the barrier for the others')
+    cp_async_wait<0>();
+    wg_barrier(bar);
+    unsigned qf[3][4][4];
+    staged_rows_to_a_split3(W.qs, t, qf);
+    wg_barrier(bar);   // the staging buffer is free
+    auto k_desc = [&](int kb_) {
+      return [&, kb_](int sp, int kk) { return b_desc_ex(k_saddr + (kb_ * 3 + sp) * AT_CHUNK_BYTES + kk * 256, 128, 1024); };
+    };
+    // ---------------- pass 1: row maxima (hi-only S) ----------------------------------------------------------------
+    float mx[2] = {-INFINITY, -INFINITY};
+    for (int c = 0; c < cur.nchunks; ++c) {
+      const int kb_ = consume(W.k_bar, kcons);
+      // next in the K stream: chunk c + 1, or the first chunk of pass 2
+      fill(W.k, W.k_bar, kfill, k_g, cur.blk_lo + (c + 1 < cur.nchunks ? 8 * (c + 1) : 0));
+      float s[32];
+      wg_gemm6_rs_issue<64, 4, 0, true>(s, qf, k_desc(kb_), false);
+      look_ahead();
+      wg_mma_wait(s);
+      const int key0 = (cur.blk_lo + 8 * c) * 8 + fc;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int kn = key0 + 8 * j + e;
+          const bool ok = kn >= cur.j0 && kn < cur.j1;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) mx[h] = fmaxf(mx[h], ok ? s[4 * j + 2 * h + e] : -INFINITY);
+        }
+      wg_barrier(bar);   // K buffer kb_ read and its phase observed by every thread
+    }
+    look_ahead();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+    }
+    // ---------------- pass 2: P = exp(S - max), O += P V ------------------------------------------------------------
+    float lh[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [fragment row][32-key half]: the row-per-thread code's per-half sums
+    float o_acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
+    if (cur.nchunks > 0 && !v_ahead) fill(W.v, W.v_bar, vfill, v_g, cur.blk_lo);
+    for (int c = 0; c < cur.nchunks; ++c) {
+      const int kb_ = consume(W.k_bar, kcons);
+      const bool last = c + 1 == cur.nchunks;
+      if (!last) {
+        fill(W.k, W.k_bar, kfill, k_g, cur.blk_lo + 8 * (c + 1));
+        fill(W.v, W.v_bar, vfill, v_g, cur.blk_lo + 8 * (c + 1));
+      } else if (ktn >= 0 && nxt.nchunks > 0) {   // the next tile's first chunks
+        fill(W.k, W.k_bar, kfill, k_g, nxt.blk_lo);
+        fill(W.v, W.v_bar, vfill, v_g, nxt.blk_lo);
+      }
+      float s[32];
+      wg_gemm6_rs_issue<64, 4>(s, qf, k_desc(kb_), false);
+      wg_mma_wait(s);
+      const int key0 = (cur.blk_lo + 8 * c) * 8 + fc;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int kn = key0 + 8 * j + e;
+          const bool ok = kn >= cur.j0 && kn < cur.j1;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float& x = s[4 * j + 2 * h + e];
+            x = ok ? expf(x - mx[h]) : 0.f;
+          }
+        }
+      {  // l: four chains per 32-key half, (l0 + l1) + (l2 + l3), added to the half's running sum
+        float ps[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) ps[i] = __shfl_xor_sync(0xffffffffu, s[i], 2);
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int ch = 0; ch < 2; ++ch) {
+            float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+            for (int c4 = 0; c4 < 8; ++c4) {
+              s0 = __fadd_rn(s0, chain_val(s, ps, h, ch, c4, 0));
+              s1 = __fadd_rn(s1, chain_val(s, ps, h, ch, c4, 1));
+            }
+            const float sp = __fadd_rn(s0, s1);
+            lh[h][ch] = __fadd_rn(lh[h][ch], __fadd_rn(sp, __shfl_xor_sync(0xffffffffu, sp, 1)));
+          }
+      }
+      unsigned pf[3][4][4];
+      acc_to_a_split3<4>(s, pf);
+      const int vb_ = consume(W.v_bar, vcons);
+      float o[32];
+      wg_gemm6_rs_issue<64, 4, 1>(o, pf, [&](int sp, int kk) {
+        return b_desc_ex(v_saddr + (vb_ * 3 + sp) * AT_CHUNK_BYTES + kk * 2048, 1024, 128); }, false);
+      wg_mma_wait(o);
+      // The tensor core truncates (round-toward-zero) every time it adds into an fp32 accumulator, a systematic bias that
+      // grows with the number of accumulation steps; each 64-key chunk is therefore accumulated on its own (4
+      // full-magnitude steps) and the chunks are summed here with round-to-nearest FADDs.
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o_acc[i] = __fadd_rn(o_acc[i], o[i]);
+      wg_barrier(bar);   // K buffer kb_ and V buffer vb_ read and their phases observed by every thread
+    }
+    k_ahead = v_ahead = ktn >= 0 && nxt.nchunks > 0 && cur.nchunks > 0;
+    // ---------------- mu = O / l --------------------------------------------------------------------------------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float l = __fadd_rn(lh[h][0], lh[h][1]);
+      const float inv = l > 0.f ? 1.f / l : 0.f;
+      const int row = fr0 + 8 * h;
+      if (row < cur.nvalid) {
+        float* dst = mu + (long)(cur.node0 + row) * EQD_HID + fc;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o_acc[4 * j + 2 * h] * inv, o_acc[4 * j + 2 * h + 1] * inv);
+      }
+    }
+    kt = ktn;
+    cur = nxt;
+  }
+  cp_async_wait<0>();
+  TRACE_END(1);
+}
+
 }  // namespace eqd
 
 EQD_TRACE_SETTER(eqd_trace_set_attn)
@@ -301,29 +527,33 @@ extern "C" int eqd_attn_prof_read(long long* out16) {
 }
 #endif
 
-template <bool X5>
-static int launch_attention_tc(const eqd_graph* g, const float* proj, int pw, const void* kv, const float* x5, float* mu,
-                               int ldmu, void* stream) {
-  if (reinterpret_cast<uintptr_t>(kv) & 15) return EQD_ERR_BAD_ARG;
-  if (g->n_node_tiles <= 0) return EQD_OK;
-  size_t smem = sizeof(eqd::AtSmem<X5>) + 128;
-  EQD_SET_SMEM((eqd::attention_tc_kernel<X5>), smem);
-  int grid = g->n_node_tiles < EQD_SMS ? g->n_node_tiles : EQD_SMS;
-  long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
-  eqd::attention_tc_kernel<X5><<<grid, AT_THREADS, smem, (cudaStream_t)stream>>>(
-      *g, proj, pw, reinterpret_cast<const unsigned char*>(kv), split_stride, x5, mu, ldmu);
-  EQD_CUDA_LAUNCH_CHECK();
-  return EQD_OK;
-}
-
 extern "C" int eqd_attention_tc(const eqd_graph* g, const float* proj, const void* kv, float* mu, void* stream) {
   if (!g || !proj || !kv || !mu) return EQD_ERR_BAD_ARG;
-  return launch_attention_tc<false>(g, proj, 320, kv, nullptr, mu, EQD_HID, stream);
+  if (reinterpret_cast<uintptr_t>(kv) & 15) return EQD_ERR_BAD_ARG;
+  if (g->n_node_tiles <= 0) return EQD_OK;
+  const size_t smem = AT_CHAINS * sizeof(eqd::AtChainSmem);
+  EQD_SET_SMEM(eqd::attention64_tc_kernel, smem);
+  const int nht = 2 * g->n_node_tiles;
+  int grid = (nht + AT_CHAINS - 1) / AT_CHAINS;
+  if (grid > EQD_SMS) grid = EQD_SMS;
+  const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
+  eqd::attention64_tc_kernel<<<grid, AT_CHAINS * 128, smem, (cudaStream_t)stream>>>(
+      *g, proj, reinterpret_cast<const unsigned char*>(kv), split_stride, mu);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
 }
 
 extern "C" int eqd_attention_tc0(const eqd_graph* g, const float* proj, const void* kv, const float* x5, float* mu,
                                  void* stream) {
   if (!g || !proj || !kv || !x5 || !mu) return EQD_ERR_BAD_ARG;
-  if (reinterpret_cast<uintptr_t>(x5) & 15) return EQD_ERR_BAD_ARG;
-  return launch_attention_tc<true>(g, proj, 128 + 3 * 72, kv, x5, mu, EQD_H0_PAD, stream);
+  if ((reinterpret_cast<uintptr_t>(kv) | reinterpret_cast<uintptr_t>(x5)) & 15) return EQD_ERR_BAD_ARG;
+  if (g->n_node_tiles <= 0) return EQD_OK;
+  const size_t smem = sizeof(eqd::AtSmem) + 128;
+  EQD_SET_SMEM(eqd::attention0_tc_kernel, smem);
+  const int grid = g->n_node_tiles < EQD_SMS ? g->n_node_tiles : EQD_SMS;
+  const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
+  eqd::attention0_tc_kernel<<<grid, AT_THREADS, smem, (cudaStream_t)stream>>>(
+      *g, proj, 128 + 3 * 72, reinterpret_cast<const unsigned char*>(kv), split_stride, x5, mu, EQD_H0_PAD);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
 }

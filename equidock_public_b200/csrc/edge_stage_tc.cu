@@ -60,17 +60,6 @@ struct TcSmem {
   unsigned long long w_bar;
 };
 
-// The row statistics (LayerNorm, phi) keep the summation order of a row-per-thread epilogue: per 32-column half ch of
-// the row, chain k = 0..3 adds the columns 32 ch + 4 c4 + k for c4 = 0..7 in turn.  In the accumulator layout lane c of a
-// quad holds the columns 8 j + 2 c + e (e = 0, 1), so chain k = 2 (c & 1) + e alternates between lane c and lane c ^ 2;
-// each lane runs its two chains from its own values v and those of lane c ^ 2 (pv), and lane c ^ 1 runs the other two.
-// Returns term c4 of chain 2 (lane & 1) + e of fragment row h (row g + 8 h).
-__device__ __forceinline__ float chain_val(const float (&v)[32], const float (&pv)[32], int h, int ch, int c4, int e) {
-  const int i = 4 * (4 * ch + (c4 >> 1)) + 2 * h + e;
-  const bool own = ((c4 & 1) == 0) == ((threadIdx.x & 2) == 0);
-  return own ? v[i] : pv[i];
-}
-
 __global__ void __launch_bounds__(TC_THREADS, 1)
 edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ EdgeConsts cst_p,
                      const float* __restrict__ proj, const double* __restrict__ x_in, const double* __restrict__ x_orig,

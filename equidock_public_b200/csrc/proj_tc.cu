@@ -5,7 +5,8 @@
 //   kv[which][split][n/8][d/8][n%8][d%8]   (1 KB per 8 nodes; a run of blocks is a ready wgmma B operand).
 // Weight-stationary: the bf16x3 panels (120 KB; 158 KB for the K = 80 layer 0) sit in shared memory for the life of
 // the CTA next to the tile's A operand and its fp32 result tile; 2 threads per node row, one 64-row warpgroup slab per
-// 128 threads (layer 0 takes 64-row tiles: its larger panels leave room for no more).
+// 128 threads (layer 0 takes 64-row tiles: its larger panels leave room for no more).  eqd_project_tc (the 64-wide
+// layers) runs project64_tc_kernel below.
 #include "tc_common.cuh"
 
 namespace eqd {
@@ -170,6 +171,137 @@ project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjCon
   TRACE_END(2);
 }
 
+// ---- the 64-wide layers ---------------------------------------------------------------------------------------------
+// One persistent CTA of two warpgroups per SM sharing the resident 120 KB panels.  Each warpgroup runs its own chain of
+// 64-row tiles and synchronises only inside itself (its named barrier).  Per tile: the h rows, cp.async'ed into the
+// chain's staging buffer during the previous tile, become bf16x3 RS A fragments once; the five N = 64 groups run as RS
+// wgmma on them, group g + 1 issued before group g's epilogue (bias, LeakyReLU on the accumulator fragments).  Psrc | Pdst
+// | Q (and K | V without K/V blocks) leave through the chain's staging tile as whole 256-byte rows; K and V go straight from
+// the fragments into the 8-node kv blocks (a quad writes 16 contiguous bytes of a block row, a warp 8 whole block rows).
+// Every output element takes the split, products, order and epilogue of the 128-row kernel it replaces.
+#define PJ_CHAINS 2
+#define PJ64_W_BYTES (5 * PjCfg<false>::GROUP_BYTES)
+#define PJ_OUT_LD 72   // fp32 row stride of the output staging tile (72 % 32 = 8: the fragment stores are conflict-free)
+
+struct __align__(128) PjChainSmem {
+  float hs[64 * 64];              // h rows of the next tile (16-byte chunks swizzled, staged_rows_to_a_split3)
+  float out[64 * PJ_OUT_LD];      // one group's outputs on their way to proj
+};
+struct Pj64Smem {
+  unsigned char w[PJ64_W_BYTES];
+  PjChainSmem ch[PJ_CHAINS];
+  float b[320];
+  unsigned long long w_bar;
+};
+
+__global__ void __launch_bounds__(PJ_CHAINS * 128, 1)
+project64_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjConsts cst, const float* __restrict__ h,
+                    float* __restrict__ proj, unsigned char* __restrict__ kv, long kv_split_stride) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  Pj64Smem& S = *reinterpret_cast<Pj64Smem*>(smem_raw);
+  const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, lane = t & 31;
+  PjChainSmem& W = S.ch[wgi];
+  const int bar = 1 + wgi;   // this chain's named barrier
+  const int ntiles = (n_nodes + 63) / 64, tstride = gridDim.x * PJ_CHAINS;
+  TRACE_START(2);
+  if (tid == 0) {
+    mbar_init(&S.w_bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_expect_tx(&S.w_bar, PJ64_W_BYTES);
+    bulk_g2s(S.w, p.w_proj_tc, PJ64_W_BYTES, &S.w_bar);
+  }
+  for (int i = tid; i < 320; i += PJ_CHAINS * 128) S.b[i] = cst.b[i];
+  __syncthreads();
+  const unsigned w_saddr = smem_u32(S.w);
+  const float slope = p.leaky_slope;
+  // accumulator-fragment rows of this thread: fr0 and fr0 + 8; columns 8 j + fc + {0, 1}, j = 0..7
+  const int fr0 = (t >> 5) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+  auto stage_h = [&](int tile) { stage_rows64(W.hs, h, EQD_HID, 0, (long)tile * 64, min(64, n_nodes - tile * 64), t); };
+  int tile = blockIdx.x * PJ_CHAINS + wgi;
+  if (tile < ntiles) stage_h(tile);
+  mbar_wait(&S.w_bar, 0);
+
+  for (; tile < ntiles; tile += tstride) {
+    if (t == 0) TRACE_PHASE(2, blockIdx.x * PJ_CHAINS + wgi, tile, 1);
+    const int node0 = tile * 64, nvalid = min(64, n_nodes - node0);
+    cp_async_wait<0>();
+    wg_barrier(bar);   // this tile's h rows have landed
+    unsigned af[3][4][4];
+    staged_rows_to_a_split3(W.hs, t, af);
+    wg_barrier(bar);   // the staging buffer is free
+    if (tile + tstride < ntiles) stage_h(tile + tstride);
+    auto group = [&](int grp) {
+      return [&, grp](int s, int kb) { return b_desc_ex(w_saddr + grp * PjCfg<false>::GROUP_BYTES + s * PjCfg<false>::SPLIT_BYTES + kb * 2048, 1024, 128); };
+    };
+    float acc[2][32];
+    wg_gemm6_rs_issue<64, 4>(acc[0], af, group(0), false);
+#pragma unroll
+    for (int grp = 0; grp < 5; ++grp) {
+      float (&d)[32] = acc[grp & 1];
+      if (grp + 1 < 5) {
+        wg_gemm6_rs_issue<64, 4>(acc[(grp + 1) & 1], af, group(grp + 1), false);
+        wg_mma_wait<1>(d);
+      } else {
+        wg_mma_wait(d);
+      }
+      const bool act = (grp == 2 || grp == 3);        // Q, K carry the LeakyReLU
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 bj = *reinterpret_cast<const float2*>(&S.b[grp * 64 + 8 * j + fc]);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          float& x0 = d[4 * j + 2 * hh];
+          float& x1 = d[4 * j + 2 * hh + 1];
+          x0 = x0 + bj.x;
+          x1 = x1 + bj.y;
+          if (act) {
+            x0 = lrelu(x0, slope);
+            x1 = lrelu(x1, slope);
+          }
+        }
+      }
+      if (grp < 3 || kv == nullptr) {   // with K/V blocks requested nobody reads the fp32 K / V columns
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+            *reinterpret_cast<float2*>(W.out + (fr0 + 8 * hh) * PJ_OUT_LD + 8 * j + fc) =
+                make_float2(d[4 * j + 2 * hh], d[4 * j + 2 * hh + 1]);
+        wg_barrier(bar);
+        // 16 lanes per 256-byte row, 8 rows per pass
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          const int row = i * 8 + (t >> 4), c4 = t & 15;
+          if (row < nvalid)
+            *reinterpret_cast<float4*>(proj + (long)(node0 + row) * 320 + grp * 64 + 4 * c4) =
+                *reinterpret_cast<const float4*>(W.out + row * PJ_OUT_LD + 4 * c4);
+        }
+        wg_barrier(bar);   // the staging tile is free for the next group
+      } else {
+        // kv[which][split][n/8][d/8][n%8][d%8]: channels (8 j + fc, + 1) of a row are one 4-byte word per split
+        unsigned char* base = kv + (long)(grp - 3) * 3 * kv_split_stride;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = fr0 + 8 * hh, node = node0 + row;
+          if (row < nvalid) {
+            unsigned char* nb = base + (long)(node >> 3) * 1024 + (node & 7) * 16 + fc * 2;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              unsigned w0, w1, w2;
+              split3_pair(d[4 * j + 2 * hh], d[4 * j + 2 * hh + 1], w0, w1, w2);
+              *reinterpret_cast<unsigned*>(nb + j * 128) = w0;
+              *reinterpret_cast<unsigned*>(nb + kv_split_stride + j * 128) = w1;
+              *reinterpret_cast<unsigned*>(nb + 2 * kv_split_stride + j * 128) = w2;
+            }
+          }
+        }
+      }
+    }
+  }
+  cp_async_wait<0>();
+  TRACE_END(2);
+}
+
 // fp32 K / V columns of a projection buffer -> bf16x3 8-node blocks (used after the FFMA layer-0 node stage)
 __global__ void kv_blocks_kernel(int n_nodes, const float* __restrict__ proj, int pw, int koff, int voff,
                                  unsigned char* __restrict__ kv, long kv_split_stride) {
@@ -221,7 +353,22 @@ extern "C" int eqd_project_tc(const eqd_graph* g, const eqd_layer* p_l, const fl
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !h || !proj) return EQD_ERR_BAD_ARG;
   if (p->dh != 64 || p->dhp != 64) return EQD_ERR_UNSUPPORTED;
-  return launch_project_tc<false>(g, p_l, h, EQD_HID, proj, 320, kv, nullptr, stream);
+  if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
+  if (!p->w_proj_tc || (reinterpret_cast<uintptr_t>(p->w_proj_tc) & 15)) return EQD_ERR_BAD_ARG;
+  if (g->n_nodes <= 0) return EQD_OK;
+  eqd::PjConsts cst;
+  memset(&cst, 0, sizeof(cst));
+  memcpy(&cst, p_l->consts.proj_bias, 320 * sizeof(float));
+  const int ntiles = (g->n_nodes + 63) / 64;
+  const size_t smem = sizeof(eqd::Pj64Smem) + 128;
+  EQD_SET_SMEM(eqd::project64_tc_kernel, smem);
+  int grid = (ntiles + PJ_CHAINS - 1) / PJ_CHAINS;
+  if (grid > EQD_SMS) grid = EQD_SMS;
+  const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
+  eqd::project64_tc_kernel<<<grid, PJ_CHAINS * 128, smem, (cudaStream_t)stream>>>(
+      g->n_nodes, *p, cst, h, proj, reinterpret_cast<unsigned char*>(kv), split_stride);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
 }
 
 extern "C" int eqd_project_tc0(const eqd_graph* g, const eqd_layer* p_l, const float* h0, float* proj, void* kv,

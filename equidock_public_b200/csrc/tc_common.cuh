@@ -125,10 +125,11 @@ __device__ __forceinline__ void wg_gemm6_issue(float (&d)[N / 2], AD a_desc, BD 
     }
   asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-// waits for every MMA group of the warpgroup; the accumulators handed in are not touched before it
-template <int M>
+// waits until at most PENDING of the warpgroup's MMA groups (the most recently committed) are in flight; the accumulators
+// handed in (those of an older group) are not touched before it
+template <int PENDING = 0, int M>
 __device__ __forceinline__ void wg_mma_wait(float (&d)[M]) {
-  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory");
 #pragma unroll
   for (int i = 0; i < M; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
@@ -138,15 +139,15 @@ __device__ __forceinline__ void wg_gemm6(float (&d)[N / 2], AD a_desc, BD b_desc
   wg_gemm6_issue<N, TB>(d, a_desc, b_desc, kblocks, accumulate, hi_only);
   asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
-// wg_gemm6_issue with A from registers: a[split][kb] are the bf16x3 A fragments (acc_to_a_split3), same product order.
-// Returns with the MMAs in flight (wg_mma_wait).
-template <int N, int KB, int TB = 0, class BD>
+// wg_gemm6_issue with A from registers: a[split][kb] are the bf16x3 A fragments (acc_to_a_split3), same product order;
+// HI_ONLY: just the leading bf16 x bf16 product.  Returns with the MMAs in flight (wg_mma_wait).
+template <int N, int KB, int TB = 0, bool HI_ONLY = false, class BD>
 __device__ __forceinline__ void wg_gemm6_rs_issue(float (&d)[N / 2], const unsigned (&a)[3][KB][4], BD b_desc, bool accumulate) {
   constexpr int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
   int scale_d = accumulate ? 1 : 0;
 #pragma unroll
-  for (int pr = 0; pr < 6; ++pr)
+  for (int pr = HI_ONLY ? 5 : 0; pr < 6; ++pr)
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb) {
       WgmmaRS<N, TB>::mma(d, a[pa[pr]][kb], b_desc(pb[pr], kb), scale_d);
@@ -226,6 +227,42 @@ __device__ __forceinline__ void acc_to_a_split3(const float (&v)[8 * KB], unsign
   for (int kb = 0; kb < KB; ++kb)
 #pragma unroll
     for (int i = 0; i < 4; ++i) split3_pair(v[8 * kb + 2 * i], v[8 * kb + 2 * i + 1], a[0][kb][i], a[1][kb][i], a[2][kb][i]);
+}
+// bf16x3 RS A fragments (k = 64 channels, 4 k-blocks) of warpgroup thread t from 64 fp32 rows of 64 channels staged in
+// shared memory by 16-byte chunks, chunk k4 of row r at position k4 ^ stage_swz(r) (the fragment loads are then free of
+// bank conflicts).  Same split as acc_to_a_split3 on the same values.
+__device__ __forceinline__ int stage_swz(int row) { return (row & 3) << 1; }
+// Columns [col0, col0 + 64) of rows row0 .. row0 + 63 of a [n][ld] fp32 array -> that staging layout by cp.async (one
+// commit group; rows from nvalid on are zero-filled), issued by the 128 threads t of a warpgroup, 16 lanes per row.
+__device__ __forceinline__ void stage_rows64(float* rows, const float* src, int ld, int col0, long row0, int nvalid, int t) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int idx = i * 128 + t, row = idx >> 4, k4 = idx & 15;
+    const bool ok = row < nvalid;
+    cp_async16(rows + row * 64 + ((k4 ^ stage_swz(row)) << 2), src + (row0 + (ok ? row : 0)) * ld + col0 + 4 * k4, ok);
+  }
+  cp_async_commit();
+}
+__device__ __forceinline__ void staged_rows_to_a_split3(const float* rows, int t, unsigned (&a)[3][4][4]) {
+  const int g = (t >> 5) * 16 + ((t & 31) >> 2), c = t & 3;
+#pragma unroll
+  for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int row = g + 8 * (i & 1), k4 = 4 * kb + 2 * (i >> 1) + (c >> 1);
+      const float2 v = *reinterpret_cast<const float2*>(rows + row * 64 + ((k4 ^ stage_swz(row)) << 2) + 2 * (c & 1));
+      split3_pair(v.x, v.y, a[0][kb][i], a[1][kb][i], a[2][kb][i]);
+    }
+}
+// Row statistics in the summation order of a row-per-thread epilogue: per 32-column half ch of the row, chain k = 0..3 adds
+// the columns 32 ch + 4 c4 + k for c4 = 0..7 in turn.  In the accumulator layout lane c of a quad holds the columns
+// 8 j + 2 c + e (e = 0, 1), so chain k = 2 (c & 1) + e alternates between lane c and lane c ^ 2; each lane runs its two
+// chains from its own values v and those of lane c ^ 2 (pv), and lane c ^ 1 runs the other two.
+// Returns term c4 of chain 2 (lane & 1) + e of fragment row h (row g + 8 h).
+__device__ __forceinline__ float chain_val(const float (&v)[32], const float (&pv)[32], int h, int ch, int c4, int e) {
+  const int i = 4 * (4 * ch + (c4 >> 1)) + 2 * h + e;
+  const bool own = ((c4 & 1) == 0) == ((threadIdx.x & 2) == 0);
+  return own ? v[i] : pv[i];
 }
 // barrier of one warpgroup (128 threads) on named barrier `id`; the _and form also returns whether pred holds on all
 __device__ __forceinline__ void wg_barrier(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
