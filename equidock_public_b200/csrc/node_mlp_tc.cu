@@ -1,8 +1,7 @@
 // Node MLP of a 64-wide IEGMN layer (rigid_docking_model.py:319-337) on the tensor cores (wgmma, bf16x6):
 //   h' = skip( W6 . LayerNorm(LeakyReLU(W5 . [h | aggr_msg | mu | h0] + b5)) + b6 )
-// Weight-stationary (W5: 64x272, W6: 64x64 as bf16x3 panels, 126 KB in shared memory); one tile of 128 node rows per
-// CTA of 256 threads at a time (2 threads per node row, two 64-row warpgroup slabs in the GEMMs).  The 272-wide input
-// is fed in 5 K-pieces; the A operand region takes each piece's fp32 result tile once its MMAs are complete.
+// Weight-stationary: W5 (64 x 272) and W6 (64 x 64) as bf16x3 panels, 126 KB in shared memory for the life of the CTA.
+// node_mlp_tc_kernel (the 64-wide layers) runs warpgroup tile chains; node_mlp0_tc_kernel (layer 0) 128-row tiles.
 #include "tc_common.cuh"
 
 namespace eqd {
@@ -12,29 +11,40 @@ namespace eqd {
 #define NM_W6_BASE 104448
 #define NM_W6_SPLIT 8192
 #define NM_W_BYTES 129024
-#define NM_A_SPLIT 16384    // A operand: 128 rows x 64 bf16 per split
-#define NM_LD 68            // fp32 row stride of the result tile
 
 struct NmConsts { float b5[64], ln_g[64], ln_b[64], b6[64]; };
 
-#define NM_SC_LD 36   // padded row stride (floats) of a warp's 32 x 32 transposition scratch: conflict-free both ways
+// ---- the 64-wide layers -------------------------------------------------------------------------------------------------
+// One persistent CTA of NM_CHAINS warpgroups per SM sharing the resident panels.  Each warpgroup runs its own chain of
+// 64-row tiles and synchronises only inside itself (its named barrier).  The 272-wide input of node_mlp.0 arrives in five
+// K-pieces: h, aggr, mu and h0[0:64] stream through the chain's ring of NM_SLOTS staging buffers by cp.async, two pieces
+// ahead of their use and across tile boundaries, and each becomes bf16x3 RS A fragments; h0[64:72] plus 8 zero channels
+// (one k-block) is read from global memory straight into A fragments.  Each piece is a fresh accumulation summed into the
+// accumulator fragments with round-to-nearest adds.  Bias, LeakyReLU and the LayerNorm run on the fragments (row
+// statistics over the quad, in the chain order of a row-per-thread epilogue), which then feed node_mlp.4 as RS A
+// fragments; the skip line takes h from the registers of piece 0 and h' leaves by direct fragment stores (a quad writes
+// 32 contiguous bytes of a row).  Every element of h' takes the splits, products, order and epilogue of the 128-row kernel
+// this one replaced, with the same multiply-add contraction (pinned below with the _rn intrinsics).
+#define NM_CHAINS 2
+#define NM_SLOTS 3   // staging buffers per chain: pieces are issued NM_SLOTS - 1 ahead
 
 struct NmSmem {
   unsigned char w[NM_W_BYTES];
-  unsigned char a[3 * NM_A_SPLIT];
-  float sc[NM_THREADS / 32][32 * NM_SC_LD];   // one 32-row x 128-byte scratch per warp (its rows x its column half)
-  float red[EQD_TM * 4];
+  float stage[NM_CHAINS][NM_SLOTS][64 * 64];   // 64 rows x 64 channels of a piece (16-byte chunks swizzled, stage_rows64)
+  float c[256];                                // b5 | ln_g | ln_b | b6
   unsigned long long w_bar;
 };
 
-__global__ void __launch_bounds__(NM_THREADS, 1)
+__global__ void __launch_bounds__(NM_CHAINS * 128, 1)
 node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmConsts cst, const float* __restrict__ h_in,
                    const float* __restrict__ aggr, const float* __restrict__ mu, const float* __restrict__ h0,
                    float* __restrict__ h_out) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   NmSmem& S = *reinterpret_cast<NmSmem*>(smem_raw);
-  const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, warp = tid >> 5, wgi = tid >> 7;
-  const int ntiles = (n_nodes + EQD_TM - 1) / EQD_TM;
+  const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, lane = t & 31;
+  float (&ring)[NM_SLOTS][64 * 64] = S.stage[wgi];
+  const int bar = 1 + wgi;   // this chain's named barrier
+  const int ntiles = (n_nodes + 63) / 64, tstride = gridDim.x * NM_CHAINS, tile0 = blockIdx.x * NM_CHAINS + wgi;
   TRACE_START(3);
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
@@ -42,152 +52,161 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
     mbar_expect_tx(&S.w_bar, NM_W_BYTES);
     bulk_g2s(S.w, p.w_node_tc, NM_W_BYTES, &S.w_bar);
   }
+  for (int i = tid; i < 256; i += NM_CHAINS * 128) S.c[i] = reinterpret_cast<const float*>(&cst)[i];
   __syncthreads();
-  const unsigned w_saddr = smem_u32(S.w), a_saddr = smem_u32(S.a);
-  float* const dtile = reinterpret_cast<float*>(S.a);
-  auto a_desc = [&](int sp, int kb) { return a_desc_at<EQD_TM>(a_saddr, NM_A_SPLIT, wgi, sp, kb); };
-  mbar_wait(&S.w_bar, 0);
-  const float slope = p.leaky_slope;
-  float* red = S.red;
+  const unsigned w_saddr = smem_u32(S.w);
+  const float slope = p.leaky_slope, sk = p.skip_weight_h, sk1 = 1.f - p.skip_weight_h;
+  // accumulator-fragment rows of this thread: fr0 and fr0 + 8; columns 8 j + fc + {0, 1}, j = 0..7
+  const int fr0 = (t >> 5) * 16 + (lane >> 2), fc = 2 * (lane & 3);
 
-  // The A operand in place (callers fence + barrier first) times K-blocks [0, nkb) of the panel at w_off -> out (my row
-  // half of the fresh product); on return the A region is free again.
-  auto gemm = [&](unsigned w_off, unsigned w_split, int nkb, float (&out)[32]) {
+  // piece q of the chain's stream: piece q & 3 (h, aggr, mu, h0[0:64]) of its tile number q >> 2, into slot q % NM_SLOTS;
+  // one commit group per piece (empty past the last tile), so cp_async_wait<NM_SLOTS - 2> waits for piece q alone
+  auto issue = [&](int q) {
+    const int tile = tile0 + (q >> 2) * tstride, pc = q & 3;
+    if (tile < ntiles) {
+      const float* src = pc == 0 ? h_in : pc == 1 ? aggr : pc == 2 ? mu : h0;
+      stage_rows64(ring[q % NM_SLOTS], src, pc == 3 ? EQD_H0_PAD : EQD_HID, 0, (long)tile * 64, min(64, n_nodes - tile * 64), t);
+    } else {
+      cp_async_commit();
+    }
+  };
+  int q = 0;
+  for (int i = 0; i < NM_SLOTS - 1; ++i) issue(i);
+  mbar_wait(&S.w_bar, 0);
+
+  for (int tile = tile0; tile < ntiles; tile += tstride) {
+    if (t == 0) TRACE_PHASE(3, blockIdx.x * NM_CHAINS + wgi, tile, 1);
+    const int node0 = tile * 64, nvalid = min(64, n_nodes - node0);
+    // piece 4 (h0[64:72]): A registers 0, 1 of the k-block = channels 64 + fc + {0, 1} of rows fr0, fr0 + 8
+    float2 x4[2];
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = fr0 + 8 * hh;
+      x4[hh] = row < nvalid ? *reinterpret_cast<const float2*>(h0 + (long)(node0 + row) * EQD_H0_PAD + 64 + fc)
+                            : make_float2(0.f, 0.f);
+    }
+    // ---- node_mlp.0 over [h | aggr | mu | h0] in 5 K-pieces ---------------------------------------------------------
+    float acc[32], hs[32];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float2 bj = *reinterpret_cast<const float2*>(&S.c[8 * j + fc]);
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        acc[4 * j + 2 * hh] = bj.x;
+        acc[4 * j + 2 * hh + 1] = bj.y;
+      }
+    }
+#pragma unroll 1   // unrolled, ptxas serialises the wgmmas (C7511: too few registers for the pipeline)
+    for (int pc = 0; pc < 4; ++pc, ++q) {
+      cp_async_wait<NM_SLOTS - 2>();
+      wg_barrier(bar);   // piece q has landed, and every thread is done with piece q - 1's slot
+      issue(q + NM_SLOTS - 1);
+      float v[32];
+      staged_rows_to_frag(ring[q % NM_SLOTS], t, v);
+      if (pc == 0) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) hs[i] = v[i];   // the skip operand
+      }
+      unsigned af[3][4][4];
+      acc_to_a_split3<4>(v, af);
+      float d[32];
+      wg_gemm6_rs_issue<64, 4>(d, af, [&](int sp, int kb) {
+        return b_desc_ex(w_saddr + (4 * pc + kb) * 2048 + sp * NM_W5_SPLIT, 1024, 128); }, false);
+      wg_mma_wait(d);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[i] = __fadd_rn(acc[i], d[i]);
+    }
+    {
+      unsigned a4[3][1][4];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) split3_pair(x4[hh].x, x4[hh].y, a4[0][0][hh], a4[1][0][hh], a4[2][0][hh]);
+#pragma unroll
+      for (int sp = 0; sp < 3; ++sp) a4[sp][0][2] = a4[sp][0][3] = 0u;
+      float d[32];
+      wg_gemm6_rs_issue<64, 1>(d, a4, [&](int sp, int kb) {
+        return b_desc_ex(w_saddr + 16 * 2048 + sp * NM_W5_SPLIT, 1024, 128); }, false);
+      wg_mma_wait(d);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[i] = __fadd_rn(acc[i], d[i]);
+    }
+    // ---- LeakyReLU, LayerNorm -> bf16x3 A fragments ; node_mlp.4 ----------------------------------------------------
+    unsigned af[3][4][4];
+    {
+      float (&v)[32] = acc;
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = fmaxf(v[i], __fmul_rn(v[i], slope));
+      // per 32-column half ch, two-pass (mean_ch, M2_ch) over four chains, then the Chan et al. combination
+      // mean = (m0 + m1) / 2, M2 = M2_0 + M2_1 + (m0 - m1)^2 * 16
+      float pv[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) pv[i] = __shfl_xor_sync(0xffffffffu, v[i], 2);
+      float msum[2], rstd[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float mh[2], qh[2];
+#pragma unroll
+        for (int ch = 0; ch < 2; ++ch) {
+          float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+          for (int c4 = 0; c4 < 8; ++c4) {
+            s0 = __fadd_rn(s0, chain_val(v, pv, h, ch, c4, 0));
+            s1 = __fadd_rn(s1, chain_val(v, pv, h, ch, c4, 1));
+          }
+          const float sp = __fadd_rn(s0, s1);
+          mh[ch] = __fmul_rn(__fadd_rn(sp, __shfl_xor_sync(0xffffffffu, sp, 1)), 1.f / 32.f);
+          float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+          for (int c4 = 0; c4 < 8; ++c4) {
+            const float d0 = __fadd_rn(chain_val(v, pv, h, ch, c4, 0), -mh[ch]);
+            const float d1 = __fadd_rn(chain_val(v, pv, h, ch, c4, 1), -mh[ch]);
+            q0 = __fmaf_rn(d0, d0, q0);
+            q1 = __fmaf_rn(d1, d1, q1);
+          }
+          const float qp = __fadd_rn(q0, q1);
+          qh[ch] = __fadd_rn(qp, __shfl_xor_sync(0xffffffffu, qp, 1));
+        }
+        msum[h] = __fadd_rn(mh[0], mh[1]);
+        const float dm = __fadd_rn(mh[0], -mh[1]);
+        const float var = __fmaf_rn(__fmul_rn(dm, dm), 16.f, __fadd_rn(qh[0], qh[1]));
+        rstd[h] = 1.f / sqrtf(__fmaf_rn(var, 1.f / 64.f, 1e-5f));
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 gj = *reinterpret_cast<const float2*>(&S.c[64 + 8 * j + fc]);
+        const float2 bj = *reinterpret_cast<const float2*>(&S.c[128 + 8 * j + fc]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {   // v - mean as v - 0.5 (m0 + m1) in one rounding
+          float& x0 = v[4 * j + 2 * h];
+          float& x1 = v[4 * j + 2 * h + 1];
+          x0 = __fmaf_rn(__fmul_rn(__fmaf_rn(msum[h], -0.5f, x0), rstd[h]), gj.x, bj.x);
+          x1 = __fmaf_rn(__fmul_rn(__fmaf_rn(msum[h], -0.5f, x1), rstd[h]), gj.y, bj.y);
+        }
+      }
+      acc_to_a_split3<4>(v, af);
+    }
     {
       float d[32];
-      wg_gemm6<64>(d, a_desc, [&](int sp, int kb) { return b_desc_ex(w_saddr + w_off + sp * w_split + kb * 2048, 1024, 128); },
-                   nkb, false);
-      __syncthreads();
-      wg_store_d<64>(dtile + wgi * 64 * NM_LD, NM_LD, d, tid & 127);
-    }
-    __syncthreads();
-    tile_ld32f(dtile, NM_LD, r, half * 32, out);
-    __syncthreads();
-  };
-
-  // Global rows travel coalesced: the warp's 32 rows x 128 bytes (its column half) are cp.async'ed into its scratch,
-  // 8 lanes per row, one piece ahead of its use; each thread then picks up its own row.
-  const int lane = tid & 31, wrow0 = 32 * (warp & 3);
-  float* sc = S.sc[warp];
-  auto fetch = [&](const float* base, int ld, int t) {
-    if (t >= ntiles) return;
+      wg_gemm6_rs_issue<64, 4>(d, af, [&](int sp, int kb) {
+        return b_desc_ex(w_saddr + NM_W6_BASE + sp * NM_W6_SPLIT + kb * 2048, 1024, 128); }, false);
+      wg_mma_wait(d);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int row = i * 4 + (lane >> 3);
-      const long nd = (long)t * EQD_TM + wrow0 + row;
-      const bool ok = nd < n_nodes;   // src-size 0 zero-fills
-      cp_async16(sc + row * NM_SC_LD + (lane & 7) * 4, base + (ok ? nd : 0) * ld + half * 32 + (lane & 7) * 4, ok);
-    }
-    cp_async_commit();
-  };
-  auto take = [&](float (&v)[32]) {
-    cp_async_wait<0>();
-    __syncwarp();
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = fr0 + 8 * hh;
+        if (row < nvalid) {
+          float* o = h_out + (long)(node0 + row) * EQD_HID + fc;
 #pragma unroll
-    for (int c4 = 0; c4 < 8; ++c4) {
-      float4 t = *reinterpret_cast<const float4*>(sc + lane * NM_SC_LD + c4 * 4);
-      v[c4 * 4] = t.x; v[c4 * 4 + 1] = t.y; v[c4 * 4 + 2] = t.z; v[c4 * 4 + 3] = t.w;
-    }
-    __syncwarp();
-  };
-  fetch(h_in, EQD_HID, blockIdx.x);
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    if (q == 0) TRACE_PHASE(3, blockIdx.x, tile, 1);
-    const int node = tile * EQD_TM + r;
-    const bool valid = node < n_nodes;
-    // ---- node_mlp.0 over [h | aggr | mu | h0] in 5 K-pieces ---------------------------------------------------
-    // Each 64-wide piece is its own accumulation (4 full-magnitude steps, like the edge-stage GEMMs) and the pieces
-    // are summed in registers with round-to-nearest FADDs.
-    float acc[32];
-#pragma unroll
-    for (int c = 0; c < 32; ++c) acc[c] = cst.b5[half * 32 + c];
-    {
-      float v[32], d[32];
-      auto piece = [&](unsigned w_off, int nkb) {
-        tc_fence_before();
-        __syncthreads();
-        gemm(w_off, NM_W5_SPLIT, nkb, d);
-#pragma unroll
-        for (int c = 0; c < 32; ++c) acc[c] += d[c];
-      };
-      take(v);
-      fetch(aggr, EQD_HID, tile);
-      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 0 (h) -> A
-      piece(0, 4);
-      take(v);
-      fetch(mu, EQD_HID, tile);
-      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 1 (aggr)
-      piece(4 * 2048, 4);
-      take(v);
-      fetch(h0, EQD_H0_PAD, tile);
-      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 2 (mu)
-      piece(8 * 2048, 4);
-      take(v);
-      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);   // piece 3 (h0[0:64])
-      piece(12 * 2048, 4);
-      // piece 4: h0[64:72] + 8 zero columns (K = 16): the half-0 threads write the k-block
-      if (half == 0) {
-        const float4* sp = reinterpret_cast<const float4*>(h0 + (long)node * EQD_H0_PAD + 64);
-        float4 a = valid ? sp[0] : make_float4(0.f, 0.f, 0.f, 0.f), b = valid ? sp[1] : make_float4(0.f, 0.f, 0.f, 0.f);
-        float t[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-        store_extra8_split3<EQD_TM>(S.a, NM_A_SPLIT, r, 0, t);
+          for (int j = 0; j < 8; ++j) {   // :332-334
+            const float2 bj = *reinterpret_cast<const float2*>(&S.c[192 + 8 * j + fc]);
+            const int i = 4 * j + 2 * hh;
+            *reinterpret_cast<float2*>(o + 8 * j) =
+                make_float2(__fmaf_rn(__fadd_rn(d[i], bj.x), sk, __fmul_rn(hs[i], sk1)),
+                            __fmaf_rn(__fadd_rn(d[i + 1], bj.y), sk, __fmul_rn(hs[i + 1], sk1)));
+          }
+        }
       }
-      piece(16 * 2048, 1);
     }
-    // ---- + bias, LeakyReLU, LayerNorm -> bf16x3 -> A ; node_mlp.4 ---------------------------------------------
-    {
-      float v[32];
-      float s4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        v[c] = lrelu(acc[c], slope);
-        s4[c & 3] += v[c];
-      }
-      const float mh = ((s4[0] + s4[1]) + (s4[2] + s4[3])) * (1.f / 32.f);
-      float q4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        float d = v[c] - mh;
-        q4[c & 3] = fmaf(d, d, q4[c & 3]);
-      }
-      red[(r * 2 + half) * 2 + 0] = mh;
-      red[(r * 2 + half) * 2 + 1] = (q4[0] + q4[1]) + (q4[2] + q4[3]);
-      __syncthreads();
-      const float m0 = red[r * 4 + 0], m1 = red[r * 4 + 2];
-      const float mean = 0.5f * (m0 + m1);
-      const float dm = m0 - m1;
-      const float var = (red[r * 4 + 1] + red[r * 4 + 3] + dm * dm * 16.f) * (1.f / 64.f);  // Chan et al. combination
-      const float rstd = 1.f / sqrtf(var + 1e-5f);
-#pragma unroll
-      for (int c = 0; c < 32; ++c) v[c] = (v[c] - mean) * rstd * cst.ln_g[half * 32 + c] + cst.ln_b[half * 32 + c];
-      store_half_split3<EQD_TM>(S.a, NM_A_SPLIT, r, half * 32, v);
-    }
-    fetch(h_in, EQD_HID, tile);   // the skip operand again (an L2 hit) rather than 32 registers held across the tile
-    tc_fence_before();
-    __syncthreads();
-    {
-      float v[32], hskip[32];
-      gemm(NM_W6_BASE, NM_W6_SPLIT, 4, v);
-      take(hskip);
-      const float sk = p.skip_weight_h, sk1 = 1.f - p.skip_weight_h;
-#pragma unroll
-      for (int c = 0; c < 32; ++c) v[c] = sk * (v[c] + cst.b6[half * 32 + c]) + sk1 * hskip[c];  // :332-334
-      // transposed through the scratch: 8 lanes write one contiguous 128-byte half row
-#pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4)
-        *reinterpret_cast<float4*>(sc + lane * NM_SC_LD + c4 * 4) = make_float4(v[c4 * 4], v[c4 * 4 + 1], v[c4 * 4 + 2], v[c4 * 4 + 3]);
-      __syncwarp();
-      float* o = h_out + ((long)tile * EQD_TM + wrow0) * EQD_HID + half * 32 + (lane & 7) * 4;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int row = i * 4 + (lane >> 3);
-        float4 t = *reinterpret_cast<const float4*>(sc + row * NM_SC_LD + (lane & 7) * 4);
-        if ((long)tile * EQD_TM + wrow0 + row < n_nodes) *reinterpret_cast<float4*>(o + (long)row * EQD_HID) = t;
-      }
-      __syncwarp();
-    }
-    fetch(h_in, EQD_HID, tile + gridDim.x);   // next tile's h rows
   }
+  cp_async_wait<0>();
   TRACE_END(3);
 }
 
@@ -385,11 +404,12 @@ extern "C" int eqd_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const f
   if (g->n_nodes <= 0) return EQD_OK;
   eqd::NmConsts cst;
   memcpy(&cst, p_l->consts.node, sizeof(cst));
-  int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
-  size_t smem = sizeof(eqd::NmSmem) + 128;
-  EQD_SET_SMEM((eqd::node_mlp_tc_kernel), smem);
-  int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
-  eqd::node_mlp_tc_kernel<<<grid, NM_THREADS, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h_in, aggr, mu, h0, h_out);
+  const int ntiles = (g->n_nodes + 63) / 64;
+  const size_t smem = sizeof(eqd::NmSmem) + 128;
+  EQD_SET_SMEM(eqd::node_mlp_tc_kernel, smem);
+  int grid = (ntiles + NM_CHAINS - 1) / NM_CHAINS;
+  if (grid > EQD_SMS) grid = EQD_SMS;
+  eqd::node_mlp_tc_kernel<<<grid, NM_CHAINS * 128, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h_in, aggr, mu, h0, h_out);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }

@@ -254,6 +254,20 @@ __device__ __forceinline__ void staged_rows_to_a_split3(const float* rows, int t
       split3_pair(v.x, v.y, a[0][kb][i], a[1][kb][i], a[2][kb][i]);
     }
 }
+// The same staged values unsplit, in the m64n64 accumulator layout (the A fragments' ownership: v[8 kb + 2 i + e] is
+// register i, element e of k-block kb): acc_to_a_split3<4> on v gives the fragments of staged_rows_to_a_split3.
+__device__ __forceinline__ void staged_rows_to_frag(const float* rows, int t, float (&v)[32]) {
+  const int g = (t >> 5) * 16 + ((t & 31) >> 2), c = t & 3;
+#pragma unroll
+  for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int row = g + 8 * (i & 1), k4 = 4 * kb + 2 * (i >> 1) + (c >> 1);
+      const float2 x = *reinterpret_cast<const float2*>(rows + row * 64 + ((k4 ^ stage_swz(row)) << 2) + 2 * (c & 1));
+      v[8 * kb + 2 * i] = x.x;
+      v[8 * kb + 2 * i + 1] = x.y;
+    }
+}
 // Row statistics in the summation order of a row-per-thread epilogue: per 32-column half ch of the row, chain k = 0..3 adds
 // the columns 32 ch + 4 c4 + k for c4 = 0..7 in turn.  In the accumulator layout lane c of a quad holds the columns
 // 8 j + 2 c + e (e = 0, 1), so chain k = 2 (c & 1) + e alternates between lane c and lane c ^ 2; each lane runs its two
