@@ -146,6 +146,29 @@ class LayerTrainPack:
         self.maps = maps
 
 
+def tn_gemm_shapes(N: int, E: int, dhps: Sequence[int] = (nat.H0_PAD, nat.HID)) -> List[tuple]:
+    """Every (rows, K, ncols) that TrainEngine.backward passes to eqd_tn_gemm, for a batch of N nodes and E edges whose
+    layers have the padded widths ``dhps`` (72 for the 69-wide layer 0, 64 for the others)."""
+    shapes = [(N, 64, 64)]                                   # head: mlp_h_mean_ROT.0 (h, dpre)
+    for dhp in dhps:
+        shapes += [(N, dhp, 64),                             # node_mlp.4 (n5, dh')
+                   (N, dhp, dhp), (N, 64, dhp), (N, nat.H0_PAD, dhp),   # node_mlp.0: h and mu | aggr | h0 blocks (du)
+                   (N, dhp, 128 + 3 * dhp),                  # projections: edge_mlp.0 node blocks, att_mlp_Q/K/V (h, dP)
+                   (E, 44, 64), (E, 64, 64)]                 # edge_mlp.0 [he | rbf] block, edge_mlp.4, coors_mlp.0
+    return sorted(set(shapes))
+
+
+def tn_workspace_floats(N: int, E: int, dhps: Sequence[int] = (nat.H0_PAD, nat.HID)) -> tuple:
+    """(partial, colsum) floats that cover every eqd_tn_gemm call of one backward (see tn_gemm_shapes)."""
+    lib = nat.load()
+    partial = colsum = 1
+    for rows, K, nc in tn_gemm_shapes(N, E, dhps):
+        nch = C.c_int32(0)
+        partial = max(partial, int(lib.eqd_tn_partial_floats(rows, K, nc, None, C.byref(nch))))
+        colsum = max(colsum, nch.value * nc)
+    return partial, colsum
+
+
 class BackwardWorkspace:
     """Device buffers of one backward, sized for a plan (reused across steps with the same sizes)."""
 
@@ -163,11 +186,8 @@ class BackwardWorkspace:
         self.n1, self.msg, self.dz3, self.dmsg, self.dz1 = (f(max(E, 1), 64) for _ in range(5))
         self.dxrel = d(max(E, 1), 3)
         lib = nat.load()
-        need = 0
-        for rows, K, nc in ((E, 64, 64), (E, 44, 64), (N, 72, 344), (N, 72, 72), (N, 72, 64)):
-            need = max(need, int(lib.eqd_tn_partial_floats(rows, K, nc, None, None)))
-        self.partial = f(max(need, 1))
-        self.colsum = f(4096 * 344)
+        n_partial, n_colsum = tn_workspace_floats(N, E)
+        self.partial, self.colsum = f(n_partial), f(n_colsum)
         self.vec = f(132 * 256)   # per-CTA partial sums of bwd_node / bwd_edge (grid <= EQD_SMS)
         self.head_ws_bytes = int(lib.eqd_bwd_head_workspace_bytes(N, plan.n_node_tiles, B))
         self.head_ws = torch.empty(self.head_ws_bytes, dtype=torch.uint8, device=device)

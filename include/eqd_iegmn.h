@@ -355,7 +355,7 @@ int eqd_grad_reduce(const float* partial, int32_t nchunks, int64_t stride, const
 int eqd_bwd_node_mlp(const eqd_graph* g, const eqd_layer* p, const float* w_node1_lin, const float* w_node2_lin,
                      const float* h_in, int32_t ldh, const float* aggr, const float* mu, int32_t ldmu, const float* h0,
                      const float* dh_out, float* dh_in, float* daggr, float* dmu, float* dh0_acc, float* n5_out,
-                     float* du_out, float* vec_partial /* [148][144] */, int32_t* n_partials_out, void* stream);
+                     float* du_out, float* vec_partial /* [132][144] */, int32_t* n_partials_out, void* stream);
 /* Cross attention backward (:46-64, 247-256): dmu [n][dhp] -> dP[:, 128:] = [dQpre | dKpre | dV] of the combined
  * projection-gradient matrix dP [n][128 + 3 dhp].  proj = this layer's fp32 projections (eqd_project), mu the stashed
  * attention output, rowstat [n][4] scratch.                                                                         */
@@ -368,7 +368,7 @@ int eqd_bwd_attention(const eqd_graph* g, const eqd_layer* p, const float* proj,
 int eqd_bwd_edge(const eqd_graph* g, const eqd_layer* p, const float* w2lin, const float* w3lin, const float* proj,
                  const double* x_in, const float* daggr, const double* dx_out, float* ein_out, float* n1_out,
                  float* msg_out, float* dz3_out, float* dmsg_out, float* dz1_out, double* dxrel_out,
-                 float* vec_partial /* [148][256] */, int32_t* n_partials_out, void* stream);
+                 float* vec_partial /* [132][256] */, int32_t* n_partials_out, void* stream);
 /* Per node: dP[:, 0:64] = sum over OUT-edges of dz1, dP[:, 64:128] = sum over IN-edges, dx_in = (1 - eta) dx_out +
  * sum_out dxrel - sum_in dxrel.  out_ptr [n+1] / out_edge [E]: edges grouped by SOURCE node (ascending edge id).      */
 int eqd_bwd_edge_gather(const eqd_graph* g, const int32_t* out_ptr, const int32_t* out_edge, const float* dz1,

@@ -215,7 +215,8 @@ def layer_backward(p, cfg, caches, dh_new, dx_new, G, stages=None):
         out.append((dh, dx, dh0))
         if stages is not None:
             stages.append({'side': i, 'dh_part': dh_part, 'daggr': daggr, 'dmu': dmu, 'dh0': dh0, 'dz1': dz1, 'dxrel': dxrel,
-                           'dpsrc': dpsrc, 'dpdst': dpdst, 'dx': dx, 'dqpre': dqpre, 'dkpre': dkpre, 'dv': dv, 'dh': dh})
+                           'dpsrc': dpsrc, 'dpdst': dpdst, 'dx': dx, 'dqpre': dqpre, 'dkpre': dkpre, 'dv': dv, 'dh': dh,
+                           'z1': c['z1'], 'z3': c['z3'], 'u5': c['u5']})
     return out
 
 

@@ -94,6 +94,36 @@ def test_workspace_bytes_host_arithmetic():
     assert lib.eqd_workspace_bytes(0, 0, 0) > 0
 
 
+def test_backward_workspace_covers_every_weight_gradient_reduction():
+    """BackwardWorkspace's partial / colsum sizes cover eqd_tn_partial_floats (and nchunks * ncols) of every eqd_tn_gemm
+    call TrainEngine.backward makes, listed here from the backward itself.  The row chunking depends on the number of
+    64 x 64 output blocks, so the largest buffer is not the largest shape: at N = 40 000 the 64-wide layers' projection
+    reduction (N, 64, 320) needs 16 384 floats more than the 69-wide layer's (N, 72, 344)."""
+    from equidock_public_b200.training import tn_gemm_shapes, tn_workspace_floats
+    lib = nat.load()
+
+    def need(rows, K, nc):
+        nch = ctypes.c_int32(0)
+        return int(lib.eqd_tn_partial_floats(rows, K, nc, None, ctypes.byref(nch))), nch.value * nc
+
+    Ns = list(range(1, 3000, 23)) + list(range(3000, 200001, 1009)) + [9600, 23700, 40000, 132000, 200000]
+    for N in Ns:
+        for E in (N // 2, N, 4 * N, 10 * N, 16 * N):
+            partial, colsum = tn_workspace_floats(N, E)
+            listed = set(tn_gemm_shapes(N, E))
+            for dhp in (nat.H0_PAD, nat.HID):
+                calls = [(N, 64, 64),                                                   # head: mlp_h_mean_ROT.0
+                         (N, dhp, 64), (N, dhp, dhp), (N, 64, dhp), (N, nat.H0_PAD, dhp),   # node_mlp.4, node_mlp.0 blocks
+                         (N, dhp, 128 + 3 * dhp),                                      # projections
+                         (E, 44, 64), (E, 64, 64)]                                      # edge_mlp.0 / .4, coors_mlp.0
+                for shape in calls:
+                    assert shape in listed, (N, E, shape)
+                    p, c = need(*shape)
+                    assert p <= partial and c <= colsum, (N, E, shape, p, partial, c, colsum)
+    # the batch where the parent's five-shape list fell short: 100 pairs of 200 + 200 nodes, ten edges per node
+    assert need(40000, 64, 320)[0] == 2150400 <= tn_workspace_floats(40000, 400000)[0]
+
+
 def test_engine_refuses_cpu_device():
     with pytest.raises(nat.NativeLibraryError):
         IEGMNEngine(torch.device('cpu'))

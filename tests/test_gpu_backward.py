@@ -19,6 +19,7 @@ from equidock_public_b200.training import TrainEngine
 
 pytestmark = pytest.mark.gpu
 PAIR = {'db5': '1QA9', 'dips': 'kq_1kq1.pdb1_2.dill'}
+KINK_MAX_FRACTION = 1e-2   # of the edge / node rows of a layer (see _stage_report's kink_band)
 
 
 def _np(t):
@@ -45,12 +46,17 @@ def _loss_grads(tgt):
     return f
 
 
-def _stage_report(model, args, pairs, grad_fns, cuda_device):
+def _stage_report(model, args, pairs, grad_fns, cuda_device, kink_band=0.0):
     """Runs forward + CUDA backward with stage capture on a batch and compares every stage output and every parameter
     gradient with the per-pair manual oracle (concatenated in engine order: ligand nodes / edges of all pairs, then the
     receptor ones).  An entry passes if max|got - ref| <= tol * max|ref| + 2e-6 * G, G = the largest reference magnitude
     of the same group (all stage tensors / all parameter gradients): fp32 cancellation noise on a tensor whose true
-    gradient is orders of magnitude below its neighbours' (a saturated attention layer) is not an error."""
+    gradient is orders of magnitude below its neighbours' (a saturated attention layer) is not an error.
+    kink_band > 0 leaves out the rows of a layer with an fp64 pre-activation (z1, z3 of an edge, u5 of a node) within
+    kink_band x (the row's max|z|) of the LeakyReLU kink: the engine's fp32 activations after several layers need not
+    resolve its sign there, and the derivative differs by (1 - slope) x the upstream gradient.  Such edges, such nodes and
+    the nodes such edges gather into are left out of the per-row stage comparisons (at most KINK_MAX_FRACTION of a
+    layer's rows)."""
     sd = {k: v.detach().cpu().numpy() for k, v in model.state_dict().items()}
     cfg = orc.OracleConfig.from_args(args)
     shared = bool(args['shared_layers'])
@@ -77,9 +83,10 @@ def _stage_report(model, args, pairs, grad_fns, cuda_device):
     torch.cuda.synchronize()
     rows = []          # (group, tag, err, refmax, tol)
 
-    def chk(group, tag, got, ref, tol):
+    def chk(group, tag, got, ref, tol, keep=None):
         got, ref = _np(got), np.asarray(ref, np.float64)
-        rows.append((group, tag, float(np.abs(got - ref).max()), float(np.abs(ref).max()), tol))
+        d = np.abs(got - ref) if keep is None else np.abs(got - ref)[keep]
+        rows.append((group, tag, float(d.max()), float(np.abs(ref).max()), tol))
 
     def cat(key, li=None, head=False):
         sides = [[], []]
@@ -94,21 +101,30 @@ def _stage_report(model, args, pairs, grad_fns, cuda_device):
 
     chk('stage', 'head dh', cap[0]['dh'], cat('dh', head=True), 2e-3)
     chk('stage', 'head dx', cap[0]['dx'], cat('dx', head=True), 2e-3)
+    plan = fwd['plan']
+    src, dst = plan.col_src.cpu().numpy(), plan.edge_dst.cpu().numpy()
+    near = lambda z: (np.abs(z) < kink_band * np.abs(z).max(1, keepdims=True)).any(1)
     for c in cap[1:]:
         li = c['layer']
         dh_w = cat('dh', li).shape[1]
         dhp = c['dmu'].shape[1]
-        chk('stage', f'L{li} node: dh (skip + W5 h block)', c['dh_part'][:, :dh_w], cat('dh_part', li), 2e-3)
-        chk('stage', f'L{li} node: daggr', c['daggr'], cat('daggr', li), 2e-3)
-        chk('stage', f'L{li} node: dmu', c['dmu'][:, :dh_w], cat('dmu', li), 2e-3)
-        chk('stage', f'L{li} edge: dz1', c['dz1'], cat('dz1', li), 2e-3)
-        chk('stage', f'L{li} edge: dxrel', c['dxrel'], cat('dxrel', li), 2e-3)
-        chk('stage', f'L{li} gather: dPsrc', c['dP'][:, 0:64], cat('dpsrc', li), 2e-3)
-        chk('stage', f'L{li} gather: dPdst', c['dP'][:, 64:128], cat('dpdst', li), 2e-3)
+        e_ok, n_ok = ~(near(cat('z1', li)) | near(cat('z3', li))), ~near(cat('u5', li))
+        g_ok = np.ones(plan.N, bool)
+        g_ok[src[~e_ok]] = g_ok[dst[~e_ok]] = False
+        assert (~e_ok).mean() <= KINK_MAX_FRACTION and (~n_ok).mean() <= KINK_MAX_FRACTION
+        if not (e_ok.all() and n_ok.all()):
+            print(f'L{li}: {(~e_ok).sum()} edge rows, {(~n_ok).sum()} node rows within the kink band')
+        chk('stage', f'L{li} node: dh (skip + W5 h block)', c['dh_part'][:, :dh_w], cat('dh_part', li), 2e-3, n_ok)
+        chk('stage', f'L{li} node: daggr', c['daggr'], cat('daggr', li), 2e-3, n_ok)
+        chk('stage', f'L{li} node: dmu', c['dmu'][:, :dh_w], cat('dmu', li), 2e-3, n_ok)
+        chk('stage', f'L{li} edge: dz1', c['dz1'], cat('dz1', li), 2e-3, e_ok)
+        chk('stage', f'L{li} edge: dxrel', c['dxrel'], cat('dxrel', li), 2e-3, e_ok)
+        chk('stage', f'L{li} gather: dPsrc', c['dP'][:, 0:64], cat('dpsrc', li), 2e-3, g_ok)
+        chk('stage', f'L{li} gather: dPdst', c['dP'][:, 64:128], cat('dpdst', li), 2e-3, g_ok)
         chk('stage', f'L{li} attn: dQpre', c['dP'][:, 128:128 + dh_w], cat('dqpre', li), 2e-3)
         chk('stage', f'L{li} attn: dKpre', c['dP'][:, 128 + dhp:128 + dhp + dh_w], cat('dkpre', li), 2e-3)
         chk('stage', f'L{li} attn: dV', c['dP'][:, 128 + 2 * dhp:128 + 2 * dhp + dh_w], cat('dv', li), 2e-3)
-        chk('stage', f'L{li} gather: dx', c['dx'], cat('dx', li), 2e-3)
+        chk('stage', f'L{li} gather: dx', c['dx'], cat('dx', li), 2e-3, g_ok)
         chk('stage', f'L{li} proj: dh', c['dh'][:, :dh_w], cat('dh', li), 2e-3)
     flat_np = _np(flat)
     lo = eng.layout
@@ -136,31 +152,45 @@ def test_backward_stage_by_stage_vs_manual_oracle(ds, cuda_device):
     assert not bad, '\n'.join(bad)
 
 
-@pytest.mark.parametrize('kind', ['db5', 'dips', 'random'])
+@pytest.mark.parametrize('kind', ['db5', 'dips', 'random', 'bulk', 'k70'])
 def test_backward_stage_by_stage_ragged_batch(kind, cuda_device):
     """B = 3 ragged pairs incl. tile boundaries (129 = 128 + 1, 131 = 128 + 3): both checkpoints (5 shared layers / 8
     layers) and a random-init 3-layer unshared model with non-trivial biases / LayerNorm affine parameters.  The random
     model's keypoint attention is sharpened: at default init it is nearly uniform, every keypoint sits at the centroid and
     the reference's SVD guard (:574) fires on all three pairs (the fp64 oracle's own verdict).  Its seed keeps every edge
     pre-activation of the fp64 oracle >= 1.5e-6 away from the LeakyReLU kink: closer than fp32 resolves, the engine may take
-    the other branch and the derivative there differs by 0.99 x the upstream gradient (seed 5 has one at 1.4e-8)."""
+    the other branch and the derivative there differs by 0.99 x the upstream gradient (seed 5 has one at 1.4e-8).
+    `bulk` (DIPS checkpoint) adds 168 pairs of 200 + 200 nodes: 67 648 nodes, so every persistent backward kernel runs at
+    least two tiles per CTA (529 node tiles on the 264 CTAs of the projection backward and the 132 of the others, 680
+    attention tiles, about 5 300 edge tiles); of its 90 M pre-activations per layer some lie closer to the kink than
+    fp32 resolves, so its rows within 1e-5 x (the row's max|z|) of it are left out (see _stage_report).  `k70`: the DIPS
+    checkpoint with graph_max_neighbor = 70 on pairs built with 70 in-edges per node, above the 64 of the forward's
+    tensor-core edge tile."""
     from test_gpu_parity import _random_model
+    k = 10
     if kind == 'random':
         model, args = _random_model(cuda_device, 3, False, seed=7)
         with torch.no_grad():
             for name, p in model.named_parameters():
                 if name.startswith(('iegmn_original.att_mlp_key_ROT.', 'iegmn_original.att_mlp_query_ROT.')):
                     p.mul_(8.0)
+    elif kind == 'k70':
+        k, args = 70, dict(gio.load_args('dips'), graph_max_neighbor=70)
+        model = gio.build_model('dips', cuda_device, args=args)
     else:
-        model, args = gio.build_model(kind, cuda_device), gio.load_args(kind)
+        ds = 'dips' if kind == 'bulk' else kind
+        model, args = gio.build_model(ds, cuda_device), gio.load_args(ds)
     model.train()
     rng = np.random.default_rng(9)
-    sizes = [(40, 131), (129, 20), (64, 64)]
-    pairs = [synthetic.synthetic_pair(rng, a, b, 10) for a, b in sizes]
+    sizes = [(100, 131), (129, 90), (75, 80)] if kind == 'k70' else [(40, 131), (129, 20), (64, 64)]
+    if kind == 'bulk':
+        sizes += [(200, 200)] * 168
+        assert -(-sum(a + b for a, b in sizes) // 128) >= 2 * 264
+    pairs = [synthetic.synthetic_pair(rng, a, b, k) for a, b in sizes]
     tg = [{'c': rng.normal(0, 5, (a, 3)), 'yl': rng.normal(0, 10, (50, 3)), 'yr': rng.normal(0, 10, (50, 3))} for a, b in sizes]
     fns = [(lambda out, t=t: (2 * (out['ligand_coors'] - t['c']), 2 * (out['keypts_ligand'] - t['yl']),
                               2 * (out['keypts_receptor'] - t['yr']))) for t in tg]
-    bad = _stage_report(model, args, pairs, fns, cuda_device)
+    bad = _stage_report(model, args, pairs, fns, cuda_device, kink_band=1e-5 if kind == 'bulk' else 0.0)
     assert not bad, '\n'.join(bad)
 
 
@@ -228,7 +258,10 @@ def test_ragged_batch_gradient_is_the_sum_of_pair_gradients(cuda_device):
 def test_tn_gemm_and_reduce_vs_torch(cuda_device):
     lib = nat.load()
     torch.manual_seed(0)
-    for rows, K, nc, ldx, ldd in ((1000, 64, 64, 64, 64), (37, 44, 64, 44, 64), (5000, 72, 344, 72, 344), (300, 72, 72, 72, 72)):
+    # the last five: the training shapes of 100 pairs of 200 + 200 nodes (E = 400 000 edge rows, N = 40 000 node rows)
+    for rows, K, nc, ldx, ldd in ((1000, 64, 64, 64, 64), (37, 44, 64, 44, 64), (5000, 72, 344, 72, 344), (300, 72, 72, 72, 72),
+                                  (400000, 64, 64, 64, 64), (400000, 44, 64, 44, 64), (40000, 64, 320, 64, 320),
+                                  (40000, 72, 344, 72, 344), (40000, 64, 72, 64, 72)):
         X = torch.randn(rows, ldx, device=cuda_device)
         D = torch.randn(rows, ldd, device=cuda_device)
         need = int(lib.eqd_tn_partial_floats(rows, K, nc, None, None))
