@@ -33,7 +33,10 @@ class PocketBatch:
 def device_losses(plan, pred_lig: torch.Tensor, keypts: torch.Tensor, tgt: PocketBatch, pocket_ot_loss_weight: float,
                   intersection_loss_weight: float, intersection_sigma: float, intersection_surface_ct: float) -> Dict:
     """-> {'total': (4,) f64 [loss, mse, ot, intersection], 'parts': (B,4) f64, 'dcoors': (N_l,3) f32,
-    'dkeypts': (2B,50,3) f64}; raises if a pocket exceeds the solver's capacity or the transport solve failed."""
+    'dkeypts': (2B,50,3) f64, 'plan': (n_pocket_total,50) i32, 'err': (1,) i32}.  'plan' is a view of the workspace
+    holding the integer transport plans (pair b: rows pocket_ptr[b]..pocket_ptr[b+1], units of 1/(N_pocket * 50); rows of
+    a pair the solver skipped are undefined).  check_loss_status(res) raises if a pocket exceeds the solver's capacity or
+    the transport solve failed."""
     lib = nat.load()
     dev = pred_lig.device
     B, N_l = plan.n_pairs, plan.N_l
@@ -54,7 +57,10 @@ def device_losses(plan, pred_lig: torch.Tensor, keypts: torch.Tensor, tgt: Pocke
                                  tgt.max_pocket, float(pocket_ot_loss_weight), float(intersection_loss_weight), float(intersection_sigma),
                                  float(intersection_surface_ct), nat.ptr(ws), ws_bytes, nat.ptr(parts), nat.ptr(total),
                                  nat.ptr(dco), nat.ptr(dkp), nat.ptr(err), st), 'eqd_losses')
-    return {'total': total, 'parts': parts, 'dcoors': dco, 'dkeypts': dkp, 'err': err, '_keep': (ws, pred, kp)}
+    off = (max(plan.N_r, 1) * 8 + 255) // 256 * 256                     # plan_flow offset (eqd_iegmn.h)
+    flow = ws[off:off + tgt.n_pocket_total * nat.HEADS * 4].view(torch.int32).view(tgt.n_pocket_total, nat.HEADS)
+    return {'total': total, 'parts': parts, 'dcoors': dco, 'dkeypts': dkp, 'plan': flow, 'err': err,
+            '_keep': (ws, pred, kp)}
 
 
 def check_loss_status(res):

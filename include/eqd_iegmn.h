@@ -391,7 +391,11 @@ int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const float* h, 
 /* ---- training losses on the device (src/train.py:41-49, 112-150; src/utils/ot_utils.py:5-29) ------------------------
  * Per pair: MSE of the predicted ligand coordinates, body-intersection loss, pocket OT loss with the EXACT earth mover's
  * distance (uniform marginals; successive shortest paths with potentials instead of POT's CPU network simplex), batch
- * means combined with the reference's weights; plus the gradients w.r.t. the predicted coordinates and the keypoints. */
+ * means combined with the reference's weights; plus the gradients w.r.t. the predicted coordinates and the keypoints.
+ * After the call the workspace holds the integer transport plans: int32 plan_flow[n_pocket_total][50] at byte offset
+ * round_up(max(N_r, 1) * 8, 256), N_r = n_nodes - n_lig_nodes; pair b owns rows pocket_ptr[b] .. pocket_ptr[b+1] in units
+ * of 1 / (N_pocket * 50) (every row sums to 50, every column to N_pocket).  Rows of a pair that err_flags reports as too
+ * large are not written. */
 size_t eqd_losses_workspace_bytes(int32_t n_rec_nodes, int32_t n_pocket_total);
 int eqd_losses(const eqd_graph* g, const float* pred_lig /*[N_l][3]*/, const float* bound_lig /*[N_l][3]*/,
                const float* bound_rec /*[N_r][3]*/, const double* keypts /*[2B][50][3]*/,

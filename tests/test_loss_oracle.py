@@ -20,6 +20,39 @@ def test_ot_emd_is_certified_optimal():
         assert (plan > 1e-14).sum() <= n + m - 1 + 1                 # a vertex of the transport polytope
 
 
+@pytest.mark.parametrize('n', [7, 50, 398])
+def test_ot_certify_accepts_the_lp_plan_and_rejects_a_perturbed_one(n):
+    """ot_certify (marginals + no negative residual cycle) accepts the HiGHS-optimal plan in integer units, also with
+    tied costs (keypoints on top of each other), and rejects the plan after one unit is moved around a 2 x 2 cycle that
+    costs more, or after the marginals are broken."""
+    rng = np.random.default_rng(n)
+    for ties in (False, True):
+        y = rng.normal(0, 10, (50, 3))
+        if ties:
+            y[25:] = y[:25]
+        cost = lo.sq_dist_mat(rng.normal(0, 10, (n, 3)), y)
+        val, plan, _ = lo.ot_emd(cost)
+        x = np.rint(plan * n * 50).astype(np.int64)
+        assert np.abs(x - plan * n * 50).max() < 1e-6                 # a vertex: integral in these units
+        assert lo.ot_certify(cost, x) == 0.0
+        # move one unit around the 2 x 2 cycle (i, k) -> (i, k2), (j, k2) -> (j, k) between two flows that costs the most
+        I, K = np.nonzero(x)
+        d = cost[I[:, None], K[None, :]] + cost[I[None, :], K[:, None]] - cost[I, K][:, None] - cost[I, K][None, :]
+        d[(I[:, None] == I[None, :]) | (K[:, None] == K[None, :])] = -np.inf
+        a, b = np.unravel_index(np.argmax(d), d.shape)
+        i, k, j, k2 = I[a], K[a], I[b], K[b]
+        assert d[a, b] > 1e-6 * np.abs(cost).max()
+        y2 = x.copy()
+        y2[i, k] -= 1; y2[i, k2] += 1; y2[j, k2] -= 1; y2[j, k] += 1
+        assert (y2 >= 0).all() and (y2.sum(1) == 50).all() and (y2.sum(0) == n).all()
+        with pytest.raises(AssertionError, match='negative residual cycle'):
+            lo.ot_certify(cost, y2)
+        y3 = x.copy()
+        y3[i, k] -= 1
+        with pytest.raises(AssertionError):
+            lo.ot_certify(cost, y3)
+
+
 def test_ot_emd_known_answers():
     # identical clouds, n == m: the identity matching costs 0
     x = np.random.default_rng(1).normal(size=(50, 3))
