@@ -16,8 +16,8 @@ __device__ __forceinline__ double warp_max_d(double v) {
 }
 
 // 3x3 SVD A = U diag(S) V^T by one-sided (Hestenes) Jacobi in fp64, singular values sorted
-// descending.  Columns of U belonging to a zero singular value are completed to an orthonormal
-// basis (such inputs are flagged by the guard anyway).
+// descending.  U is orthonormal for every input: columns of U that belong to a singular value at
+// rounding level of S[0] are completed from V (see the end).
 __device__ inline void svd3(const double (&A)[9], double (&U)[9], double (&S)[3], double (&V)[9]) {
   double G[9];
 #pragma unroll
@@ -40,7 +40,9 @@ __device__ inline void svd3(const double (&A)[9], double (&U)[9], double (&S)[3]
       if (fabs(gamma) <= 1e-18 * lim) continue;
       off = fmax(off, fabs(gamma) / fmax(lim, 1e-300));
       double zeta = (beta - alpha) / (2.0 * gamma);
-      double t = (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+      // |zeta| > 1e153 (a column at rounding level of the other): zeta * zeta overflows from ~1.3e154 on and the textbook t
+      // would be 0, which stalls the sweep; t = 1 / (2 zeta) is its limit there
+      double t = fabs(zeta) > 1e153 ? 0.5 / zeta : (zeta >= 0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
       double c = 1.0 / sqrt(1.0 + t * t), sn = c * t;
 #pragma unroll
       for (int r = 0; r < 3; ++r) {
@@ -75,11 +77,31 @@ __device__ inline void svd3(const double (&A)[9], double (&U)[9], double (&S)[3]
   }
 #pragma unroll
   for (int q = 0; q < 9; ++q) V[q] = Vs[q];
-  // complete U if rank deficient: u2 = u0 x u1 (only matters for flagged inputs)
-  if (S[2] <= 1e-300 * S[0] || S[2] == 0.0) {
-    U[2] = U[3] * U[7] - U[6] * U[4];
-    U[5] = U[6] * U[1] - U[0] * U[7];
-    U[8] = U[0] * U[4] - U[3] * U[1];
+  // Rank-deficient A (collinear or coplanar point sets, 1-3 points): a column whose singular value is at rounding level of
+  // S[0] carries no direction -- its normalised G column is zero or noise.  Complete U from the matching columns of V,
+  // Gram-Schmidt against the columns already fixed, so that U stays orthonormal: a symmetric PSD A (Kabsch of a trace onto
+  // itself) then gives U = V, i.e. R = I, and any other A an optimal proper rotation after the reflection fix.
+  const double tol = 64.0 * 2.220446049250313e-16 * S[0];
+  if (!(S[0] > tol)) {            // A = 0
+    U[0] = V[0]; U[3] = V[3]; U[6] = V[6];
+  }
+  if (!(S[1] > tol)) {            // rank <= 1: v1, else v2, minus its u0 component (one of the two keeps |w|^2 >= 1/2)
+    double w[3], ww = 0.0;
+    for (int k = 1; k < 3 && ww < 0.5; ++k) {
+      const double d = U[0] * V[k] + U[3] * V[3 + k] + U[6] * V[6 + k];
+      ww = 0.0;
+      for (int r = 0; r < 3; ++r) {
+        w[r] = V[r * 3 + k] - d * U[r * 3];
+        ww += w[r] * w[r];
+      }
+    }
+    const double inv = 1.0 / sqrt(ww);
+    for (int r = 0; r < 3; ++r) U[r * 3 + 1] = w[r] * inv;
+  }
+  if (!(S[2] > tol)) {            // rank <= 2: u2 = +-(u0 x u1), the sign of v2
+    const double w[3] = {U[3] * U[7] - U[6] * U[4], U[6] * U[1] - U[0] * U[7], U[0] * U[4] - U[3] * U[1]};
+    const double sg = w[0] * V[2] + w[1] * V[5] + w[2] * V[8] < 0.0 ? -1.0 : 1.0;
+    for (int r = 0; r < 3; ++r) U[r * 3 + 2] = sg * w[r];
   }
 }
 

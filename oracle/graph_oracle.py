@@ -75,7 +75,6 @@ def residue_distance_matrix_fast(atoms, atom_ptr):
     cnt = np.diff(atom_ptr).astype(np.float64)
     out = np.zeros((N, N))
     step = max(1, int(4e7 // max(A, 1)))
-    rows = np.zeros((N, A))
     starts = np.asarray(atom_ptr[:-1], dtype=np.int64)
     for r0 in range(0, A, step):
         blk = np.sqrt(((a[r0:r0 + step, None, :] - a[None, :, :]) ** 2).sum(-1))         # (step, A)
@@ -89,28 +88,48 @@ def residue_distance_matrix_fast(atoms, atom_ptr):
     return D
 
 
-def build_graph(protein, cutoff=30.0, max_neighbor=10, fast=True):
-    """-> dict(src, dst int32 (edges grouped by destination), he (E,27) f32, x (N,3) f32, mu_r_norm (N,5) f32,
-    res_feat (N,1) f32) for ONE protein: compute_dig_kNN_graph (protein_utils.py:311-397) after the unbound->bound
-    alignment (:279-308)."""
+def residue_distance_rows(atoms, atom_ptr, rows):
+    """Rows ``rows`` of the residue distance matrix, (len(rows), N) fp64 with inf at each row's own residue: that residue's
+    atoms against all atoms, O(rows x A) -- for proteins too large for the dense (A, A) matrix."""
+    a = atoms.astype(np.float64)
+    atom_ptr = np.asarray(atom_ptr, np.int64)
+    cnt = np.diff(atom_ptr).astype(np.float64)
+    out = np.empty((len(rows), len(atom_ptr) - 1))
+    for k, i in enumerate(rows):
+        blk = np.sqrt(((a[atom_ptr[i]:atom_ptr[i + 1], None, :] - a[None, :, :]) ** 2).sum(-1))   # (atoms of i, A)
+        out[k] = np.add.reduceat(blk.sum(0), atom_ptr[:-1]) / (cnt[i] * cnt)
+        out[k, i] = np.inf
+    return out
+
+
+def _align(protein, kabsch64):
+    """x (N,3) and the rotated local frames n, u, v of one protein after the unbound->bound alignment (:279-308)."""
     nca_c = np.asarray(protein['nca_c'], np.float32)
-    N = nca_c.shape[0]
     n_f, u_f, v_f = local_frames(nca_c)
     x = nca_c[:, 1].astype(np.float32)                                  # residue_loc_is_alphaC (:255-256)
-    R, t = kabsch(x.T.astype(np.float64) if False else x.T, np.asarray(protein['bound_ca'], np.float32).T)   # (:284-285)
-    x = ((R @ x.T) + t).T                                               # fp64 from here on, like the reference (:286-291)
-    n_f, u_f, v_f = (R @ n_f.T).T, (R @ u_f.T).T, (R @ v_f.T).T
-    atom_ptr = np.asarray(protein['atom_ptr'], np.int64)
-    D = (residue_distance_matrix_fast if fast else residue_distance_matrix)(np.asarray(protein['atoms'], np.float32), atom_ptr)
+    bound = np.asarray(protein['bound_ca'], np.float32)
+    if kabsch64:                  # fp64 fit, x and frames rotated in fp64 (the device's arithmetic)
+        x, bound = x.astype(np.float64), bound.astype(np.float64)
+    R, t = kabsch(x.T, bound.T)                                         # (:284-285)
+    x = ((R @ x.T) + t).T                                               # (:286-291)
+    return x, ((R @ n_f.T).T, (R @ u_f.T).T, (R @ v_f.T).T)
+
+
+def _graph_rows(D, rows, x, frames, cutoff, max_neighbor):
+    """compute_dig_kNN_graph (protein_utils.py:311-397) for destination rows ``rows``, D[k] = distance row of rows[k]."""
+    n_f, u_f, v_f = frames
     src, dst, dist, mu = [], [], [], []
-    for i in range(N):
-        valid = list(np.where(D[i, :] < cutoff)[0])                     # (:340)
+    for k, i in enumerate(rows):
+        valid = list(np.where(D[k, :] < cutoff)[0])                     # (:340)
         if len(valid) > max_neighbor:
-            valid = list(np.argsort(D[i, :]))[0:max_neighbor]            # (:342-343)
+            valid = list(np.argsort(D[k, :], kind='stable'))[0:max_neighbor]            # (:342-343)
         dst += [i] * len(valid)
         src += valid
-        dv = D[i, valid]
+        dv = D[k, valid]
         dist += list(dv)
+        if not valid:             # degree 0: the reference's w.max raises on the empty row; the device writes 0
+            mu.append(np.zeros(len(MU_SIGMAS)))
+            continue
         w = -dv.reshape(1, -1) ** 2 / MU_SIGMAS.reshape(-1, 1)          # softmax over the neighbours (:349-351)
         w = np.exp(w - w.max(axis=1, keepdims=True))
         w = w / w.sum(axis=1, keepdims=True)
@@ -123,9 +142,40 @@ def build_graph(protein, cutoff=30.0, max_neighbor=10, fast=True):
     basis = np.stack([n_f[dst], u_f[dst], v_f[dst]], axis=1)            # (E, 3, 3): rows n, u, v of the destination (:378)
     mm = lambda vec: np.einsum('erc,ec->er', basis, vec)
     ori = np.concatenate([mm(x[src] - x[dst]), mm(n_f[src]), mm(u_f[src]), mm(v_f[src])], axis=1).astype(np.float32)   # (:379-384)
-    return {'src': src.astype(np.int32), 'dst': dst.astype(np.int32), 'he': np.concatenate([rbf, ori], axis=1),
-            'x': x.astype(np.float32), 'mu_r_norm': np.asarray(mu).astype(np.float32),
-            'res_feat': np.asarray(protein['res_feat'], np.float32).reshape(-1, 1), 'dist': dist}
+    return {'src': src.astype(np.int32), 'dst': dst.astype(np.int32), 'he': np.concatenate([rbf, ori], axis=1).reshape(-1, 27),
+            'mu_r_norm': np.asarray(mu).astype(np.float32).reshape(-1, 5), 'dist': dist}
+
+
+def build_graph(protein, cutoff=30.0, max_neighbor=10, fast=True, kabsch64=False):
+    """-> dict(src, dst int32 (edges grouped by destination), he (E,27) f32, x (N,3) f32, mu_r_norm (N,5) f32,
+    res_feat (N,1) f32) for ONE protein: compute_dig_kNN_graph (protein_utils.py:311-397) after the unbound->bound
+    alignment (:279-308).
+
+    ``kabsch64=False`` aligns in fp32 like the reference (fp32 x and bound_ca into the SVD; R, t, x stay fp32, ~1e-7 |x|
+    from an fp64 fit); ``True`` fits and rotates x and the frames in fp64, the device's arithmetic.
+    Among more than ``max_neighbor`` residues inside the cutoff the closest are taken by a STABLE argsort: ascending
+    distance, exact ties by ascending index, the device's rule.  The reference's default argsort is not stable, so under
+    exact ties its order depends on the platform; without ties both are the same.
+    A residue with no neighbour inside the cutoff gets mu_r_norm = 0 (the reference raises on it)."""
+    atom_ptr = np.asarray(protein['atom_ptr'], np.int64)
+    N = atom_ptr.shape[0] - 1
+    x, frames = _align(protein, kabsch64)
+    D = (residue_distance_matrix_fast if fast else residue_distance_matrix)(np.asarray(protein['atoms'], np.float32), atom_ptr)
+    g = _graph_rows(D, range(N), x, frames, cutoff, max_neighbor)
+    g.update(x=x.astype(np.float32), res_feat=np.asarray(protein['res_feat'], np.float32).reshape(-1, 1))
+    return g
+
+
+def build_rows(protein, rows, cutoff=30.0, max_neighbor=10, kabsch64=False):
+    """``build_graph`` restricted to the destination residues ``rows`` (edges of each row in the order given; x and
+    mu_r_norm of those rows only), with distances computed per row (``residue_distance_rows``): the check of proteins of
+    thousands of residues."""
+    rows = [int(i) for i in rows]
+    x, frames = _align(protein, kabsch64)
+    D = residue_distance_rows(np.asarray(protein['atoms'], np.float32), protein['atom_ptr'], rows)
+    g = _graph_rows(D, rows, x, frames, cutoff, max_neighbor)
+    g['x'] = x[rows].astype(np.float32)
+    return g
 
 
 def build_pair(ligand, receptor, cutoff=30.0, max_neighbor=10):
