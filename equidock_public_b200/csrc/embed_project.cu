@@ -20,10 +20,11 @@ __global__ void embed_kernel(eqd_graph g, const float* __restrict__ emb, const f
   float4 v;
   if (q < 16) {
     // .view(-1).long() truncation of the fp32-encoded residue index (:460)
-    int r = (int)(lig ? res_l[ln] : res_r[ln]);
+    const float rf = lig ? res_l[ln] : res_r[ln];
+    int r = (int)rf;
     // nn.Embedding raises on an index outside [0, 21): flag it (the host raises in resolve_status); the clamp only
-    // keeps this launch memory-safe
-    if ((r < 0 || r >= EQD_N_RES_TYPES) && status && q == 0) atomicOr(status + g.n_pairs, EQD_STATUS_BAD_RESIDUE);
+    // keeps this launch memory-safe.  NaN converts to 0 here but to INT64_MIN under .long(): it is out of range too.
+    if ((rf != rf || r < 0 || r >= EQD_N_RES_TYPES) && status && q == 0) atomicOr(status + g.n_pairs, EQD_STATUS_BAD_RESIDUE);
     r = min(max(r, 0), EQD_N_RES_TYPES - 1);
     v = *reinterpret_cast<const float4*>(emb + r * 64 + q * 4);
   } else {

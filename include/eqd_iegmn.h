@@ -158,7 +158,14 @@ typedef struct eqd_head_params {
 
 int eqd_abi_version(void);
 
-/* Bytes of scratch the layer / head entry points need for this graph (host-side arithmetic). */
+/* Bytes of scratch the layer / head entry points need for this graph (host-side arithmetic).
+ * After eqd_keypoints the workspace holds, at byte offsets (round_up(v) = v rounded up to a multiple of 256, T =
+ * max(n_node_tiles, 1), B = n_pairs):
+ *   0                                              float part[T][64]   per node tile column sums of LeakyReLU(W_m h + b_m)
+ *   round_up(T*256)                                int tile_ptr[2B+1]  first node tile of every protein
+ *   q = round_up(T*256) + round_up((2B+1)*4)       double qbar[2B][64] mean-pooled queries (:525, :529), segment order
+ *   q + round_up(2B*64*8)                          double u[2B][50][64] u[s][k] = m_qk[k]^T qbar[partner of s]
+ * so the fp64 stages of the head can be checked one at a time.                                                      */
 size_t eqd_workspace_bytes(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs);
 
 /* Input stage, IEGMN.forward :452-471.

@@ -38,6 +38,7 @@ import torch
 import torch.nn.functional as F
 
 import backward_manual as bm
+import fp64_stages as fs
 import golden_io as gio
 import iegmn_oracle as orc
 from equidock_public_b200 import _native as nat
@@ -163,14 +164,6 @@ def _reduce(lib, vec, nparts, stride, src, dev):
     return out
 
 
-def _seg_pairs(plan):
-    """(segment, its partner segment, node range, partner range) for every protein of the batch."""
-    seg, B = plan.seg_ptr_host, plan.n_pairs
-    for s in range(2 * B):
-        p = s + B if s < B else s - B
-        yield s, p, (int(seg[s]), int(seg[s + 1])), (int(seg[p]), int(seg[p + 1]))
-
-
 # ---- node MLP -----------------------------------------------------------------------------------------------------
 
 @pytest.mark.parametrize('kind,li', [('bulk', 1), ('bulk', 0), ('ragged', 1), ('ragged', 0)])
@@ -273,11 +266,7 @@ def test_bwd_attention_vs_fp64_autograd(kind, li, qk_scale, cuda_device):
     kpre = torch.where(K > 0, K, K / slope).requires_grad_(True)
     v = V.clone().requires_grad_(True)
     q, k = F.leaky_relu(qpre, slope), F.leaky_relu(kpre, slope)
-    mu_ref = torch.zeros(N, dh, dtype=F64, device=dev)
-    parts = []
-    for s, p, (a, b), (c, d) in _seg_pairs(plan):
-        parts.append(torch.softmax(q[a:b] @ k[c:d].t(), 1) @ v[c:d])
-    mu_ref = torch.cat(parts, 0)
+    mu_ref = fs.attention(plan.seg_ptr_host, q, k, v)
     (mu_ref * _d(dmu[:, :dh])).sum().backward()
     mu = torch.zeros(N, dhp, device=dev)
     mu[:, :dh] = mu_ref.detach().float()           # the stashed forward output, rounded to fp32

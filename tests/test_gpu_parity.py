@@ -150,9 +150,9 @@ def test_single_layer_operator_matches_oracle(ds, name, li, models, cuda_device)
     assert np.abs(_np(out[2]) - xr).max() < 4e-6 * scale_x + 1e-5
 
 
-def _random_model(cuda_device, n_layers, shared, seed):
+def _random_model(cuda_device, n_layers, shared, seed, eta=0.0):
     args = gio.load_args('db5')
-    args.update({'iegmn_n_lays': n_layers, 'shared_layers': shared, 'skip_weight_h': 0.6})
+    args.update({'iegmn_n_lays': n_layers, 'shared_layers': shared, 'skip_weight_h': 0.6, 'x_connection_init': eta})
     torch.manual_seed(seed)
     from equidock_public_b200.rigid_docking_model import Rigid_Body_Docking_Net
     args['device'] = cuda_device
@@ -171,7 +171,18 @@ def _random_model(cuda_device, n_layers, shared, seed):
 def test_ragged_synthetic_graphs_vs_oracle(sizes, k, cuda_device):
     """Seeded random-init weights (default nn init, 3-layer unshared), ragged sizes incl. N < k+1 (in-degree < 10),
     N_l != N_r, tile boundaries (128/129, 257): engine == numpy fp64 oracle."""
-    model, args = _random_model(cuda_device, 3, False, seed=sum(a + b for a, b in sizes))
+    _ragged_vs_oracle(sizes, k, 0.0, cuda_device)
+
+
+def test_ragged_synthetic_graphs_with_x_connection_vs_oracle(cuda_device):
+    """x_connection_init = 0.3 (both shipped checkpoints have 0): every layer's coordinate update must mix in the
+    embedding-stage coordinates x0 (:286-292), not the layer's own input."""
+    _ragged_vs_oracle([(9, 40), (33, 5), (128, 129), (2, 2)], 10, 0.3, cuda_device)
+
+
+def _ragged_vs_oracle(sizes, k, eta, cuda_device):
+    model, args = _random_model(cuda_device, 3, False, seed=sum(a + b for a, b in sizes), eta=eta)
+    assert model.iegmn_original.iegmn_layers[1].packed(cuda_device).struct.dev.x_connection_init == pytest.approx(eta)
     rng = np.random.default_rng(len(sizes) * 100 + k)
     pairs = [synthetic.synthetic_pair(rng, a, b, k) for a, b in sizes]
     coors, kp_l, kp_r, rot, trans = model(gio.make_batch(pairs, cuda_device), epoch=0)
@@ -385,12 +396,14 @@ def test_model_on_unbatched_subgraph_with_misaligned_he(models, cuda_device):
 
 
 def test_out_of_range_residue_index_raises_like_nn_embedding(models, cuda_device):
+    """NaN too: .long() makes it INT64_MIN, so nn.Embedding raises; a plain float-to-int conversion would give 0."""
     names, pairs, outs, _ = gio.load_pairs('dips')
-    lig, rec = [dict(d) for d in pairs[names[0]]]
-    lig['res_feat'] = lig['res_feat'].copy()
-    lig['res_feat'][3, 0] = 21.0
-    with pytest.raises(IndexError):
-        models['dips'](gio.make_batch([(lig, rec)], cuda_device), epoch=0)
+    for bad in (21.0, float('nan')):
+        lig, rec = [dict(d) for d in pairs[names[0]]]
+        lig['res_feat'] = lig['res_feat'].copy()
+        lig['res_feat'][3, 0] = bad
+        with pytest.raises(IndexError):
+            models['dips'](gio.make_batch([(lig, rec)], cuda_device), epoch=0)
 
 
 def test_cuda_graph_replay_equals_eager_and_serves_new_batches(models, cuda_device):
