@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # EQD_LIB_PATH: load another build of the same ABI instead (A/B runs of kernel variants, scripts/forward_ab.py)
 LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.so')
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
@@ -95,6 +95,8 @@ PROTOTYPES = {
     'eqd_bwd_embed': (C.c_int, [_G, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_bwd_head_workspace_bytes': (C.c_size_t, [_i32, _i32, _i32]),
     'eqd_bwd_head': (C.c_int, [_G, _H] + [_vp] * 9 + [C.c_size_t] + [_vp] * 6),
+    'eqd_bwd_layer_inputs': (C.c_int, [_G, _L] + [_vp] * 5),
+    'eqd_bwd_inputs': (C.c_int, [_G] + [_vp] * 11),
     'eqd_losses_workspace_bytes': (C.c_size_t, [_i32, _i32]),
     'eqd_losses': (C.c_int, [_G] + [_vp] * 7 + [_i32, _i32, _f32, _f32, _f32, _f32, _vp, C.c_size_t] + [_vp] * 6),
     'eqd_graph_build_workspace_bytes': (C.c_size_t, [_i32]),

@@ -252,6 +252,7 @@ class GraphPlan:
         self.row_ptr = torch.searchsorted(self.edge_dst, torch.arange(self.N + 1, **i32), out_int32=True).contiguous()
         self.he_l, self.he_r = _aligned_he(he_l, device), _aligned_he(he_r, device)
         assert self.he_l.shape == (self.E_l, nat.EDGE_FEATS) and self.he_r.shape == (self.E_r, nat.EDGE_FEATS)
+        self.edge_perm = None   # (ligand, receptor) caller edge ids of a plan built from a sorted copy (_sorted_copy)
         seg = np.zeros(2 * self.n_pairs + 1, dtype=np.int64)
         seg[1:] = np.cumsum(np.asarray(n_lig + n_rec, dtype=np.int64))
         tiles = []
@@ -315,14 +316,16 @@ class GraphPlan:
 
 
 def _sorted_copy(plan_args):
-    """Slow path for graphs whose edges are not grouped by destination: stable sort + permute."""
+    """Slow path for graphs whose edges are not grouped by destination: stable sort + permute.  Returns the sorted
+    GraphPlan arguments and the (ligand, receptor) permutations: sorted edge i is the caller's edge perm[i]."""
     n_l, n_r, src_l, dst_l, src_r, dst_r, he_l, he_r, device, mid = plan_args
-    out = []
+    out, perms = [], []
     for s, d, he in ((src_l, dst_l, he_l), (src_r, dst_r, he_r)):
         perm = torch.sort(d.long(), stable=True).indices
         out.append((s[perm], d[perm], he[perm]))
+        perms.append(perm)
     (sl, dl, hl), (sr, dr, hr) = out
-    return n_l, n_r, sl, dl, sr, dr, hl, hr, device, mid
+    return (n_l, n_r, sl, dl, sr, dr, hl, hr, device, mid), tuple(perms)
 
 
 class _StatusPool:

@@ -19,8 +19,10 @@ Scope of this engine: forward AND backward of the configuration the shipped chec
 (``nonlin='lkyrelu'``, ``layer_norm='LN'``, ``layer_norm_coors='0'``, ``final_h_layer_norm='0'``,
 ``cross_msgs``, ``use_dist_in_layers``, ``rot_model='kb_att'``, ``fine_tune=False``, dropout inactive).
 Anything else raises ``NotImplementedError``; a missing CUDA library raises -- there is no CPU path.
-In training mode (``model.train()`` with grad enabled) the outputs of ``Rigid_Body_Docking_Net.forward`` are
-autograd-connected: the whole path is one autograd node backed by the CUDA backward kernels (``training.py``).
+In training mode (``model.train()`` with grad enabled), and in any mode when one of the graph's ``new_x`` / ``x`` /
+``mu_r_norm`` / ``he`` requires grad, the outputs of ``Rigid_Body_Docking_Net.forward`` are autograd-connected: the whole
+path is one autograd node backed by the CUDA backward kernels (``training.py``), differentiable with respect to every
+parameter and to those graph tensors.
 """
 import math  # noqa: F401  (re-exported, see module docstring)
 import sys  # noqa: F401
@@ -128,12 +130,21 @@ def _sorted_plan(graph, device, max_in_degree):
     args = (graph.batch_num_nodes(LIGAND).tolist(), graph.batch_num_nodes(RECEPTOR).tolist(), src_l.to(device),
             dst_l.to(device), src_r.to(device), dst_r.to(device), graph.edges[LL].data['he'].to(device),
             graph.edges[RR].data['he'].to(device), device, max_in_degree)
-    plan = GraphPlan(*_sorted_copy(args))
+    sorted_args, perms = _sorted_copy(args)
+    plan = GraphPlan(*sorted_args)
+    plan.edge_perm = perms        # scatters edge gradients back to the caller's edge order (training.TrainEngine)
     try:
         graph._eqd_plan = plan
     except AttributeError:
         pass
     return plan
+
+
+def graph_inputs(graph):
+    """The graph's floating-point tensors the reference differentiates through: ligand ``new_x``, receptor ``x``,
+    ligand / receptor ``mu_r_norm``, ``he`` of the ligand / receptor edges.  (``res_feat`` enters through ``.long()``.)"""
+    nl, nr = graph.nodes[LIGAND].data, graph.nodes[RECEPTOR].data
+    return nl['new_x'], nr['x'], nl['mu_r_norm'], nr['mu_r_norm'], graph.edges[LL].data['he'], graph.edges[RR].data['he']
 
 
 def _module_state(module):
@@ -411,24 +422,27 @@ class Rigid_Body_Docking_Net(nn.Module):
         return GraphedForward(self, device_batch)
 
     def forward(self, batch_hetero_graph, epoch):
-        if (self.training or getattr(self, 'force_autograd', False)) and torch.is_grad_enabled():
+        if torch.is_grad_enabled() and (self.training or getattr(self, 'force_autograd', False)
+                                        or any(t.requires_grad for t in graph_inputs(batch_hetero_graph))):
             return self._forward_autograd(batch_hetero_graph)
         return self._assemble(self.iegmn_original(batch_hetero_graph, epoch))
 
     def _forward_autograd(self, batch_hetero_graph):
-        """Training mode (``model.train()``, src/train.py:64): the whole hot path is ONE autograd node whose backward is the
-        hand-written CUDA backward (``training.TrainEngine``), so ``loss.backward()`` (train.py:154) fills ``param.grad`` of
-        every parameter exactly like the reference's autograd graph does.  Outputs are autograd-connected views of the
-        node's four raw outputs.  Evaluation under ``torch.no_grad()`` / ``model.eval()`` keeps the inference path."""
+        """Training mode (``model.train()``, src/train.py:64), or any mode when a graph input tensor requires grad: the
+        whole hot path is ONE autograd node whose backward is the hand-written CUDA backward (``training.TrainEngine``), so
+        ``loss.backward()`` (train.py:154) fills ``param.grad`` of every parameter and ``.grad`` of the graph's ``new_x`` /
+        ``x`` / ``mu_r_norm`` / ``he`` exactly like the reference's autograd graph does.  Outputs, and ``x_iegmn_out`` /
+        ``hv_iegmn_out`` in the graph, are autograd-connected views of the node's outputs.  Evaluation under
+        ``torch.no_grad()``, or in ``model.eval()`` with no input requiring grad, keeps the inference path."""
         from .training import autograd_forward
-        fwd, (coors, keypts, rot, trans) = autograd_forward(self, batch_hetero_graph, self.log)
+        fwd, (coors, keypts, rot, trans, x_fin, h_fin) = autograd_forward(self, batch_hetero_graph, self.log)
         plan = fwd['plan']
         B, N_l = plan.n_pairs, plan.N_l
         nl, nr = batch_hetero_graph.nodes[LIGAND].data, batch_hetero_graph.nodes[RECEPTOR].data
         dt = nl['new_x'].dtype
-        x_fin = fwd['x64'].to(dt)
+        x_fin = x_fin.to(dt)
         nl['x_iegmn_out'], nr['x_iegmn_out'] = x_fin[:N_l], x_fin[N_l:]
-        nl['hv_iegmn_out'], nr['hv_iegmn_out'] = fwd['h'][:N_l], fwd['h'][N_l:]
+        nl['hv_iegmn_out'], nr['hv_iegmn_out'] = h_fin[:N_l], h_fin[N_l:]
         self.iegmn_original.last_outputs = fwd
         keyp = keypts.to(dt)
         return (list(torch.split(coors, plan.n_lig_list, dim=0)), list(keyp[:B].unbind(0)), list(keyp[B:].unbind(0)),

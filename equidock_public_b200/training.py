@@ -5,7 +5,8 @@ losses.cu) driven over the C ABI, a ``torch.autograd.Function`` so that the refe
 src/train.py:98-165, 302).
 
 PyTorch is plumbing here too: device memory, streams, ``torch.distributed``; a few index ops build the by-source edge
-permutation once per batch topology.  No gradient arithmetic is done by torch.  There is no CPU fallback.
+permutation once per batch topology.  No gradient arithmetic is done by torch beyond adding the upstream gradients of
+the last layer's outputs (``x_iegmn_out`` / ``hv_iegmn_out``) to the head's.  There is no CPU fallback.
 
 Gradient layout: ONE flat fp32 buffer holding every unique parameter in the order [head, layer L-1, ..., layer 0,
 embedding] (the order the backward finishes them in, so that all-reduce buckets are contiguous and can start while
@@ -283,12 +284,18 @@ class TrainEngine:
                                            nat.ptr(flat), st), 'eqd_grad_reduce')
 
     def backward(self, fwd, d_coors, d_keypts, d_rot=None, d_trans=None, flat: Optional[torch.Tensor] = None,
-                 on_bucket_done=None, capture: Optional[list] = None) -> torch.Tensor:
+                 on_bucket_done=None, capture: Optional[list] = None, d_x_out=None, d_h_out=None,
+                 inputs_out: Optional[dict] = None) -> torch.Tensor:
         """Gradients of every parameter for upstream gradients w.r.t. the four raw outputs (ligand coordinates
-        (N_l,3) f32, keypoints (2B,50,3) f64, rotations (B,3,3) f32, translations (B,1,3) f32; any may be None).
+        (N_l,3) f32, keypoints (2B,50,3) f64, rotations (B,3,3) f32, translations (B,1,3) f32; any may be None) and
+        w.r.t. the last layer's coordinates and features (``d_x_out`` (N,3), ``d_h_out`` (N,64), global node order;
+        None = no loss on them).
         Returns the flat gradient buffer (see ParamLayout).  ``on_bucket_done(label, lo, hi)`` is called on the host
         right after the kernels that complete a bucket have been queued (the data-parallel trainer launches that
-        bucket's all-reduce there)."""
+        bucket's all-reduce there).  A dict ``inputs_out`` receives the gradients w.r.t. the graph's input tensors:
+        'x_lig' (N_l,3) and 'x_rec' (N_r,3) f64, 'mu_lig' / 'mu_rec' (N,5) f32, 'he_lig' / 'he_rec' (E,27) f32 in the
+        graph's own edge order.  Without it the input-gradient kernels are not launched; the parameter gradients are
+        the same either way."""
         lib, dev, lay_out = self.lib, self.device, self.layout
         plan: GraphPlan = fwd['plan']
         iegmn = self.iegmn
@@ -316,6 +323,14 @@ class TrainEngine:
                                        nat.ptr(d_rot), nat.ptr(d_trans), nat.ptr(ws.head_ws), ws.head_ws_bytes,
                                        nat.ptr(dh_cur), nat.ptr(dx_cur), nat.ptr(ws.dpre), nat.ptr(gk), nat.ptr(gq), st),
                       'eqd_bwd_head')
+            # eqd_bwd_head overwrote dh / dx: add the gradients that reach the last layer's outputs directly
+            if d_x_out is not None:
+                dx_cur.add_(d_x_out.detach().to(device=dev, dtype=torch.float64))
+            if d_h_out is not None:
+                dh_cur.reshape(-1)[:N * 64].view(N, 64).add_(d_h_out.detach().to(device=dev, dtype=_f32))
+            if inputs_out is not None:
+                dhe = torch.zeros(max(E, 1), nat.EDGE_FEATS, dtype=_f32, device=dev)
+                dx_orig = torch.zeros(N, 3, dtype=torch.float64, device=dev)
             if capture is not None:
                 capture.append({'head': True, 'dh': dh_cur.reshape(-1)[:N * 64].clone().view(N, 64), 'dx': dx_cur.clone()})
             hm = self.head_maps()
@@ -371,6 +386,9 @@ class TrainEngine:
                                            nat.ptr(ws.daggr), nat.ptr(dx_cur), nat.ptr(ws.ein), nat.ptr(ws.n1),
                                            nat.ptr(ws.msg), nat.ptr(ws.dz3), nat.ptr(ws.dmsg), nat.ptr(ws.dz1),
                                            nat.ptr(ws.dxrel), nat.ptr(ws.vec), C.byref(nparts), st), 'eqd_bwd_edge')
+                if inputs_out is not None:
+                    nat.check(lib.eqd_bwd_layer_inputs(g, lp, nat.ptr(ws.dz1), nat.ptr(dx_cur), nat.ptr(dhe),
+                                                       nat.ptr(dx_orig), st), 'eqd_bwd_layer_inputs')
                 self._reduce(ws.vec, nparts.value, 256, tp.maps['edgevec'], flat, st)
                 nch = self._tn(ws, ws.ein, 44, 44, ws.dz1, 64, 64, E, 1.0, False, st)
                 self._reduce(ws.partial, nch, 44 * 64, tp.maps['edge1'], flat, st)
@@ -407,36 +425,71 @@ class TrainEngine:
                                         nat.ptr(demb), st), 'eqd_bwd_embed')
             if on_bucket_done:
                 on_bucket_done('emb', *buckets['emb'])
+            if inputs_out is not None:
+                from .hetero_graph import LIGAND, RECEPTOR
+                dmu = torch.empty(N, 5, dtype=_f32, device=dev)
+                dx_in = torch.empty(N, 3, dtype=torch.float64, device=dev)
+                mu = [fwd['graph'].nodes[nt].data['mu_r_norm'].detach().to(device=dev, dtype=_f32).contiguous()
+                      for nt in (LIGAND, RECEPTOR)]
+                nat.check(lib.eqd_bwd_inputs(g, nat.ptr(ws.dh0), nat.ptr(dh_cur), nat.ptr(mu[0]), nat.ptr(mu[1]),
+                                             nat.ptr(dx_cur), nat.ptr(dx_orig), nat.ptr(fwd['rotation']), nat.ptr(d_coors),
+                                             nat.ptr(dmu), nat.ptr(dx_in), st), 'eqd_bwd_inputs')
+                N_l, E_l = plan.N_l, plan.E_l
+                dhe_l, dhe_r = dhe[:E_l], dhe[E_l:E]
+                if plan.edge_perm is not None:     # the plan holds a destination-sorted copy: sorted edge i = perm[i]
+                    dhe_l = torch.empty_like(dhe_l).index_copy_(0, plan.edge_perm[0].to(dev), dhe_l)
+                    dhe_r = torch.empty_like(dhe_r).index_copy_(0, plan.edge_perm[1].to(dev), dhe_r)
+                inputs_out.update(x_lig=dx_in[:N_l], x_rec=dx_in[N_l:], mu_lig=dmu[:N_l], mu_rec=dmu[N_l:],
+                                  he_lig=dhe_l, he_rec=dhe_r)
         return flat
 
 
+_INPUT_KEYS = ('x_lig', 'x_rec', 'mu_lig', 'mu_rec', 'he_lig', 'he_rec')   # TrainEngine.backward's inputs_out keys
+
+
 class _HotPath(torch.autograd.Function):
-    """autograd node of the whole hot path: forward = eqd_iegmn_forward with a stash, backward = the CUDA backward."""
+    """autograd node of the whole hot path: forward = eqd_iegmn_forward with a stash, backward = the CUDA backward.
+    Inputs: the graph's differentiable tensors (rigid_docking_model.graph_inputs; the forward reads them from the graph)
+    and every parameter.  Outputs: the four raw outputs, then the last layer's coordinates (N,3) f64 and features
+    (N,64) f32."""
 
     @staticmethod
-    def forward(ctx, holder, *params):
+    def forward(ctx, holder, x_lig, x_rec, mu_lig, mu_rec, he_lig, he_rec, *params):
         eng: TrainEngine = holder['engine']
         fwd = eng.forward(holder['graph'], holder.get('log'))
         holder['fwd'] = fwd
         ctx.holder = holder
-        return fwd['ligand_coors'], fwd['keypts'], fwd['rotation'], fwd['translation']
+        ctx.input_meta = [(t.dtype, t.device) for t in (x_lig, x_rec, mu_lig, mu_rec, he_lig, he_rec)]
+        ctx.set_materialize_grads(False)    # an unused side output then costs nothing in the backward
+        return fwd['ligand_coors'], fwd['keypts'], fwd['rotation'], fwd['translation'], fwd['x64'], fwd['h']
 
     @staticmethod
-    def backward(ctx, d_coors, d_keypts, d_rot, d_trans):
+    def backward(ctx, d_coors, d_keypts, d_rot, d_trans, d_x, d_h):
         holder = ctx.holder
         eng: TrainEngine = holder['engine']
-        flat = eng.backward(holder['fwd'], d_coors, d_keypts, d_rot, d_trans)
-        return (None, *eng.layout.views(flat))
+        fwd = holder['fwd']
+        # zeros for the raw outputs without a gradient, as autograd would materialise them
+        z = lambda d, key: torch.zeros_like(fwd[key]) if d is None else d
+        d_coors, d_keypts = z(d_coors, 'ligand_coors'), z(d_keypts, 'keypts')
+        d_rot, d_trans = z(d_rot, 'rotation'), z(d_trans, 'translation')
+        need = ctx.needs_input_grad[1:1 + len(_INPUT_KEYS)]
+        inputs = {} if any(need) else None
+        flat = eng.backward(fwd, d_coors, d_keypts, d_rot, d_trans, d_x_out=d_x, d_h_out=d_h, inputs_out=inputs)
+        in_grads = [inputs[k].to(device=dev, dtype=dt) if want else None
+                    for k, want, (dt, dev) in zip(_INPUT_KEYS, need, ctx.input_meta)]
+        return (None, *in_grads, *eng.layout.views(flat))
 
 
 def autograd_forward(model, graph, log=None):
-    """Runs the model's hot path as ONE autograd node and returns (raw outputs dict, the four differentiable tensors)."""
+    """Runs the model's hot path as ONE autograd node and returns (raw outputs dict, the six differentiable outputs:
+    ligand coordinates, keypoints, rotations, translations, last-layer coordinates (N,3) f64, last-layer features)."""
+    from .rigid_docking_model import graph_inputs
     eng = getattr(model, '_eqd_train_engine', None)
     if eng is None or eng.device != model.iegmn_original.residue_emb_layer.weight.device:
         eng = TrainEngine(model)
         model._eqd_train_engine = eng
     holder = {'engine': eng, 'graph': graph, 'log': log}
-    outs = _HotPath.apply(holder, *eng.layout.params)
+    outs = _HotPath.apply(holder, *graph_inputs(graph), *eng.layout.params)
     return holder['fwd'], outs
 
 

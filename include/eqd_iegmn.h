@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define EQD_ABI_VERSION 8
+#define EQD_ABI_VERSION 9
 
 #define EQD_EDGE_FEATS 27     /* input_edge_feats_dim, protein_utils.py:71-86 + :373-389 */
 #define EQD_N_RBF 15          /* all_sigmas_dist = 1.5**s, rigid_docking_model.py:116 */
@@ -394,6 +394,26 @@ int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const float* h, 
                  const float* x_lig_in, const float* dcoors, const double* dkeypts, const float* drot,
                  const float* dtrans, void* workspace, size_t workspace_bytes, float* dh, double* dx, float* dpre,
                  float* g_wkey, float* g_wquery, void* stream);
+
+/* ---- gradients w.r.t. the graph's input tensors (optional: the parameter gradients neither need nor change them) ----
+ * eqd_bwd_layer_inputs, once per layer right after eqd_bwd_edge (any layer order; each output element is accumulated by
+ * one thread, no atomics):
+ *   dhe[e][f]    += sum_n dz1[e][n] * w_edge1[f][n]   (f < 27: he enters every layer through edge_mlp.0, :229-231)
+ *   dx_orig[n]   += x_connection_init * dx_out[n]     (x_orig = the input coordinates in every layer, :286-292)
+ * dz1 [E][64] as eqd_bwd_edge leaves it (16-byte aligned), dx_out [n][3] fp64 = the gradient w.r.t. this layer's output
+ * coordinates (eqd_bwd_edge's dx_out); dhe [E][27] fp32 (ligand edges, then receptor edges), dx_orig [n][3] fp64:
+ * zero them before the first layer.
+ * eqd_bwd_inputs, once after the layer loop, per node n (global order):
+ *   dmu[n][c] = (dh0_acc[n][64+c] + dh_layer0[n][64+c]) / mu[n][c]       (c < 5; h0 = [emb | log mu_r_norm], :468-471)
+ *   dx[n]     = dx_layer0[n] + dx_orig[n]  (+ T_b^T dcoors[n] for a ligand node of pair b: ligand_out = T new_x + b, :665)
+ * dh0_acc / dh_layer0 [n][72] as eqd_bwd_embed takes them, mu_lig [N_l][5] / mu_rec [N_r][5] the forward's mu_r_norm,
+ * dx_layer0 [n][3] fp64 = the layer-0 dx_in of eqd_bwd_edge_gather, rot [B][9] = eqd_kabsch_apply's T, dcoors
+ * [N_l][3] or NULL.  Outputs (overwritten): dmu [n][5] fp32, dx [n][3] fp64.                                          */
+int eqd_bwd_layer_inputs(const eqd_graph* g, const eqd_layer* p, const float* dz1, const double* dx_out, float* dhe,
+                         double* dx_orig, void* stream);
+int eqd_bwd_inputs(const eqd_graph* g, const float* dh0_acc, const float* dh_layer0, const float* mu_lig,
+                   const float* mu_rec, const double* dx_layer0, const double* dx_orig, const float* rot,
+                   const float* dcoors, float* dmu, double* dx, void* stream);
 
 /* ---- training losses on the device (src/train.py:41-49, 112-150; src/utils/ot_utils.py:5-29) ------------------------
  * Per pair: MSE of the predicted ligand coordinates, body-intersection loss, pocket OT loss with the EXACT earth mover's
