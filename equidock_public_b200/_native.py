@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # EQD_LIB_PATH: load another build of the same ABI instead (A/B runs of kernel variants, scripts/forward_ab.py)
 LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.so')
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
@@ -79,6 +79,8 @@ PROTOTYPES = {
     'eqd_node_mlp_tc': (C.c_int, [_G, _L, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_node_stage_tc': (C.c_int, [_G, _L, _L, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_iegmn_layer_forward': (C.c_int, [_G, _L, _L, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'eqd_iegmn_layer_forward_stash': (C.c_int, [_G, _L, _L, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                _vp]),
     'eqd_head_fold': (C.c_int, [_H, _vp, _vp]),
     'eqd_forward_workspace_bytes': (C.c_size_t, [_G]),
     'eqd_iegmn_forward': (C.c_int, [_G, C.POINTER(_L), _i32, _H, C.POINTER(EqdForwardIO), _vp, C.c_size_t, _vp]),

@@ -22,7 +22,10 @@ Anything else raises ``NotImplementedError``; a missing CUDA library raises -- t
 In training mode (``model.train()`` with grad enabled), and in any mode when one of the graph's ``new_x`` / ``x`` /
 ``mu_r_norm`` / ``he`` requires grad, the outputs of ``Rigid_Body_Docking_Net.forward`` are autograd-connected: the whole
 path is one autograd node backed by the CUDA backward kernels (``training.py``), differentiable with respect to every
-parameter and to those graph tensors.
+parameter and to those graph tensors.  ``IEGMN.forward`` runs the same node under the same condition.  ``IEGMN_Layer.forward``
+is differentiable on its own under that condition (its ten tensor arguments in place of the graph tensors): each call is
+one autograd node whose backward is the CUDA per-layer backward (``training.layer_backward``), so models built from the
+layers train like the reference's.
 """
 import math  # noqa: F401  (re-exported, see module docstring)
 import sys  # noqa: F401
@@ -140,6 +143,34 @@ def _sorted_plan(graph, device, max_in_degree):
     return plan
 
 
+def _layer_plan(graph, device, max_in_degree, he_l, he_r):
+    """GraphPlan of an IEGMN_Layer call under autograd: the graph's cached plan when ``he_l`` / ``he_r`` are the tensors it
+    was built from, else one built with the caller's edge features.  Edges not grouped by destination get a
+    destination-sorted copy whose ``edge_perm`` maps edge gradients back to the caller's order."""
+    plan = _plan_for(graph, device, max_in_degree)
+    if plan.edge_perm is None and bool(plan.unsorted.item()):
+        plan = _sorted_plan(graph, device, max_in_degree)
+    if plan.edge_perm is None and he_l.data_ptr() == plan.he_l.data_ptr() and he_r.data_ptr() == plan.he_r.data_ptr():
+        return plan
+    src_l, dst_l = graph.edges(etype=LL)
+    src_r, dst_r = graph.edges(etype=RR)
+    args = (plan.n_lig_list, plan.n_rec_list, src_l.to(device), dst_l.to(device), src_r.to(device), dst_r.to(device),
+            he_l.detach().to(device), he_r.detach().to(device), device, max_in_degree)
+    if plan.edge_perm is None:
+        return GraphPlan(*args)
+    sorted_args, perms = _sorted_copy(args)
+    plan = GraphPlan(*sorted_args)
+    plan.edge_perm = perms
+    return plan
+
+
+def _wants_autograd(module, tensors):
+    """The condition under which a module's forward runs as an autograd node: grad mode on, and training mode,
+    ``force_autograd``, or an input tensor that requires grad."""
+    return torch.is_grad_enabled() and (module.training or getattr(module, 'force_autograd', False)
+                                        or any(t.requires_grad for t in tensors))
+
+
 def graph_inputs(graph):
     """The graph's floating-point tensors the reference differentiates through: ligand ``new_x``, receptor ``x``,
     ligand / receptor ``mu_r_norm``, ``he`` of the ligand / receptor edges.  (``res_feat`` enters through ``.long()``.)"""
@@ -223,9 +254,17 @@ class IEGMN_Layer(nn.Module):
                 original_edge_feats_ligand, orig_coors_ligand, coors_receptor, h_feats_receptor,
                 original_receptor_node_features, original_edge_feats_receptor, orig_coors_receptor):
         """Per-layer operator with the reference's signature and return value
-        ``(x_final_ligand, node_upd_ligand, x_final_receptor, node_upd_receptor)``."""
+        ``(x_final_ligand, node_upd_ligand, x_final_receptor, node_upd_receptor)``.  In training mode (grad enabled), with
+        ``force_autograd``, or when an input requires grad, the call is one autograd node whose backward is the CUDA
+        per-layer backward (``training.layer_backward``): gradients reach the layer's parameters and all ten tensor
+        inputs."""
         import ctypes as C
         self._check_mode()
+        inputs = (coors_ligand, h_feats_ligand, original_ligand_node_features, original_edge_feats_ligand,
+                  orig_coors_ligand, coors_receptor, h_feats_receptor, original_receptor_node_features,
+                  original_edge_feats_receptor, orig_coors_receptor)
+        if _wants_autograd(self, inputs):
+            return self._forward_autograd(hetero_graph, inputs)
         dev = coors_ligand.device
         eng = IEGMNEngine(dev)
         plan = _plan_for(hetero_graph, dev, self.graph_max_neighbor)
@@ -256,6 +295,14 @@ class IEGMN_Layer(nn.Module):
             raise nat.NativeLibraryError('IEGMN_Layer.forward: edges must be grouped by destination with in-degree '
                                          f'<= {self.graph_max_neighbor}')
         x_out = x_out.to(coors_ligand.dtype)
+        return x_out[:plan.N_l], h_out[:plan.N_l], x_out[plan.N_l:], h_out[plan.N_l:]
+
+    def _forward_autograd(self, hetero_graph, inputs):
+        from .training import layer_autograd
+        dev = inputs[0].device
+        plan = _layer_plan(hetero_graph, dev, self.graph_max_neighbor, inputs[3], inputs[8])
+        x_out, h_out = layer_autograd(self, plan, inputs)
+        x_out = x_out.to(inputs[0].dtype)
         return x_out[:plan.N_l], h_out[:plan.N_l], x_out[plan.N_l:], h_out[plan.N_l:]
 
     def __repr__(self):
@@ -360,8 +407,25 @@ class IEGMN(nn.Module):
 
     def forward(self, batch_hetero_graph, epoch):
         """Returns ``[T list, b list, Y_ligand list, Y_receptor list]`` like the reference (:602) and
-        writes ``x_iegmn_out`` / ``hv_iegmn_out`` into the graph (:507-510)."""
+        writes ``x_iegmn_out`` / ``hv_iegmn_out`` into the graph (:507-510).  Under the condition of
+        ``Rigid_Body_Docking_Net.forward`` the whole stack is the same single autograd node (``training._HotPath``)."""
+        if _wants_autograd(self, graph_inputs(batch_hetero_graph)):
+            return self._forward_autograd(batch_hetero_graph)
         return self.package(self.run_engine(batch_hetero_graph), batch_hetero_graph)
+
+    def _forward_autograd(self, batch_hetero_graph):
+        from .training import autograd_forward
+        fwd, (_, keypts, rot, trans, x_fin, h_fin) = autograd_forward(self, batch_hetero_graph, self.log)
+        plan = fwd['plan']
+        B, N_l = plan.n_pairs, plan.N_l
+        nl, nr = batch_hetero_graph.nodes[LIGAND].data, batch_hetero_graph.nodes[RECEPTOR].data
+        dt = nl['new_x'].dtype
+        x_fin = x_fin.to(dt)
+        nl['x_iegmn_out'], nr['x_iegmn_out'] = x_fin[:N_l], x_fin[N_l:]
+        nl['hv_iegmn_out'], nr['hv_iegmn_out'] = h_fin[:N_l], h_fin[N_l:]
+        self.last_outputs = fwd
+        keyp = keypts.to(dt)
+        return [list(rot.unbind(0)), list(trans.unbind(0)), list(keyp[:B].unbind(0)), list(keyp[B:].unbind(0))]
 
     def package(self, out, batch_hetero_graph):
         plan = out['plan']
@@ -422,8 +486,7 @@ class Rigid_Body_Docking_Net(nn.Module):
         return GraphedForward(self, device_batch)
 
     def forward(self, batch_hetero_graph, epoch):
-        if torch.is_grad_enabled() and (self.training or getattr(self, 'force_autograd', False)
-                                        or any(t.requires_grad for t in graph_inputs(batch_hetero_graph))):
+        if _wants_autograd(self, graph_inputs(batch_hetero_graph)):
             return self._forward_autograd(batch_hetero_graph)
         return self._assemble(self.iegmn_original(batch_hetero_graph, epoch))
 

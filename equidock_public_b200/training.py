@@ -27,10 +27,11 @@ _f32 = torch.float32
 
 
 class ParamLayout:
-    """Flat layout of a model's unique parameters in backward-completion order."""
+    """Flat layout of a model's unique parameters in backward-completion order.  ``model`` is a Rigid_Body_Docking_Net or
+    its IEGMN module (the same parameters; names keep the ``iegmn_original.`` prefix either way)."""
 
     def __init__(self, model):
-        iegmn = model.iegmn_original
+        iegmn = getattr(model, 'iegmn_original', model)
         seen, self.entries = set(), []          # (qualified name, param)
         self.buckets: List[tuple] = []          # (label, lo, hi) contiguous slices, in completion order
         self.module_bucket: Dict[int, str] = {}  # id(layer module) -> its bucket label
@@ -199,12 +200,103 @@ class BackwardWorkspace:
                                           torch.arange(N + 1, dtype=torch.int32, device=device), out_int32=True).contiguous()
 
 
+def _vp(t):
+    """A device pointer given as a tensor or already as c_void_p (a slice of the forward stash)."""
+    return t if t is None or isinstance(t, C.c_void_p) else nat.ptr(t)
+
+
+def _tn(lib, ws, X, ldx, K, D, ldd, ncols, nrows, alpha, want_colsum, st):
+    nch = C.c_int32(0)
+    nat.check(lib.eqd_tn_gemm(_vp(X), ldx, K, _vp(D), ldd, ncols, nrows, alpha, nat.ptr(ws.partial),
+                              nat.ptr(ws.colsum) if want_colsum else None, C.byref(nch), st), 'eqd_tn_gemm')
+    return nch.value
+
+
+def _reduce(lib, src_t, nch, stride, mp, flat, st):
+    nat.check(lib.eqd_grad_reduce(nat.ptr(src_t), nch, stride, nat.ptr(mp[0]), nat.ptr(mp[1]), int(mp[0].numel()),
+                                  nat.ptr(flat), st), 'eqd_grad_reduce')
+
+
+def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack, ws: BackwardWorkspace, h_in, x_in, aggr,
+                   mu, h0, dh_out, dx_out, dh_in, dx_in, flat, st, dhe=None, dx_orig=None, capture=None, li=None):
+    """Backward of ONE IEGMN_Layer, the fixed kernel sequence eqd_project (recompute) -> eqd_bwd_node_mlp ->
+    eqd_bwd_attention -> eqd_bwd_edge -> (eqd_bwd_layer_inputs) -> eqd_bwd_edge_gather -> eqd_bwd_project, with the weight
+    gradients of each stage through eqd_tn_gemm + eqd_grad_reduce.
+
+    The layer's stashed inputs (tensors or device pointers): h_in [N][dhp] f32 (row stride 72 for the 69-wide layer 0,
+    else 64), x_in [N][3] f64, aggr [N][64] f32, mu [N][dhp] f32, h0 [N][72] f32.  Upstream gradients: dh_out [N][64] f32
+    and dx_out [N][3] f64 of the layer's output features and coordinates.  Writes dh_in [N][dhp] and dx_in [N][3] f64
+    (overwritten), adds the gradient w.r.t. h0 into ws.dh0 and the parameter gradients into `flat` (through the index maps
+    of `tp`).  With dhe [E][27] f32 / dx_orig [N][3] f64 given, it also adds the gradients w.r.t. the edge features and the
+    original coordinates there (eqd_bwd_layer_inputs); without them that kernel is not launched.
+    Returns (dh_in, dx_in, ws.dh0, dhe, dx_orig)."""
+    g = C.byref(plan.struct)
+    N, E = plan.N, plan.E
+    lp = C.byref(lp_obj.struct)
+    dh, dhp, pw = tp.dh, tp.dhp, tp.pw
+    ldh = nat.H0_PAD if dh == nat.H0 else nat.HID
+    ldmu = nat.H0_PAD if dh == nat.H0 else nat.HID
+    h_in, x_in, aggr, mu, h0 = _vp(h_in), _vp(x_in), _vp(aggr), _vp(mu), _vp(h0)
+    nat.check(lib.eqd_project(g, lp, h_in, ldh, nat.ptr(ws.proj), st), 'eqd_project')
+    nparts = C.c_int32(0)
+    nat.check(lib.eqd_bwd_node_mlp(g, lp, nat.ptr(tp.t['w_node1_lin']), nat.ptr(tp.t['w_node2_lin']), h_in, ldh,
+                                   aggr, mu, ldmu, h0, nat.ptr(dh_out), nat.ptr(dh_in), nat.ptr(ws.daggr),
+                                   nat.ptr(ws.dmu), nat.ptr(ws.dh0), nat.ptr(ws.n5), nat.ptr(ws.du),
+                                   nat.ptr(ws.vec), C.byref(nparts), st), 'eqd_bwd_node_mlp')
+    _reduce(lib, ws.vec, nparts.value, 144, tp.maps['nodevec'], flat, st)
+    # node MLP weight gradients
+    sk = float(lp_obj.struct.dev.skip_weight_h) if dh == nat.HID else 1.0
+    nch = _tn(lib, ws, ws.n5, dhp, dhp, dh_out, 64, 64, N, sk, True, st)
+    _reduce(lib, ws.partial, nch, dhp * 64, tp.maps['node2'], flat, st)
+    _reduce(lib, ws.colsum, nch, 64, tp.maps['node2_bias'], flat, st)
+    for name, X, ldx, K, want in (('node_h', h_in, ldh, dhp, True), ('node_aggr', aggr, 64, 64, False),
+                                  ('node_mu', mu, ldmu, dhp, False), ('node_h0', h0, nat.H0_PAD, nat.H0_PAD, False)):
+        nchx = _tn(lib, ws, X, ldx, K, ws.du, dhp, dhp, N, 1.0, want, st)
+        _reduce(lib, ws.partial, nchx, K * dhp, tp.maps[name], flat, st)
+        if want:
+            _reduce(lib, ws.colsum, nchx, dhp, tp.maps['node1_bias'], flat, st)
+    nat.check(lib.eqd_bwd_attention(g, lp, nat.ptr(ws.proj), mu, ldmu, nat.ptr(ws.dmu), nat.ptr(ws.dP),
+                                    nat.ptr(ws.rowstat), st), 'eqd_bwd_attention')
+    nat.check(lib.eqd_bwd_edge(g, lp, nat.ptr(tp.t['w2lin']), nat.ptr(tp.t['w3lin']), nat.ptr(ws.proj), x_in,
+                               nat.ptr(ws.daggr), nat.ptr(dx_out), nat.ptr(ws.ein), nat.ptr(ws.n1),
+                               nat.ptr(ws.msg), nat.ptr(ws.dz3), nat.ptr(ws.dmsg), nat.ptr(ws.dz1),
+                               nat.ptr(ws.dxrel), nat.ptr(ws.vec), C.byref(nparts), st), 'eqd_bwd_edge')
+    if dhe is not None:
+        nat.check(lib.eqd_bwd_layer_inputs(g, lp, nat.ptr(ws.dz1), nat.ptr(dx_out), nat.ptr(dhe),
+                                           nat.ptr(dx_orig), st), 'eqd_bwd_layer_inputs')
+    _reduce(lib, ws.vec, nparts.value, 256, tp.maps['edgevec'], flat, st)
+    nch = _tn(lib, ws, ws.ein, 44, 44, ws.dz1, 64, 64, E, 1.0, False, st)
+    _reduce(lib, ws.partial, nch, 44 * 64, tp.maps['edge1'], flat, st)
+    nch = _tn(lib, ws, ws.n1, 64, 64, ws.dmsg, 64, 64, E, 1.0, True, st)
+    _reduce(lib, ws.partial, nch, 64 * 64, tp.maps['edge2'], flat, st)
+    _reduce(lib, ws.colsum, nch, 64, tp.maps['edge2_bias'], flat, st)
+    nch = _tn(lib, ws, ws.msg, 64, 64, ws.dz3, 64, 64, E, 1.0, True, st)
+    _reduce(lib, ws.partial, nch, 64 * 64, tp.maps['edge3'], flat, st)
+    _reduce(lib, ws.colsum, nch, 64, tp.maps['edge3_bias'], flat, st)
+    nat.check(lib.eqd_bwd_edge_gather(g, nat.ptr(ws.out_ptr), nat.ptr(ws.out_edge), nat.ptr(ws.dz1),
+                                      nat.ptr(ws.dxrel), nat.ptr(dx_out), float(lp_obj.struct.dev.x_connection_init),
+                                      nat.ptr(ws.dP), pw, nat.ptr(dx_in), st), 'eqd_bwd_edge_gather')
+    if capture is not None:
+        rows = lambda t, w, n=N: t.reshape(-1)[:n * w].clone().view(n, w)
+        capture.append({'layer': li, 'dh_part': rows(dh_in, dhp), 'daggr': ws.daggr.clone(), 'dmu': rows(ws.dmu, dhp),
+                        'dz1': ws.dz1[:E].clone(), 'dxrel': ws.dxrel[:E].clone(), 'dP': rows(ws.dP, pw),
+                        'dx': dx_in.clone(), 'dh0': ws.dh0.clone()})
+    nat.check(lib.eqd_bwd_project(g, lp, nat.ptr(tp.t['w_projT']), nat.ptr(ws.dP), nat.ptr(dh_in), st),
+              'eqd_bwd_project')
+    if capture is not None:
+        capture[-1]['dh'] = dh_in.reshape(-1)[:N * dhp].clone().view(N, dhp)
+    nchx = _tn(lib, ws, h_in, ldh, dhp, ws.dP, pw, pw, N, 1.0, True, st)
+    _reduce(lib, ws.partial, nchx, dhp * pw, tp.maps['proj'], flat, st)
+    _reduce(lib, ws.colsum, nchx, pw, tp.maps['proj_bias'], flat, st)
+    return dh_in, dx_in, ws.dh0, dhe, dx_orig
+
+
 class TrainEngine:
-    """Forward-with-stash and backward of one model on one device."""
+    """Forward-with-stash and backward of one model on one device (a Rigid_Body_Docking_Net, or an IEGMN module)."""
 
     def __init__(self, model):
         self.model = model
-        self.iegmn = model.iegmn_original
+        self.iegmn = getattr(model, 'iegmn_original', model)
         self.device = self.iegmn.residue_emb_layer.weight.device
         if self.device.type != 'cuda':
             raise nat.NativeLibraryError('training runs on a CUDA device only (no CPU fallback)')
@@ -274,14 +366,10 @@ class TrainEngine:
 
     # ---- backward -------------------------------------------------------------------------------------------------
     def _tn(self, ws, X, ldx, K, D, ldd, ncols, nrows, alpha, want_colsum, st):
-        nch = C.c_int32(0)
-        nat.check(self.lib.eqd_tn_gemm(nat.ptr(X), ldx, K, nat.ptr(D), ldd, ncols, nrows, alpha, nat.ptr(ws.partial),
-                                       nat.ptr(ws.colsum) if want_colsum else None, C.byref(nch), st), 'eqd_tn_gemm')
-        return nch.value
+        return _tn(self.lib, ws, X, ldx, K, D, ldd, ncols, nrows, alpha, want_colsum, st)
 
     def _reduce(self, src_t, nch, stride, mp, flat, st):
-        nat.check(self.lib.eqd_grad_reduce(nat.ptr(src_t), nch, stride, nat.ptr(mp[0]), nat.ptr(mp[1]), int(mp[0].numel()),
-                                           nat.ptr(flat), st), 'eqd_grad_reduce')
+        _reduce(self.lib, src_t, nch, stride, mp, flat, st)
 
     def backward(self, fwd, d_coors, d_keypts, d_rot=None, d_trans=None, flat: Optional[torch.Tensor] = None,
                  on_bucket_done=None, capture: Optional[list] = None, d_x_out=None, d_h_out=None,
@@ -328,6 +416,7 @@ class TrainEngine:
                 dx_cur.add_(d_x_out.detach().to(device=dev, dtype=torch.float64))
             if d_h_out is not None:
                 dh_cur.reshape(-1)[:N * 64].view(N, 64).add_(d_h_out.detach().to(device=dev, dtype=_f32))
+            dhe = dx_orig = None
             if inputs_out is not None:
                 dhe = torch.zeros(max(E, 1), nat.EDGE_FEATS, dtype=_f32, device=dev)
                 dx_orig = torch.zeros(N, 3, dtype=torch.float64, device=dev)
@@ -351,70 +440,11 @@ class TrainEngine:
                 first_use.setdefault(id(lm), li)
             for li in reversed(range(L)):
                 lm = iegmn.iegmn_layers[li]
-                lp_obj: PackedLayer = fwd['layers'][li]
-                tp = self.layer_pack(lm)
-                lp = C.byref(lp_obj.struct)
-                dh, dhp, pw = tp.dh, tp.dhp, tp.pw
                 h_in = h0_ptr if li == 0 else sp(so[3] + li * so[4])
-                ldh = nat.H0_PAD if li == 0 else nat.HID
                 x_in = sp(so[1] + li * so[2])
                 aggr, mu = sp(so[5] + li * so[6]), sp(so[7] + li * so[8])
-                ldmu = nat.H0_PAD if dh == nat.H0 else nat.HID
-                nat.check(lib.eqd_project(g, lp, h_in, ldh, nat.ptr(ws.proj), st), 'eqd_project')
-                nparts = C.c_int32(0)
-                nat.check(lib.eqd_bwd_node_mlp(g, lp, nat.ptr(tp.t['w_node1_lin']), nat.ptr(tp.t['w_node2_lin']), h_in, ldh,
-                                               aggr, mu, ldmu, h0_ptr, nat.ptr(dh_cur), nat.ptr(dh_nxt), nat.ptr(ws.daggr),
-                                               nat.ptr(ws.dmu), nat.ptr(ws.dh0), nat.ptr(ws.n5), nat.ptr(ws.du),
-                                               nat.ptr(ws.vec), C.byref(nparts), st), 'eqd_bwd_node_mlp')
-                self._reduce(ws.vec, nparts.value, 144, tp.maps['nodevec'], flat, st)
-                # node MLP weight gradients
-                sk = float(lp_obj.struct.dev.skip_weight_h) if dh == nat.HID else 1.0
-                nch = self._tn(ws, ws.n5, dhp, dhp, dh_cur, 64, 64, N, sk, True, st)
-                self._reduce(ws.partial, nch, dhp * 64, tp.maps['node2'], flat, st)
-                self._reduce(ws.colsum, nch, 64, tp.maps['node2_bias'], flat, st)
-                for name, X, ldx, K, want in (('node_h', h_in, ldh, dhp, True), ('node_aggr', aggr, 64, 64, False),
-                                              ('node_mu', mu, ldmu, dhp, False), ('node_h0', h0_ptr, nat.H0_PAD, nat.H0_PAD, False)):
-                    nchx = C.c_int32(0)
-                    nat.check(lib.eqd_tn_gemm(X, ldx, K, nat.ptr(ws.du), dhp, dhp, N, 1.0, nat.ptr(ws.partial),
-                                              nat.ptr(ws.colsum) if want else None, C.byref(nchx), st), 'eqd_tn_gemm')
-                    self._reduce(ws.partial, nchx.value, K * dhp, tp.maps[name], flat, st)
-                    if want:
-                        self._reduce(ws.colsum, nchx.value, dhp, tp.maps['node1_bias'], flat, st)
-                nat.check(lib.eqd_bwd_attention(g, lp, nat.ptr(ws.proj), mu, ldmu, nat.ptr(ws.dmu), nat.ptr(ws.dP),
-                                                nat.ptr(ws.rowstat), st), 'eqd_bwd_attention')
-                nat.check(lib.eqd_bwd_edge(g, lp, nat.ptr(tp.t['w2lin']), nat.ptr(tp.t['w3lin']), nat.ptr(ws.proj), x_in,
-                                           nat.ptr(ws.daggr), nat.ptr(dx_cur), nat.ptr(ws.ein), nat.ptr(ws.n1),
-                                           nat.ptr(ws.msg), nat.ptr(ws.dz3), nat.ptr(ws.dmsg), nat.ptr(ws.dz1),
-                                           nat.ptr(ws.dxrel), nat.ptr(ws.vec), C.byref(nparts), st), 'eqd_bwd_edge')
-                if inputs_out is not None:
-                    nat.check(lib.eqd_bwd_layer_inputs(g, lp, nat.ptr(ws.dz1), nat.ptr(dx_cur), nat.ptr(dhe),
-                                                       nat.ptr(dx_orig), st), 'eqd_bwd_layer_inputs')
-                self._reduce(ws.vec, nparts.value, 256, tp.maps['edgevec'], flat, st)
-                nch = self._tn(ws, ws.ein, 44, 44, ws.dz1, 64, 64, E, 1.0, False, st)
-                self._reduce(ws.partial, nch, 44 * 64, tp.maps['edge1'], flat, st)
-                nch = self._tn(ws, ws.n1, 64, 64, ws.dmsg, 64, 64, E, 1.0, True, st)
-                self._reduce(ws.partial, nch, 64 * 64, tp.maps['edge2'], flat, st)
-                self._reduce(ws.colsum, nch, 64, tp.maps['edge2_bias'], flat, st)
-                nch = self._tn(ws, ws.msg, 64, 64, ws.dz3, 64, 64, E, 1.0, True, st)
-                self._reduce(ws.partial, nch, 64 * 64, tp.maps['edge3'], flat, st)
-                self._reduce(ws.colsum, nch, 64, tp.maps['edge3_bias'], flat, st)
-                nat.check(lib.eqd_bwd_edge_gather(g, nat.ptr(ws.out_ptr), nat.ptr(ws.out_edge), nat.ptr(ws.dz1),
-                                                  nat.ptr(ws.dxrel), nat.ptr(dx_cur), float(lp_obj.struct.dev.x_connection_init),
-                                                  nat.ptr(ws.dP), pw, nat.ptr(dx_nxt), st), 'eqd_bwd_edge_gather')
-                if capture is not None:
-                    rows = lambda t, w, n=N: t.reshape(-1)[:n * w].clone().view(n, w)
-                    capture.append({'layer': li, 'dh_part': rows(dh_nxt, dhp), 'daggr': ws.daggr.clone(), 'dmu': rows(ws.dmu, dhp),
-                                    'dz1': ws.dz1[:E].clone(), 'dxrel': ws.dxrel[:E].clone(), 'dP': rows(ws.dP, pw),
-                                    'dx': dx_nxt.clone(), 'dh0': ws.dh0.clone()})
-                nat.check(lib.eqd_bwd_project(g, lp, nat.ptr(tp.t['w_projT']), nat.ptr(ws.dP), nat.ptr(dh_nxt), st),
-                          'eqd_bwd_project')
-                if capture is not None:
-                    capture[-1]['dh'] = dh_nxt.reshape(-1)[:N * dhp].clone().view(N, dhp)
-                nchx = C.c_int32(0)
-                nat.check(lib.eqd_tn_gemm(h_in, ldh, dhp, nat.ptr(ws.dP), pw, pw, N, 1.0, nat.ptr(ws.partial),
-                                          nat.ptr(ws.colsum), C.byref(nchx), st), 'eqd_tn_gemm')
-                self._reduce(ws.partial, nchx.value, dhp * pw, tp.maps['proj'], flat, st)
-                self._reduce(ws.colsum, nchx.value, pw, tp.maps['proj_bias'], flat, st)
+                layer_backward(lib, plan, fwd['layers'][li], self.layer_pack(lm), ws, h_in, x_in, aggr, mu, h0_ptr,
+                               dh_cur, dx_cur, dh_nxt, dx_nxt, flat, st, dhe, dx_orig, capture, li)
                 dh_cur, dh_nxt = dh_nxt, dh_cur
                 dx_cur, dx_nxt = dx_nxt, dx_cur
                 if on_bucket_done and first_use[id(lm)] == li:   # a shared module completes at its FIRST use
@@ -482,15 +512,146 @@ class _HotPath(torch.autograd.Function):
 
 def autograd_forward(model, graph, log=None):
     """Runs the model's hot path as ONE autograd node and returns (raw outputs dict, the six differentiable outputs:
-    ligand coordinates, keypoints, rotations, translations, last-layer coordinates (N,3) f64, last-layer features)."""
+    ligand coordinates, keypoints, rotations, translations, last-layer coordinates (N,3) f64, last-layer features).
+    ``model`` is a Rigid_Body_Docking_Net or an IEGMN module."""
     from .rigid_docking_model import graph_inputs
     eng = getattr(model, '_eqd_train_engine', None)
-    if eng is None or eng.device != model.iegmn_original.residue_emb_layer.weight.device:
+    if eng is None or eng.device != getattr(model, 'iegmn_original', model).residue_emb_layer.weight.device:
         eng = TrainEngine(model)
         model._eqd_train_engine = eng
     holder = {'engine': eng, 'graph': graph, 'log': log}
     outs = _HotPath.apply(holder, *graph_inputs(graph), *eng.layout.params)
     return holder['fwd'], outs
+
+
+# ---- one IEGMN_Layer as an autograd node ------------------------------------------------------------------------------
+
+class LayerLayout:
+    """Flat gradient layout of ONE IEGMN_Layer module: its parameters in ``module.parameters()`` order, each on a 256-byte
+    boundary as in ParamLayout (LayerTrainPack's index maps read ``offset``)."""
+
+    def __init__(self, layer_module):
+        self.params, self.offset, self.total = [], {}, 0
+        for p in layer_module.parameters():
+            self.offset[id(p)] = self.total
+            self.params.append(p)
+            self.total += (p.numel() + 63) & ~63
+
+    views = ParamLayout.views
+
+
+def layer_train_pack(layer_module, packed: PackedLayer, device):
+    """(LayerLayout, LayerTrainPack) of a layer module for its current packed weights, cached on the module; the index
+    maps are built once per module and device."""
+    hit = getattr(layer_module, '_eqd_layer_train', None)
+    if hit is not None and hit[0] is packed:
+        return hit[1], hit[2]
+    if hit is not None and hit[2].maps['proj'][0].device == torch.device(device):
+        layout, maps = hit[1], hit[2].maps
+    else:
+        layout, maps = LayerLayout(layer_module), None
+    tp = LayerTrainPack(layer_module, packed, layout, device, maps)
+    layer_module._eqd_layer_train = (packed, layout, tp)
+    return layout, tp
+
+
+class _LayerFn(torch.autograd.Function):
+    """autograd node of one IEGMN_Layer call: forward = eqd_project + eqd_iegmn_layer_forward_stash, backward =
+    layer_backward.  Inputs: the ten floating-point tensors of IEGMN_Layer.forward (ligand coordinates, features, original
+    features, edge features, original coordinates, then the receptor's five) and the layer's parameters.  Outputs: the
+    layer's coordinates (N,3) f64 and features (N,64) f32 of both proteins in global node order."""
+
+    @staticmethod
+    def forward(ctx, holder, x_l, h_l, h0_l, he_l, xo_l, x_r, h_r, h0_r, he_r, xo_r, *params):
+        module, plan = holder['module'], holder['plan']
+        dev = x_l.device
+        lib = nat.load()
+        lay = module.packed(dev)
+        layout, tp = layer_train_pack(module, lay, dev)
+        N, dhp = plan.N, lay.dhp
+        f32, f64 = dict(dtype=_f32, device=dev), dict(dtype=torch.float64, device=dev)
+        h = torch.zeros(N, dhp, **f32)
+        h[:, :lay.dh] = torch.cat([h_l, h_r])
+        h0 = torch.zeros(N, nat.H0_PAD, **f32)
+        h0[:, :nat.H0] = torch.cat([h0_l, h0_r])
+        x_in = torch.cat([x_l, x_r]).to(**f64).contiguous()
+        x_orig = torch.cat([xo_l, xo_r]).to(**f64).contiguous()
+        proj = torch.empty(N, 128 + 3 * dhp, **f32)
+        aggr, mu, h_out = torch.empty(N, nat.HID, **f32), torch.empty(N, dhp, **f32), torch.empty(N, nat.HID, **f32)
+        x_out = torch.empty(N, 3, **f64)
+        status = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            g, lp = C.byref(plan.struct), C.byref(lay.struct)
+            nat.check(lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
+            nat.check(lib.eqd_iegmn_layer_forward_stash(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
+                                                        nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(mu),
+                                                        nat.ptr(h_out), nat.ptr(x_out), nat.ptr(status), st),
+                      'eqd_iegmn_layer_forward_stash')
+        if int(status[plan.n_pairs].item()) & nat.STATUS_DEGREE_OVERFLOW:
+            raise nat.NativeLibraryError(f'IEGMN_Layer.forward: in-degree above {plan.struct.max_in_degree}')
+        ctx.saved = (plan, lay, layout, tp, h, h0, x_in, aggr, mu)
+        ctx.input_meta = [(t.dtype, t.device) for t in (x_l, h_l, h0_l, he_l, xo_l, x_r, h_r, h0_r, he_r, xo_r)]
+        ctx.set_materialize_grads(False)    # a loss on only one of the two outputs launches nothing for the other
+        return x_out, h_out
+
+    @staticmethod
+    def backward(ctx, d_x, d_h):
+        plan, lay, layout, tp, h, h0, x_in, aggr, mu = ctx.saved
+        n_in = len(ctx.input_meta)
+        if d_x is None and d_h is None:
+            return (None,) * (1 + n_in + len(layout.params))
+        dev, lib = h.device, nat.load()
+        N, E, N_l, E_l = plan.N, plan.E, plan.N_l, plan.E_l
+        need = ctx.needs_input_grad[1:1 + n_in]
+        with torch.cuda.device(dev):
+            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            ws = getattr(plan, '_eqd_layer_ws', None)
+            if ws is None:
+                ws = plan._eqd_layer_ws = BackwardWorkspace(plan, dev)
+            # fresh, 16-byte aligned operands: every gradient handed to autograd is its own tensor, never the workspace
+            dh_out = torch.zeros(N, nat.HID, dtype=_f32, device=dev)
+            dx_out = torch.zeros(N, 3, dtype=torch.float64, device=dev)
+            if d_h is not None:
+                dh_out.copy_(d_h)
+            if d_x is not None:
+                dx_out.copy_(d_x)
+            dh_in = torch.empty(N, lay.dhp, dtype=_f32, device=dev)
+            dx_in = torch.empty(N, 3, dtype=torch.float64, device=dev)
+            dhe = dx_orig = None
+            if need[3] or need[4] or need[8] or need[9]:
+                dhe = torch.zeros(max(E, 1), nat.EDGE_FEATS, dtype=_f32, device=dev)
+                dx_orig = torch.zeros(N, 3, dtype=torch.float64, device=dev)
+            flat = torch.zeros(layout.total, dtype=_f32, device=dev)
+            ws.dh0.zero_()
+            layer_backward(lib, plan, lay, tp, ws, h, x_in, aggr, mu, h0, dh_out, dx_out, dh_in, dx_in, flat, st, dhe,
+                           dx_orig)
+            dh0 = ws.dh0[:, :nat.H0].clone() if need[2] or need[7] else None
+            if dhe is not None:
+                dhe_l, dhe_r = dhe[:E_l], dhe[E_l:E]
+                if plan.edge_perm is not None:     # the plan holds a destination-sorted copy: sorted edge i = perm[i]
+                    dhe_l = torch.empty_like(dhe_l).index_copy_(0, plan.edge_perm[0].to(dev), dhe_l)
+                    dhe_r = torch.empty_like(dhe_r).index_copy_(0, plan.edge_perm[1].to(dev), dhe_r)
+        dh_in = dh_in[:, :lay.dh]
+        per_side = {0: dx_in, 1: dh_in, 2: dh0, 4: dx_orig}
+        grads = []
+        for i, ((dt, d), want) in enumerate(zip(ctx.input_meta, need)):
+            k, lig = i % 5, i < 5
+            if not want:
+                grads.append(None)
+            elif k == 3:
+                grads.append((dhe_l if lig else dhe_r).to(device=d, dtype=dt))
+            else:
+                t = per_side[k]
+                grads.append((t[:N_l] if lig else t[N_l:]).to(device=d, dtype=dt))
+        p_need = ctx.needs_input_grad[1 + n_in:]
+        return (None, *grads, *[v if want else None for v, want in zip(layout.views(flat), p_need)])
+
+
+def layer_autograd(module, plan: GraphPlan, inputs):
+    """Runs one IEGMN_Layer call as an autograd node (see _LayerFn); ``inputs`` are the ten floating-point tensors of
+    IEGMN_Layer.forward in its argument order.  Returns (coordinates (N,3) f64, features (N,64) f32), global node order."""
+    return _LayerFn.apply({'module': module, 'plan': plan}, *inputs, *module.parameters())
 
 
 # ---- fused data-parallel training step -------------------------------------------------------------------------------

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define EQD_ABI_VERSION 9
+#define EQD_ABI_VERSION 10
 
 #define EQD_EDGE_FEATS 27     /* input_edge_feats_dim, protein_utils.py:71-86 + :373-389 */
 #define EQD_N_RBF 15          /* all_sigmas_dist = 1.5**s, rigid_docking_model.py:116 */
@@ -263,6 +263,14 @@ int eqd_iegmn_layer_forward(const eqd_graph* g, const eqd_layer* p, const eqd_la
                             const double* x_in, const double* x_orig,
                             float* proj, float* proj_next, float* aggr,
                             float* h_out, double* x_out, int32_t* status, void* stream);
+/* Same outputs (bit for bit), and the layer's attention output mu [n][dhp] (row stride 72 with columns 69..71 zero for
+ * the 69-wide layer 0, 64 otherwise; 16-byte aligned, required): the operand of eqd_bwd_node_mlp / eqd_bwd_attention
+ * that the per-layer backward reads together with h_in, h0, x_in and aggr.                                    */
+int eqd_iegmn_layer_forward_stash(const eqd_graph* g, const eqd_layer* p, const eqd_layer* p_next,
+                                  const float* h_in, int32_t ldh, const float* h0,
+                                  const double* x_in, const double* x_orig,
+                                  float* proj, float* proj_next, float* aggr, float* mu,
+                                  float* h_out, double* x_out, int32_t* status, void* stream);
 
 /* Weights-only fold of the 50-head key / query projections (att_mlp_key_ROT, att_mlp_query_ROT :427-438) into
  * m_qk (see eqd_head_params), so that the per-protein logits are h_j . (m_qk[k]^T qbar) (:544-546, :555-557).
