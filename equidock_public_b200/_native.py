@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # EQD_LIB_PATH: load another build of the same ABI instead (A/B runs of kernel variants, scripts/forward_ab.py)
 LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.so')
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
@@ -49,8 +49,9 @@ class EqdLayer(C.Structure):
 
 class EqdForwardIO(C.Structure):
     _fields_ = [(n, _vp) for n in ('emb', 'res_lig', 'res_rec', 'mu_lig', 'mu_rec', 'x_lig', 'x_rec', 'rot', 'trans',
-                                   'ligand_out', 'sing', 'status', 'h_out', 'x_out', 'keypts', 'cov', 'ymean', 'stage_events')] + \
-               [('layer0_fp32', _i32), ('train_stash', _vp), ('train_stash_bytes', C.c_size_t)]
+                                   'ligand_out', 'sing', 'status', 'h_out', 'x_out', 'keypts', 'cov', 'ymean', 'stage_events',
+                                   'train_stash')] + \
+               [('train_stash_bytes', C.c_size_t)]
 
 
 class EqdHeadParams(C.Structure):
@@ -67,7 +68,7 @@ PROTOTYPES = {
     'eqd_project': (C.c_int, [_G, _L, _vp, _i32, _vp, _vp]),
     'eqd_edge_stage': (C.c_int, [_G, _L, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_edge_stage_ffma': (C.c_int, [_G, _L, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    'eqd_node_stage': (C.c_int, [_G, _L, _L, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'eqd_node_stage': (C.c_int, [_G, _L, _L, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_kv_blocks_bytes': (C.c_size_t, [_i32]),
     'eqd_project_tc': (C.c_int, [_G, _L, _vp, _vp, _vp, _vp]),
     'eqd_project_tc0': (C.c_int, [_G, _L, _vp, _vp, _vp, _vp, _vp]),
@@ -78,9 +79,8 @@ PROTOTYPES = {
     'eqd_attention_tc': (C.c_int, [_G, _vp, _vp, _vp, _vp]),
     'eqd_node_mlp_tc': (C.c_int, [_G, _L, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_node_stage_tc': (C.c_int, [_G, _L, _L, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    'eqd_iegmn_layer_forward': (C.c_int, [_G, _L, _L, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    'eqd_iegmn_layer_forward_stash': (C.c_int, [_G, _L, _L, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                                                _vp]),
+    'eqd_iegmn_layer_forward': (C.c_int, [_G, _L, _L, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _vp]),
     'eqd_head_fold': (C.c_int, [_H, _vp, _vp]),
     'eqd_forward_workspace_bytes': (C.c_size_t, [_G]),
     'eqd_iegmn_forward': (C.c_int, [_G, C.POINTER(_L), _i32, _H, C.POINTER(EqdForwardIO), _vp, C.c_size_t, _vp]),

@@ -16,14 +16,6 @@
 
 namespace eqd {
 
-// -DATTN_PROF: thread 0 of CTA 0 accumulates the SM cycles it spends in each phase of the tile loop (scripts/attn_variants.py)
-#ifdef ATTN_PROF
-__device__ long long g_attn_prof[16];
-#define PROF_MARK(k) do { if (tid == 0 && blockIdx.x == 0) { const long long t_ = clock64(); prof_acc[k] += t_ - prof_t; prof_t = t_; } } while (0)
-#else
-#define PROF_MARK(k) do { } while (0)
-#endif
-
 #define AT_THREADS 256
 #define AT_KEYS 64            // keys per chunk = 8 blocks
 #define AT_CHUNK_BYTES 8192   // per split
@@ -54,7 +46,6 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
   AtSmem& S = *reinterpret_cast<AtSmem*>(smem_raw);
   const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, wgi = tid >> 7;
   AtGroupSmem& G = S.grp;
-  TRACE_START(1);
   if (tid == 0) {
     for (int b = 0; b < 2; ++b) {
       mbar_init(&S.k_bar[b], 1);
@@ -62,9 +53,7 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (q == 0) TRACE_PHASE(1, blockIdx.x, 0, 14);
   __syncthreads();
-  if (q == 0) TRACE_PHASE(1, blockIdx.x, 0, 13);
   const unsigned k_saddr = smem_u32(G.k), v_saddr = smem_u32(G.v);
   const unsigned qa_saddr = smem_u32(S.qa), pa_saddr = smem_u32(S.pa);
   float* const dtile = reinterpret_cast<float*>(S.pa);
@@ -115,15 +104,7 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
     wg_store_d<64>(dtile + wgi * 64 * AT_LD, AT_LD, d, tid & 127);
   };
 
-#ifdef ATTN_PROF
-  __shared__ long long prof_acc[16];
-  long long prof_t = clock64();
-  if (tid == 0)
-    for (int k = 0; k < 16; ++k) prof_acc[k] = 0;
-#endif
   for (int tile = blockIdx.x; tile < g.n_node_tiles; tile += gridDim.x) {
-    PROF_MARK(15);
-    if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, 1);
     const int seg = g.node_tiles[2 * tile], node0 = g.node_tiles[2 * tile + 1];
     const int nvalid = min(EQD_TM, g.seg_ptr[seg + 1] - node0);
     const int pseg = seg < B ? seg + B : seg - B;
@@ -132,7 +113,6 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
     const int nchunks = (blk_hi - blk_lo + 7) >> 3;
     const int node = node0 + r;
     const bool valid = r < nvalid;
-    PROF_MARK(0);   // tile metadata (dependent global loads)
     if (nchunks > 0) load_chunk(k_g, G.k[0], &S.k_bar[0], blk_lo, 0);
     float q5[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
     if (valid) {
@@ -151,22 +131,17 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
     }
     tc_fence_before();
     __syncthreads();
-    PROF_MARK(1);   // Q row -> A + barrier
     // ---------------- pass 1: row maxima ----------------------------------------------------------------
     float mx = -INFINITY;
     for (int c = 0; c < nchunks; ++c) {
       const int kb_ = c & 1;
-      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 2);
       mbar_wait(&S.k_bar[kb_], kph[kb_]);
       kph[kb_] ^= 1;
-      PROF_MARK(2);   // pass 1: K chunk wait
       // the other K buffer was last read by the S GEMM of chunk c-1, complete before the last barrier: prefetch into it
       if (c + 1 < nchunks) load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[kb_ ^ 1], blk_lo + 8 * (c + 1), kb_ ^ 1);
       else load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[kb_ ^ 1], blk_lo, kb_ ^ 1);   // first chunk of pass 2
-      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 3);
       gemm_s(kb_, true);
       __syncthreads();
-      PROF_MARK(3);   // pass 1: S(hi) MMAs
       float s[32];
       tile_ld32f(dtile, AT_LD, r, half * 32, s);
       add_s5(s, G.x5c[kb_], q5);
@@ -177,7 +152,6 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
         mx = fmaxf(mx, (kn >= j0 && kn < j1) ? s[i] : -INFINITY);
       }
       __syncthreads();  // S drained before the next S GEMM overwrites it
-      PROF_MARK(4);   // pass 1: ld + max + barrier
     }
     G.red[r * 2 + half] = mx;
     __syncthreads();
@@ -191,18 +165,14 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
     float o5[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
     for (int c = 0; c < nchunks; ++c) {
       const int kb_ = (nchunks + c) & 1, vb_ = c & 1;   // K buffers keep alternating after pass 1
-      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 4);
       mbar_wait(&S.k_bar[kb_], kph[kb_]);
       kph[kb_] ^= 1;
-      PROF_MARK(5);   // pass 2: K chunk wait (+ row-max exchange on the first chunk)
       if (c + 1 < nchunks) {
         load_chunk(k_g, G.k[kb_ ^ 1], &S.k_bar[kb_ ^ 1], blk_lo + 8 * (c + 1), kb_ ^ 1);
         load_chunk(v_g, G.v[vb_ ^ 1], &S.v_bar[vb_ ^ 1], blk_lo + 8 * (c + 1), -1);   // its last reader (P V of c-1) is done
       }
-      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 5);
       gemm_s(kb_, false);
       __syncthreads();
-      PROF_MARK(6);   // pass 2: S MMAs
       float s[32];
       tile_ld32f(dtile, AT_LD, r, half * 32, s);
       add_s5(s, G.x5c[kb_], q5);
@@ -225,20 +195,14 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
         }
       }
       l += (l4[0] + l4[1]) + (l4[2] + l4[3]);
-      PROF_MARK(7);   // pass 2: ld + exp
       __syncthreads();  // every S value is in registers: the P splits may overwrite the S tile
-      PROF_MARK(8);   // pass 2: barrier 1
       store_half_split3<EQD_TM>(S.pa, AT_A_SPLIT, r, half * 32, s);
       tc_fence_before();
       __syncthreads();
-      PROF_MARK(9);   // pass 2: P split/store + barrier 2
-      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 6);
       mbar_wait(&S.v_bar[vb_], vph[vb_]);
       vph[vb_] ^= 1;
       gemm_pv(vb_);
       __syncthreads();
-      if (q == 0) TRACE_PHASE(1, blockIdx.x, tile, (c << 4) | 7);
-      PROF_MARK(10);  // pass 2: V wait + P.V MMAs
       // The tensor core truncates (round-toward-zero) every time it adds into an fp32 accumulator, a systematic
       // bias that grows with the number of accumulation steps; each 64-key chunk is therefore accumulated on its
       // own (4 full-magnitude steps) and the chunks are summed here with round-to-nearest FADDs.
@@ -251,7 +215,6 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
       // Every thread has read its O row (the next S tile overwrites it), and has observed this chunk's v_bar phase
       // before the V refill two chunks ahead re-arms that mbarrier.
       __syncthreads();
-      PROF_MARK(11);  // pass 2: O ld + accumulate + barrier 3
     }
     // ---------------- mu = O / l -----------------------------------------------------------------------------
     G.red[r * 2 + half] = l;
@@ -280,14 +243,7 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
       }
     }
     __syncthreads();
-    PROF_MARK(12);  // mu = O / l, stores, barrier
   }
-#ifdef ATTN_PROF
-  if (tid == 0 && blockIdx.x == 0)
-    for (int k = 0; k < 16; ++k) g_attn_prof[k] = prof_acc[k];
-#endif
-  if (q == 0) TRACE_PHASE(1, blockIdx.x, 0xffff, 15);
-  TRACE_END(1);
 }
 
 // ---- the 64-wide layers ---------------------------------------------------------------------------------------------
@@ -323,7 +279,6 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
   AtChainSmem& W = reinterpret_cast<AtChainSmem*>(smem_raw)[threadIdx.x >> 7];
   const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, lane = t & 31;
   const int bar = 1 + wgi;   // this chain's named barrier
-  TRACE_START(1);
   if (t == 0) {
     for (int b = 0; b < 2; ++b) {
       mbar_init(&W.k_bar[b], 1);
@@ -384,7 +339,6 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
   bool k_ahead = false, v_ahead = false;   // the current tile's first K / V chunk is already in flight
   if (kt >= 0) stage_q(cur);
   while (kt >= 0) {
-    if (t == 0) TRACE_PHASE(1, chain, kt, 1);
     // The next tile's metadata (dependent global loads) and Q rows are fetched once the first S GEMM of pass 1 is in flight.
     int ktn = -1;
     bool looked = false;
@@ -514,18 +468,9 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
     cur = nxt;
   }
   cp_async_wait<0>();
-  TRACE_END(1);
 }
 
 }  // namespace eqd
-
-EQD_TRACE_SETTER(eqd_trace_set_attn)
-
-#ifdef ATTN_PROF
-extern "C" int eqd_attn_prof_read(long long* out16) {
-  return (int)cudaMemcpyFromSymbol(out16, eqd::g_attn_prof, sizeof(long long) * 16);
-}
-#endif
 
 extern "C" int eqd_attention_tc(const eqd_graph* g, const float* proj, const void* kv, float* mu, void* stream) {
   if (!g || !proj || !kv || !mu) return EQD_ERR_BAD_ARG;

@@ -43,31 +43,6 @@
 
 namespace eqd {
 
-// ---- optional flight recorder (builds with -DEQD_TRACE only; scripts/hang_trace.py) -------------------------------
-// eqd_trace points at host-mapped memory: [kernel 0..7][1024] (EQD_TRACE=2 only) per-(CTA, tile group) progress words = tile << 8 | phase,
-// then [8192 + k] = launches started, [8200 + k] = CTAs finished.
-#ifdef EQD_TRACE
-static __device__ int* eqd_trace = nullptr;
-#define EQD_TRACE_SETTER(name) \
-  extern "C" void name(void* p) { int* q = (int*)p; cudaMemcpyToSymbol(eqd::eqd_trace, &q, sizeof(q)); }
-#if EQD_TRACE >= 2
-#define TRACE_PHASE(k, slot, tile, phase) \
-  do { if (eqd_trace) reinterpret_cast<volatile int*>(eqd_trace)[(k) * 1024 + (slot)] = ((tile) << 8) | (phase); } while (0)
-#else
-#define TRACE_PHASE(k, slot, tile, phase) do { } while (0)
-#endif
-#define TRACE_START(k) \
-  do { if (eqd_trace && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd_system(eqd_trace + 8192 + (k), 1); } while (0)
-#define TRACE_END(k) \
-  do { if (eqd_trace && threadIdx.x == 0) atomicAdd_system(eqd_trace + 8200 + (k), 1); } while (0)
-#else
-#define EQD_TRACE_SETTER(name)
-#define TRACE_PHASE(k, slot, tile, phase) do { } while (0)
-#define TRACE_START(k) do { } while (0)
-#define TRACE_END(k) do { } while (0)
-#endif
-
-
 // LeakyReLU for 0 <= slope <= 1 (checked by the launchers): max(v, slope*v) is bit-identical to the select form
 // and one instruction shorter (FMUL + FMNMX)
 __device__ __forceinline__ float lrelu(float v, float slope) { return fmaxf(v, v * slope); }

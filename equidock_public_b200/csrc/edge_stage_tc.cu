@@ -75,7 +75,6 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
   const int ntiles = (g.n_nodes + tn - 1) / tn;
   const float slope = p.leaky_slope;
 
-  TRACE_START(0);
   // ---- one-time setup: barriers, weights (one TMA bulk copy), per-layer vectors ------------------------------------
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
@@ -179,7 +178,6 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
       e0 = e0n; ne = nen; off_l = off_ln; n_l = n_ln; off_r = off_rn; buf ^= 1;
       continue;
     }
-    if (t == 0) TRACE_PHASE(0, blockIdx.x * TC_WGS + wgi, tile, 2);
     // The coordinate update's x_orig / x_in loads go out now and are consumed at the end of the tile.
     const int o_upd = 127 - t;                 // nn * 3 <= 96 outputs on the last threads
     const int nd_upd = o_upd / 3, comp_upd = o_upd - nd_upd * 3;
@@ -433,15 +431,11 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     }
     e0 = e0n; ne = nen; off_l = off_ln; n_l = n_ln; off_r = off_rn; buf ^= 1;
   }
-  if (t == 0) TRACE_PHASE(0, blockIdx.x * TC_WGS + wgi, 0xffff, 16);
   cp_async_wait<0>();
   __syncthreads();
-  TRACE_END(0);
 }
 
 }  // namespace eqd
-
-EQD_TRACE_SETTER(eqd_trace_set_edge)
 
 extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const float* proj, const double* x_in,
                               const double* x_orig, float* aggr, double* x_out, int32_t* status, void* stream) {

@@ -9,7 +9,6 @@ __global__ void embed_kernel(eqd_graph g, const float* __restrict__ emb, const f
                              const float* __restrict__ mu_r, const float* __restrict__ x_l,
                              const float* __restrict__ x_r, float* __restrict__ h0, double* __restrict__ x64,
                              int32_t* __restrict__ status) {
-  TRACE_START(4);
   const int per_node = EQD_H0_PAD / 4;  // 18 float4 per node
   long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
   long total = (long)g.n_nodes * per_node;
@@ -67,8 +66,6 @@ __global__ void __launch_bounds__(EQD_THREADS) project_kernel(eqd_graph g, eqd_l
 }
 
 }  // namespace eqd
-
-EQD_TRACE_SETTER(eqd_trace_set_embed)
 
 extern "C" int eqd_embed_checked(const eqd_graph* g, const float* emb, const float* res_feat_lig,
                                  const float* res_feat_rec, const float* mu_lig, const float* mu_rec, const float* x_lig,

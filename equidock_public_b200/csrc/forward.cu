@@ -3,8 +3,6 @@
 // per-stage entry points of this library on one stream, so a binding pays one foreign call (and ~40 kernel launches)
 // per batch instead of ~45 calls plus as many device allocations.
 #include <cstdint>
-#include <cstdlib>
-#include <cstring>
 
 #include "common.cuh"
 
@@ -97,8 +95,6 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return EQD_ERR_BAD_ARG;
   if (g->n_pairs <= 0 || g->n_nodes <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  // debugging knobs (bit mask): 1 skip the head, 2 skip the memsets, 4 synchronise after every stage, 8 stop after layer 0
-  static const int dbg = getenv("EQD_FORWARD_DEBUG") ? atoi(getenv("EQD_FORWARD_DEBUG")) : 0;
   unsigned char* w = reinterpret_cast<unsigned char*>(workspace);
   float* h0 = reinterpret_cast<float*>(w + c.h0);
   double* x0 = reinterpret_cast<double*>(w + c.x0);
@@ -127,14 +123,12 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
 
   // rows the kernels never write but the tensor cores / TMA read: the tail of the last 8-node block and the 8 pad
   // blocks of each (K|V, split) plane, and the pad rows of x5 (they reach P.V as 0 x value: must be finite)
-  if (!(dbg & 2)) {
-    const size_t plane = c.kv_bytes / 6, from = (size_t)(N / 8) * 1024;
-    cudaError_t me = cudaSuccess;
-    for (int pl = 0; pl < 6 && me == cudaSuccess; ++pl) me = cudaMemsetAsync(kv + pl * plane + from, 0, plane - from, st);
-    if (me == cudaSuccess) me = cudaMemsetAsync(x5 + (size_t)N * 16, 0, (c.x5_rows - (size_t)N) * 16 * 4, st);
-    if (me == cudaSuccess) me = cudaMemsetAsync(io->status, 0, (size_t)(B + 1) * sizeof(int32_t), st);
-    if (me != cudaSuccess) return -(1000 + (int)me);
-  }
+  const size_t plane = c.kv_bytes / 6, from = (size_t)(N / 8) * 1024;
+  cudaError_t me = cudaSuccess;
+  for (int pl = 0; pl < 6 && me == cudaSuccess; ++pl) me = cudaMemsetAsync(kv + pl * plane + from, 0, plane - from, st);
+  if (me == cudaSuccess) me = cudaMemsetAsync(x5 + (size_t)N * 16, 0, (c.x5_rows - (size_t)N) * 16 * 4, st);
+  if (me == cudaSuccess) me = cudaMemsetAsync(io->status, 0, (size_t)(B + 1) * sizeof(int32_t), st);
+  if (me != cudaSuccess) return -(1000 + (int)me);
   auto stage_event = [&](int li, int which) {   // which: 0 edge begin, 1 edge end, 2 node begin, 3 node end
     if (io->stage_events && io->stage_events[li * 4 + which]) cudaEventRecord((cudaEvent_t)io->stage_events[li * 4 + which], st);
   };
@@ -143,7 +137,7 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
   if (rc) return rc;
   const eqd_layer* l0_l = layers[0];
   const eqd_layer_params* l0 = &l0_l->dev;
-  const bool tc0 = l0->dh == EQD_H0 && l0->w_proj_tc && l0->w_node_tc && !io->layer0_fp32;
+  const bool tc0 = l0->dh == EQD_H0 && l0->w_proj_tc && l0->w_node_tc;
   if (tc0) rc = eqd_project_tc0(g, l0_l, h0, pa, kv, x5, stream);
   else rc = eqd_project(g, l0_l, h0, l0->dh == EQD_H0 ? EQD_H0_PAD : EQD_HID, pa, stream);
   if (rc) return rc;
@@ -176,19 +170,16 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
     } else if (li == 0 && tc0 && (!lpn || lpn->w_proj_tc)) {
       rc = eqd_node_stage_tc0(g, lp_l, lpn_l, h0, pa, aggr, kv, x5, mu, h_out, pb, stream);
     } else {   // fp32 CUDA-core node stage (fused projections); the next layer's tensor-core attention needs K/V blocks
-      rc = eqd_node_stage(g, lp_l, lpn_l, h_in, ldh, h0, pa, aggr, h_out, pb, stream);
+      rc = eqd_node_stage(g, lp_l, lpn_l, h_in, ldh, h0, pa, aggr, sb ? mu : nullptr, h_out, pb, stream);
       if (!rc && lpn && lpn->dh == EQD_HID && lpn->w_node_tc) rc = eqd_kv_blocks(g, pb, 320, 192, 256, kv, stream);
     }
     if (rc) return rc;
     stage_event(li, 3);
-    if (dbg & 4) cudaStreamSynchronize(st);
-    if ((dbg & 8) && li == 0) return EQD_OK;
     float* t = pa; pa = pb; pb = t;
     h_in = h_out;
     ldh = EQD_HID;
     x_in = x_out;
   }
-  if (dbg & 1) return EQD_OK;
   rc = eqd_keypoints(g, hp, h_in, x_in, w + c.head, c.head_bytes, keypts, ymean, cov, stream);
   if (rc) return rc;
   return eqd_kabsch_apply(g, cov, ymean, io->x_lig, nullptr, io->rot, io->trans, io->ligand_out, io->sing, io->status, stream);

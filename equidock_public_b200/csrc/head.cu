@@ -22,7 +22,6 @@ namespace eqd {
 // ---- partial column sums of LeakyReLU(W_m h + b_m) over each node tile (:525, :529) -------------
 __global__ void __launch_bounds__(EQD_THREADS, 2)
 head_mean_kernel(eqd_graph g, eqd_head_params hp, const float* __restrict__ h, float* __restrict__ part) {
-  TRACE_START(5);
   extern __shared__ __align__(16) float smem[];
   constexpr int LD = 68;
   float* A = smem;                   // [128][68]
@@ -145,7 +144,6 @@ struct KeypSmem {
 __global__ void __launch_bounds__(KP_THREADS, 4)
 keypoints_kernel(eqd_graph g, const float* __restrict__ h, const double* __restrict__ x,
                  const double* __restrict__ u_all /* [2B][50][64] */, double* __restrict__ keypts) {
-  TRACE_START(6);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   KeypSmem& s = *reinterpret_cast<KeypSmem*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -285,7 +283,6 @@ __global__ void kabsch_apply_kernel(eqd_graph g, const double* __restrict__ cov,
                                     const float* __restrict__ x_lig_in, const int* __restrict__ pair_mask,
                                     float* __restrict__ rot, float* __restrict__ trans, float* __restrict__ ligand_out,
                                     double* __restrict__ sing, int* __restrict__ status) {
-  TRACE_START(7);
   const int b = blockIdx.x;
   if (pair_mask && pair_mask[b] == 0) return;
   __shared__ double Tb[12];
@@ -360,8 +357,6 @@ __global__ void tile_ptr_kernel(eqd_graph g, int* __restrict__ tile_ptr) {
 }
 
 }  // namespace eqd
-
-EQD_TRACE_SETTER(eqd_trace_set_head)
 
 static inline size_t eqd_align256(size_t v) { return (v + 255) & ~(size_t)255; }
 

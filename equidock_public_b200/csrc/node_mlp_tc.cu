@@ -45,7 +45,6 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
   float (&ring)[NM_SLOTS][64 * 64] = S.stage[wgi];
   const int bar = 1 + wgi;   // this chain's named barrier
   const int ntiles = (n_nodes + 63) / 64, tstride = gridDim.x * NM_CHAINS, tile0 = blockIdx.x * NM_CHAINS + wgi;
-  TRACE_START(3);
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -75,7 +74,6 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
   mbar_wait(&S.w_bar, 0);
 
   for (int tile = tile0; tile < ntiles; tile += tstride) {
-    if (t == 0) TRACE_PHASE(3, blockIdx.x * NM_CHAINS + wgi, tile, 1);
     const int node0 = tile * 64, nvalid = min(64, n_nodes - node0);
     // piece 4 (h0[64:72]): A registers 0, 1 of the k-block = channels 64 + fc + {0, 1} of rows fr0, fr0 + 8
     float2 x4[2];
@@ -207,7 +205,6 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
     }
   }
   cp_async_wait<0>();
-  TRACE_END(3);
 }
 
 
@@ -238,7 +235,6 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
   Nm0Smem& S = *reinterpret_cast<Nm0Smem*>(smem_raw);
   const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, wgi = tid >> 7;
   const int ntiles = (n_nodes + EQD_TM - 1) / EQD_TM;
-  TRACE_START(3);
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -254,7 +250,6 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
   float* red = S.red;
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    if (q == 0) TRACE_PHASE(3, blockIdx.x, tile, 1);
     const int node = tile * EQD_TM + r;
     const bool valid = node < n_nodes;
     auto row32 = [&](const float* base, int ld, float (&v)[32]) {   // my half row of a [n][ld] array
@@ -387,12 +382,9 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
     }
     __syncthreads();   // the result tile has been read: the region takes the next tile's A operand
   }
-  TRACE_END(3);
 }
 
 }  // namespace eqd
-
-EQD_TRACE_SETTER(eqd_trace_set_mlp)
 
 extern "C" int eqd_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const float* h_in, const float* aggr,
                                const float* mu, const float* h0, float* h_out, void* stream) {

@@ -5,7 +5,7 @@
 //      softmax -- the per-pair block of the reference's dense masked softmax (:61-63), no 1/sqrt(d);
 //   2. node MLP on [h | aggr_msg | mu | h0] (Linear, LeakyReLU, LayerNorm, Linear) + skip (:332-337);
 //   3. writes h' and, when a next layer exists, that layer's projections of h' (Psrc, Pdst, Q, K, V)
-//      so h' is never re-read from HBM for them; with mu_out != NULL also mu (the per-layer backward reads it).
+//      so h' is never re-read from HBM for them; with mu != NULL also mu (the per-layer backward reads it).
 #include "common.cuh"
 
 namespace eqd {
@@ -189,13 +189,13 @@ node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_
 }
 }  // namespace eqd
 
-static int node_stage_launch(const eqd_graph* g, const eqd_layer* p_l, const eqd_layer* p_next_l, const float* h_in,
-                             int32_t ldh, const float* h0, const float* proj, const float* aggr, float* h_out,
-                             float* proj_next, float* mu_out, void* stream) {
+extern "C" int eqd_node_stage(const eqd_graph* g, const eqd_layer* p_l, const eqd_layer* p_next_l, const float* h_in,
+                              int32_t ldh, const float* h0, const float* proj, const float* aggr, float* mu,
+                              float* h_out, float* proj_next, void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   const eqd_layer_params* p_next = p_next_l ? &p_next_l->dev : nullptr;
   if (!g || !p || !h_in || !h0 || !proj || !aggr || !h_out) return EQD_ERR_BAD_ARG;
-  if (reinterpret_cast<uintptr_t>(mu_out) & 15) return EQD_ERR_BAD_ARG;   // rows are written 16 bytes at a time
+  if (reinterpret_cast<uintptr_t>(mu) & 15) return EQD_ERR_BAD_ARG;   // rows are written 16 bytes at a time
   if (p_next && (!proj_next || p_next->dh != 64 || p_next->dhp != 64)) return EQD_ERR_BAD_ARG;
   const bool extra = (p->dh == 69 && p->dhp == 72);
   if (!extra && !(p->dh == 64 && p->dhp == 64)) return EQD_ERR_UNSUPPORTED;
@@ -209,39 +209,23 @@ static int node_stage_launch(const eqd_graph* g, const eqd_layer* p_l, const eqd
     EQD_SET_SMEM((eqd::node_stage_kernel<true>), smem);
     int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
     eqd::node_stage_kernel<true><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr,
-                                                                  h_out, proj_next, mu_out);
+                                                                  h_out, proj_next, mu);
   } else {
     size_t smem = eqd::NodeCfg<false>::SMEM;
     EQD_SET_SMEM((eqd::node_stage_kernel<false>), smem);
     int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
     eqd::node_stage_kernel<false><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr,
-                                                                   h_out, proj_next, mu_out);
+                                                                   h_out, proj_next, mu);
   }
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }
 
-extern "C" int eqd_node_stage(const eqd_graph* g, const eqd_layer* p_l, const eqd_layer* p_next_l,
-                              const float* h_in, int32_t ldh, const float* h0, const float* proj, const float* aggr,
-                              float* h_out, float* proj_next, void* stream) {
-  return node_stage_launch(g, p_l, p_next_l, h_in, ldh, h0, proj, aggr, h_out, proj_next, nullptr, stream);
-}
-
 extern "C" int eqd_iegmn_layer_forward(const eqd_graph* g, const eqd_layer* p_l, const eqd_layer* p_next_l,
                                        const float* h_in, int32_t ldh, const float* h0, const double* x_in,
-                                       const double* x_orig, float* proj, float* proj_next, float* aggr, float* h_out,
-                                       double* x_out, int32_t* status, void* stream) {
+                                       const double* x_orig, float* proj, float* proj_next, float* aggr, float* mu,
+                                       float* h_out, double* x_out, int32_t* status, void* stream) {
   int rc = eqd_edge_stage(g, p_l, proj, x_in, x_orig, aggr, x_out, status, stream);
   if (rc) return rc;
-  return eqd_node_stage(g, p_l, p_next_l, h_in, ldh, h0, proj, aggr, h_out, proj_next, stream);
-}
-
-extern "C" int eqd_iegmn_layer_forward_stash(const eqd_graph* g, const eqd_layer* p_l, const eqd_layer* p_next_l,
-                                             const float* h_in, int32_t ldh, const float* h0, const double* x_in,
-                                             const double* x_orig, float* proj, float* proj_next, float* aggr,
-                                             float* mu, float* h_out, double* x_out, int32_t* status, void* stream) {
-  if (!mu) return EQD_ERR_BAD_ARG;
-  int rc = eqd_edge_stage(g, p_l, proj, x_in, x_orig, aggr, x_out, status, stream);
-  if (rc) return rc;
-  return node_stage_launch(g, p_l, p_next_l, h_in, ldh, h0, proj, aggr, h_out, proj_next, mu, stream);
+  return eqd_node_stage(g, p_l, p_next_l, h_in, ldh, h0, proj, aggr, mu, h_out, proj_next, stream);
 }

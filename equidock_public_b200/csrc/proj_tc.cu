@@ -64,7 +64,6 @@ project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjCon
   PjSmem<L0>& S = *reinterpret_cast<PjSmem<L0>*>(smem_raw);
   const int tid = threadIdx.x, half = tid / R, r = tid % R, warp = tid >> 5, wgi = tid >> 7;
   const int ntiles = (n_nodes + R - 1) / R;
-  TRACE_START(2);
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -80,7 +79,6 @@ project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjCon
   const int lane = tid & 31, wrow0 = (warp * 32) % R;   // the warp's 32 rows (of its column half)
 
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    if (tid == 0) TRACE_PHASE(2, blockIdx.x, tile, 1);
     const int node0 = tile * R;
     const int node = node0 + r;
     const bool valid = node < n_nodes;
@@ -168,7 +166,6 @@ project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjCon
     }
     __syncthreads();     // A may be overwritten by the next tile
   }
-  TRACE_END(2);
 }
 
 // ---- the 64-wide layers ---------------------------------------------------------------------------------------------
@@ -203,7 +200,6 @@ project64_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjC
   PjChainSmem& W = S.ch[wgi];
   const int bar = 1 + wgi;   // this chain's named barrier
   const int ntiles = (n_nodes + 63) / 64, tstride = gridDim.x * PJ_CHAINS;
-  TRACE_START(2);
   if (tid == 0) {
     mbar_init(&S.w_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -222,7 +218,6 @@ project64_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjC
   mbar_wait(&S.w_bar, 0);
 
   for (; tile < ntiles; tile += tstride) {
-    if (t == 0) TRACE_PHASE(2, blockIdx.x * PJ_CHAINS + wgi, tile, 1);
     const int node0 = tile * 64, nvalid = min(64, n_nodes - node0);
     cp_async_wait<0>();
     wg_barrier(bar);   // this tile's h rows have landed
@@ -299,7 +294,6 @@ project64_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjC
     }
   }
   cp_async_wait<0>();
-  TRACE_END(2);
 }
 
 // fp32 K / V columns of a projection buffer -> bf16x3 8-node blocks (used after the FFMA layer-0 node stage)
@@ -319,8 +313,6 @@ __global__ void kv_blocks_kernel(int n_nodes, const float* __restrict__ proj, in
 }
 
 }  // namespace eqd
-
-EQD_TRACE_SETTER(eqd_trace_set_proj)
 
 extern "C" size_t eqd_kv_blocks_bytes(int32_t n_nodes) {
   // [which 2][split 3][ceil(n/8) + 8 pad groups][1024 B]; the pad groups must be zero (they feed P.V as 0 x V)

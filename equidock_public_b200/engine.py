@@ -61,10 +61,8 @@ def umma_bf16x3(w: torch.Tensor) -> torch.Tensor:
     return torch.cat(out)
 
 
-# EQD_LAYER0_FFMA=1 keeps the 69-wide layer 0 on the fp32 CUDA-core kernels (A/B comparisons)
-_LAYER0_FFMA = bool(int(__import__('os').environ.get('EQD_LAYER0_FFMA', '0')))
-# EQD_PY_FORWARD=1: drive the stages one C call at a time from Python instead of through eqd_iegmn_forward
-_PY_FORWARD = bool(int(__import__('os').environ.get('EQD_PY_FORWARD', '0')))
+# read by bench.py; the forward is always the one C call of IEGMNEngine.forward
+_PY_FORWARD = False
 
 
 class PackedLayer:
@@ -377,7 +375,7 @@ class _StatusLease:
 
 class NativeStageTimer:
     """CUDA events recorded by eqd_iegmn_forward around every edge / node stage (io.stage_events), on the launching
-    stream; in the Python driver the same handles are recorded through begin() / end()."""
+    stream."""
 
     def __init__(self):
         self.lib, self.sets, self.spare = nat.load(), [], []
@@ -440,166 +438,57 @@ class IEGMNEngine:
                 res_l, res_r, mu_l, mu_r, x_l, x_r, check_status: bool = True, log=None,
                 stage_timer=None, record_event: bool = True, train_stash=None) -> Dict[str, torch.Tensor]:
         """One forward = ONE call into the library (eqd_iegmn_forward): the per-stage entry points are chained in C on
-        the current stream out of a single workspace allocation.  EQD_PY_FORWARD=1 selects the stage-by-stage Python
-        driver below instead (same kernels; used to A/B the two and by the per-stage tests)."""
+        the current stream out of a single workspace allocation."""
         with torch.cuda.device(self.device):   # the raw launches below go to the CURRENT device: make it the model's
-            if _PY_FORWARD:
-                return self._forward_py(plan, emb, layers, head, res_l, res_r, mu_l, mu_r, x_l, x_r, check_status, log,
-                                        stage_timer)
-            return self._forward_native(plan, emb, layers, head, res_l, res_r, mu_l, mu_r, x_l, x_r, check_status, log,
-                                        stage_timer, record_event, train_stash)
-
-    def _forward_native(self, plan, emb, layers, head, res_l, res_r, mu_l, mu_r, x_l, x_r, check_status, log,
-                        stage_timer, record_event=True, train_stash=None):
-        lib, dev = self.lib, self.device
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        N, B = plan.N, plan.n_pairs
-        f32 = dict(dtype=torch.float32, device=dev)
-        f64 = dict(dtype=torch.float64, device=dev)
-        cf = lambda t: t.to(**f32).contiguous()
-        res_l, res_r, mu_l, mu_r, x_l, x_r = map(cf, (res_l, res_r, mu_l, mu_r, x_l, x_r))
-        assert x_l.shape == (plan.N_l, 3) and x_r.shape == (plan.N_r, 3)
-        g = C.byref(plan.struct)
-        if plan.forward_ws_bytes is None:
-            plan.forward_ws_bytes = int(lib.eqd_forward_workspace_bytes(g))
-        ws = torch.empty(plan.forward_ws_bytes, dtype=torch.uint8, device=dev)
-        # outputs (separate allocations: the kernels assume 16-byte aligned rows)
-        rot, trans = torch.empty(B, 3, 3, **f32), torch.empty(B, 1, 3, **f32)
-        lig_out, h_fin = torch.empty(plan.N_l, 3, **f32), torch.empty(N, nat.HID, **f32)
-        sing, x_fin = torch.empty(B, 3, **f64), torch.empty(N, 3, **f64)
-        keyp, cov, ymean = torch.empty(2 * B, nat.HEADS, 3, **f64), torch.empty(B, 9, **f64), torch.empty(2 * B, 3, **f64)
-        status = torch.empty(B + 1, dtype=torch.int32, device=dev)
-        io = nat.EqdForwardIO()
-        for name, t in (('emb', emb), ('res_lig', res_l), ('res_rec', res_r), ('mu_lig', mu_l), ('mu_rec', mu_r),
-                        ('x_lig', x_l), ('x_rec', x_r), ('rot', rot), ('trans', trans), ('ligand_out', lig_out),
-                        ('sing', sing), ('status', status), ('h_out', h_fin), ('x_out', x_fin), ('keypts', keyp),
-                        ('cov', cov), ('ymean', ymean)):
-            setattr(io, name, t.data_ptr())
-        io.layer0_fp32 = 1 if _LAYER0_FFMA else 0
-        if train_stash is not None:   # training: keep every layer's inputs for the backward kernels
-            io.train_stash, io.train_stash_bytes = train_stash.data_ptr(), int(train_stash.numel())
-        events = stage_timer.new_forward(len(layers)) if stage_timer is not None else None
-        io.stage_events = C.cast(events, C.c_void_p) if events is not None else None
-        larr = (C.POINTER(nat.EqdLayer) * len(layers))(*[C.pointer(l.struct) for l in layers])
-        nat.check(lib.eqd_iegmn_forward(g, larr, len(layers), C.byref(head.struct), C.byref(io), nat.ptr(ws),
-                                        plan.forward_ws_bytes, st), 'eqd_iegmn_forward')
-        kab = lambda mask: nat.check(lib.eqd_kabsch_apply(
-            g, nat.ptr(cov), nat.ptr(ymean), nat.ptr(x_l), nat.ptr(mask), nat.ptr(rot), nat.ptr(trans),
-            nat.ptr(lig_out), nat.ptr(sing), nat.ptr(status), st), 'eqd_kabsch_apply')
-        lease = _StatusLease(B + 2)
-        status_host = lease.view()
-        status_host[:B + 1].copy_(status, non_blocking=True)
-        status_host[B + 1:].copy_(plan.unsorted_i32, non_blocking=True)
-        status_event = None
-        if record_event:     # (a CUDA-graph capture records its own event after every replay instead)
-            status_event = torch.cuda.Event()
-            status_event.record()
-        out = {'status_lease': lease, 'ligand_coors': lig_out, 'keypts': keyp, 'rotation': rot, 'translation': trans,
-               'h': h_fin, 'x64': x_fin, 'cov': cov, 'sing': sing, 'status': status, 'unsorted': plan.unsorted,
-               'kabsch': kab, 'status_host': status_host, 'status_event': status_event, '_keep': (ws, ymean, x_l)}
-        if check_status:
-            self.resolve_status(plan, out, kab, log)
-        return out
-
-    def _forward_py(self, plan: GraphPlan, emb: torch.Tensor, layers: List[PackedLayer], head: PackedHead,
-                    res_l, res_r, mu_l, mu_r, x_l, x_r, check_status: bool = True, log=None,
-                    stage_timer=None) -> Dict[str, torch.Tensor]:
-        lib, dev = self.lib, self.device
-        g = C.byref(plan.struct)
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        N, B = plan.N, plan.n_pairs
-        f32 = dict(dtype=torch.float32, device=dev)
-        f64 = dict(dtype=torch.float64, device=dev)
-        cf = lambda t: t.to(**f32).contiguous()
-        res_l, res_r, mu_l, mu_r, x_l, x_r = map(cf, (res_l, res_r, mu_l, mu_r, x_l, x_r))
-        assert x_l.shape == (plan.N_l, 3) and x_r.shape == (plan.N_r, 3)
-        h0 = torch.empty(N, nat.H0_PAD, **f32)
-        x0 = torch.empty(N, 3, **f64)
-        xa, xb = torch.empty(N, 3, **f64), torch.empty(N, 3, **f64)
-        ha, hb = torch.empty(N, nat.HID, **f32), torch.empty(N, nat.HID, **f32)
-        pa, pb = torch.empty(N, 128 + 3 * nat.H0_PAD, **f32), torch.empty(N, 128 + 3 * nat.H0_PAD, **f32)
-        aggr = torch.empty(N, nat.HID, **f32)
-        status = torch.zeros(B + 1, dtype=torch.int32, device=dev)
-        mu = torch.empty(N, nat.HID, **f32)
-        kv_bytes = lib.eqd_kv_blocks_bytes(N)
-        kv = torch.empty(kv_bytes, dtype=torch.uint8, device=dev)
-        # rows never written (tail of the last 8-node block + the 8 pad blocks of each (K|V, split) plane) reach
-        # the P.V MMA as 0 x V: they must be finite
-        kv.view(6, -1)[:, (N // 8) * 1024:].zero_()
-        nat.check(lib.eqd_embed(g, nat.ptr(emb), nat.ptr(res_l), nat.ptr(res_r), nat.ptr(mu_l), nat.ptr(mu_r),
-                                nat.ptr(x_l), nat.ptr(x_r), nat.ptr(h0), nat.ptr(x0), st), 'eqd_embed')
-        tc0 = layers[0].dh == nat.H0 and not _LAYER0_FFMA   # 69-wide layer 0 on the tensor cores too
-        if tc0:
-            x5 = torch.empty(((N + 7) // 8 + 8) * 8, 16, **f32)   # channels 64..68 of K, V, Q; pad rows must be finite
-            x5[N:].zero_()
-            mu0 = torch.empty(N, nat.H0_PAD, **f32)
-            nat.check(lib.eqd_project_tc0(g, C.byref(layers[0].struct), nat.ptr(h0), nat.ptr(pa), nat.ptr(kv), nat.ptr(x5),
-                                          st), 'eqd_project_tc0')
-        else:
-            nat.check(lib.eqd_project(g, C.byref(layers[0].struct), nat.ptr(h0), nat.H0_PAD, nat.ptr(pa), st),
-                      'eqd_project')
-        h_in, ldh, x_in = h0, nat.H0_PAD, x0
-        h_out, x_out = ha, xa
-        for li, lay in enumerate(layers):
-            nxt = layers[li + 1] if li + 1 < len(layers) else None
-            lp = C.byref(lay.struct)
-            lpn = C.byref(nxt.struct) if nxt is not None else None
-            tmr = stage_timer
-            if tmr is not None:
-                tmr.begin('edge_stage', li)
-            nat.check(lib.eqd_edge_stage(g, lp, nat.ptr(pa), nat.ptr(x_in), nat.ptr(x0), nat.ptr(aggr),
-                                         nat.ptr(x_out), nat.ptr(status), st), f'eqd_edge_stage[{li}]')
-            if tmr is not None:
-                tmr.end('edge_stage', li)
-                tmr.begin('node_stage', li)
-            if lay.dh == nat.HID:   # tensor-core node stage: attention, node MLP, next layer's projections + K/V blocks
-                nat.check(lib.eqd_node_stage_tc(g, lp, lpn, nat.ptr(h_in), nat.ptr(h0), nat.ptr(pa), nat.ptr(aggr),
-                                                nat.ptr(kv), nat.ptr(mu), nat.ptr(h_out), nat.ptr(pb), st),
-                          f'eqd_node_stage_tc[{li}]')
-            elif tc0 and li == 0:   # 69-wide layer 0: 64 tensor-core channels + 5 fp32 ones
-                nat.check(lib.eqd_node_stage_tc0(g, lp, lpn, nat.ptr(h0), nat.ptr(pa), nat.ptr(aggr), nat.ptr(kv),
-                                                 nat.ptr(x5), nat.ptr(mu0), nat.ptr(h_out), nat.ptr(pb), st),
-                          'eqd_node_stage_tc0')
-            else:                   # fp32 CUDA-core node stage (fused projections), then K/V blocks
-                nat.check(lib.eqd_node_stage(g, lp, lpn, nat.ptr(h_in), ldh, nat.ptr(h0), nat.ptr(pa), nat.ptr(aggr),
-                                             nat.ptr(h_out), nat.ptr(pb), st), f'eqd_node_stage[{li}]')
-                if nxt is not None:
-                    nat.check(lib.eqd_kv_blocks(g, nat.ptr(pb), 320, 192, 256, nat.ptr(kv), st), 'eqd_kv_blocks')
-            if tmr is not None:
-                tmr.end('node_stage', li)
-            pa, pb = pb, pa
-            h_in, ldh, x_in = h_out, nat.HID, x_out
-            h_out = hb if h_out is ha else ha
-            x_out = xb if x_out is xa else xa
-        h_fin, x_fin = h_in, x_in
-        ws_bytes = lib.eqd_workspace_bytes(N, plan.n_node_tiles, B)
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-        keyp = torch.empty(2 * B, nat.HEADS, 3, **f64)
-        ymean = torch.empty(2 * B, 3, **f64)
-        cov = torch.empty(B, 9, **f64)
-        nat.check(lib.eqd_keypoints(g, C.byref(head.struct), nat.ptr(h_fin), nat.ptr(x_fin), nat.ptr(ws), ws_bytes,
-                                    nat.ptr(keyp), nat.ptr(ymean), nat.ptr(cov), st), 'eqd_keypoints')
-        rot, trans = torch.empty(B, 3, 3, **f32), torch.empty(B, 1, 3, **f32)
-        lig_out = torch.empty(plan.N_l, 3, **f32)
-        sing = torch.empty(B, 3, **f64)
-        kab = lambda mask: nat.check(lib.eqd_kabsch_apply(
-            g, nat.ptr(cov), nat.ptr(ymean), nat.ptr(x_l), nat.ptr(mask), nat.ptr(rot), nat.ptr(trans),
-            nat.ptr(lig_out), nat.ptr(sing), nat.ptr(status), st), 'eqd_kabsch_apply')
-        kab(None)
-        # status words -> pinned host memory, asynchronously; resolve_status() waits on the event only, so a caller
-        # may launch the next forward before looking at this one's flags (bench.py keeps two steps in flight)
-        lease = _StatusLease(B + 2)
-        status_host = lease.view()
-        status_host[:B + 1].copy_(status, non_blocking=True)
-        status_host[B + 1:].copy_(plan.unsorted_i32, non_blocking=True)
-        status_event = torch.cuda.Event()
-        status_event.record()
-        out = {'status_lease': lease,'ligand_coors': lig_out, 'keypts': keyp, 'rotation': rot, 'translation': trans, 'h': h_fin,
-               'x64': x_fin, 'cov': cov, 'sing': sing, 'status': status, 'unsorted': plan.unsorted, 'kabsch': kab,
-               'status_host': status_host, 'status_event': status_event}
-        if check_status:
-            self.resolve_status(plan, out, kab, log)
-        return out
+            lib, dev = self.lib, self.device
+            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            N, B = plan.N, plan.n_pairs
+            f32 = dict(dtype=torch.float32, device=dev)
+            f64 = dict(dtype=torch.float64, device=dev)
+            cf = lambda t: t.to(**f32).contiguous()
+            res_l, res_r, mu_l, mu_r, x_l, x_r = map(cf, (res_l, res_r, mu_l, mu_r, x_l, x_r))
+            assert x_l.shape == (plan.N_l, 3) and x_r.shape == (plan.N_r, 3)
+            g = C.byref(plan.struct)
+            if plan.forward_ws_bytes is None:
+                plan.forward_ws_bytes = int(lib.eqd_forward_workspace_bytes(g))
+            ws = torch.empty(plan.forward_ws_bytes, dtype=torch.uint8, device=dev)
+            # outputs (separate allocations: the kernels assume 16-byte aligned rows)
+            rot, trans = torch.empty(B, 3, 3, **f32), torch.empty(B, 1, 3, **f32)
+            lig_out, h_fin = torch.empty(plan.N_l, 3, **f32), torch.empty(N, nat.HID, **f32)
+            sing, x_fin = torch.empty(B, 3, **f64), torch.empty(N, 3, **f64)
+            keyp = torch.empty(2 * B, nat.HEADS, 3, **f64)
+            cov, ymean = torch.empty(B, 9, **f64), torch.empty(2 * B, 3, **f64)
+            status = torch.empty(B + 1, dtype=torch.int32, device=dev)
+            io = nat.EqdForwardIO()
+            for name, t in (('emb', emb), ('res_lig', res_l), ('res_rec', res_r), ('mu_lig', mu_l), ('mu_rec', mu_r),
+                            ('x_lig', x_l), ('x_rec', x_r), ('rot', rot), ('trans', trans), ('ligand_out', lig_out),
+                            ('sing', sing), ('status', status), ('h_out', h_fin), ('x_out', x_fin), ('keypts', keyp),
+                            ('cov', cov), ('ymean', ymean)):
+                setattr(io, name, t.data_ptr())
+            if train_stash is not None:   # training: keep every layer's inputs for the backward kernels
+                io.train_stash, io.train_stash_bytes = train_stash.data_ptr(), int(train_stash.numel())
+            events = stage_timer.new_forward(len(layers)) if stage_timer is not None else None
+            io.stage_events = C.cast(events, C.c_void_p) if events is not None else None
+            larr = (C.POINTER(nat.EqdLayer) * len(layers))(*[C.pointer(l.struct) for l in layers])
+            nat.check(lib.eqd_iegmn_forward(g, larr, len(layers), C.byref(head.struct), C.byref(io), nat.ptr(ws),
+                                            plan.forward_ws_bytes, st), 'eqd_iegmn_forward')
+            kab = lambda mask: nat.check(lib.eqd_kabsch_apply(
+                g, nat.ptr(cov), nat.ptr(ymean), nat.ptr(x_l), nat.ptr(mask), nat.ptr(rot), nat.ptr(trans),
+                nat.ptr(lig_out), nat.ptr(sing), nat.ptr(status), st), 'eqd_kabsch_apply')
+            lease = _StatusLease(B + 2)
+            status_host = lease.view()
+            status_host[:B + 1].copy_(status, non_blocking=True)
+            status_host[B + 1:].copy_(plan.unsorted_i32, non_blocking=True)
+            status_event = None
+            if record_event:     # (a CUDA-graph capture records its own event after every replay instead)
+                status_event = torch.cuda.Event()
+                status_event.record()
+            out = {'status_lease': lease, 'ligand_coors': lig_out, 'keypts': keyp, 'rotation': rot,
+                   'translation': trans, 'h': h_fin, 'x64': x_fin, 'cov': cov, 'sing': sing, 'status': status,
+                   'unsorted': plan.unsorted, 'kabsch': kab, 'status_host': status_host, 'status_event': status_event, '_keep': (ws, ymean, x_l)}
+            if check_status:
+                self.resolve_status(plan, out, kab, log)
+            return out
 
     def resolve_status(self, plan: GraphPlan, out, kab, log=None):
         """The ONE host sync of a forward: reads the status words and replays the reference's

@@ -289,8 +289,9 @@ class IEGMN_Layer(nn.Module):
         g, lp = C.byref(plan.struct), C.byref(lay.struct)
         nat.check(eng.lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
         nat.check(eng.lib.eqd_iegmn_layer_forward(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
-                                                  nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(h_out),
-                                                  nat.ptr(x_out), nat.ptr(status), st), 'eqd_iegmn_layer_forward')
+                                                  nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), None,
+                                                  nat.ptr(h_out), nat.ptr(x_out), nat.ptr(status), st),
+                  'eqd_iegmn_layer_forward')
         if int(status[plan.n_pairs].item()) & nat.STATUS_DEGREE_OVERFLOW or bool(plan.unsorted.item()):
             raise nat.NativeLibraryError('IEGMN_Layer.forward: edges must be grouped by destination with in-degree '
                                          f'<= {self.graph_max_neighbor}')

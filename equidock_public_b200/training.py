@@ -556,7 +556,7 @@ def layer_train_pack(layer_module, packed: PackedLayer, device):
 
 
 class _LayerFn(torch.autograd.Function):
-    """autograd node of one IEGMN_Layer call: forward = eqd_project + eqd_iegmn_layer_forward_stash, backward =
+    """autograd node of one IEGMN_Layer call: forward = eqd_project + eqd_iegmn_layer_forward (with mu), backward =
     layer_backward.  Inputs: the ten floating-point tensors of IEGMN_Layer.forward (ligand coordinates, features, original
     features, edge features, original coordinates, then the receptor's five) and the layer's parameters.  Outputs: the
     layer's coordinates (N,3) f64 and features (N,64) f32 of both proteins in global node order."""
@@ -584,10 +584,10 @@ class _LayerFn(torch.autograd.Function):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             g, lp = C.byref(plan.struct), C.byref(lay.struct)
             nat.check(lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
-            nat.check(lib.eqd_iegmn_layer_forward_stash(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
-                                                        nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(mu),
-                                                        nat.ptr(h_out), nat.ptr(x_out), nat.ptr(status), st),
-                      'eqd_iegmn_layer_forward_stash')
+            nat.check(lib.eqd_iegmn_layer_forward(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
+                                                  nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(mu),
+                                                  nat.ptr(h_out), nat.ptr(x_out), nat.ptr(status), st),
+                      'eqd_iegmn_layer_forward')
         if int(status[plan.n_pairs].item()) & nat.STATUS_DEGREE_OVERFLOW:
             raise nat.NativeLibraryError(f'IEGMN_Layer.forward: in-degree above {plan.struct.max_in_degree}')
         ctx.saved = (plan, lay, layout, tp, h, h0, x_in, aggr, mu)

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define EQD_ABI_VERSION 10
+#define EQD_ABI_VERSION 11
 
 #define EQD_EDGE_FEATS 27     /* input_edge_feats_dim, protein_utils.py:71-86 + :373-389 */
 #define EQD_N_RBF 15          /* all_sigmas_dist = 1.5**s, rigid_docking_model.py:116 */
@@ -202,10 +202,12 @@ int eqd_edge_stage_ffma(const eqd_graph* g, const eqd_layer* p, const float* pro
 
 /* Node stage (:244-256, 319-349): segmented cross attention mu = softmax(q k^T) v over the partner
  * protein, node MLP + LayerNorm + skip -> h_out[n][64]; if p_next != NULL also the next layer's
- * projections (fused eqd_project on h_out) into proj_next.                                    */
+ * projections (fused eqd_project on h_out) into proj_next.  mu: NULL, or [n][dhp] (16-byte aligned) that
+ * receives the attention output (row stride 72 with columns 69..71 zero for the 69-wide layer 0, 64
+ * otherwise): the operand of eqd_bwd_node_mlp / eqd_bwd_attention that the per-layer backward reads.  */
 int eqd_node_stage(const eqd_graph* g, const eqd_layer* p, const eqd_layer* p_next,
                    const float* h_in, int32_t ldh, const float* h0, const float* proj,
-                   const float* aggr, float* h_out, float* proj_next, void* stream);
+                   const float* aggr, float* mu, float* h_out, float* proj_next, void* stream);
 
 /* ---- tensor-core node stage (wgmma, layers with dh == 64) ---------------------------------------------
  * K and V of every node travel as bf16x3 "8-node blocks": kv[which 2 (K,V)][split 3][n/8 (+8 zero pad
@@ -257,20 +259,13 @@ int eqd_node_stage_tc0(const eqd_graph* g, const eqd_layer* p, const eqd_layer* 
                        float* proj_next, void* stream);
 
 /* One whole IEGMN_Layer.forward = eqd_edge_stage + eqd_node_stage (proj must hold this layer's
- * projections on entry; holds the next layer's on exit when p_next != NULL).                  */
+ * projections on entry; holds the next layer's on exit when p_next != NULL).  mu as in eqd_node_stage: NULL, or the
+ * layer's attention output, which the per-layer backward reads together with h_in, h0, x_in and aggr.          */
 int eqd_iegmn_layer_forward(const eqd_graph* g, const eqd_layer* p, const eqd_layer* p_next,
                             const float* h_in, int32_t ldh, const float* h0,
                             const double* x_in, const double* x_orig,
-                            float* proj, float* proj_next, float* aggr,
+                            float* proj, float* proj_next, float* aggr, float* mu,
                             float* h_out, double* x_out, int32_t* status, void* stream);
-/* Same outputs (bit for bit), and the layer's attention output mu [n][dhp] (row stride 72 with columns 69..71 zero for
- * the 69-wide layer 0, 64 otherwise; 16-byte aligned, required): the operand of eqd_bwd_node_mlp / eqd_bwd_attention
- * that the per-layer backward reads together with h_in, h0, x_in and aggr.                                    */
-int eqd_iegmn_layer_forward_stash(const eqd_graph* g, const eqd_layer* p, const eqd_layer* p_next,
-                                  const float* h_in, int32_t ldh, const float* h0,
-                                  const double* x_in, const double* x_orig,
-                                  float* proj, float* proj_next, float* aggr, float* mu,
-                                  float* h_out, double* x_out, int32_t* status, void* stream);
 
 /* Weights-only fold of the 50-head key / query projections (att_mlp_key_ROT, att_mlp_query_ROT :427-438) into
  * m_qk (see eqd_head_params), so that the per-protein logits are h_j . (m_qk[k]^T qbar) (:544-546, :555-557).
@@ -323,7 +318,6 @@ typedef struct eqd_forward_io {
   /* optional: HOST array of 4*n_layers cudaEvent_t handles (edge begin, edge end, node begin, node end per layer) recorded
    * on `stream`; NULL entries are skipped.  eqd_event_create / _elapsed_ms / _destroy wrap the CUDA calls.          */
   void* const* stage_events;
-  int32_t layer0_fp32;        /* != 0: keep the 69-wide layer 0 on the fp32 CUDA-core kernels */
   /* training: NULL, or eqd_forward_stash_bytes(g, n_layers) bytes of 256-byte aligned device memory that receives every
    * layer's inputs and intermediate node tensors (layout: eqd_forward_stash_offsets) for the backward entry points */
   void* train_stash;

@@ -38,7 +38,8 @@ for li in range(cfg.n_layers):
     st = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
     lib.eqd_edge_stage(G, L, nat.ptr(proj), nat.ptr(xin), nat.ptr(x0), nat.ptr(aggr), nat.ptr(xo), nat.ptr(st), None)
     hf = torch.zeros(N, 64, device=dev)
-    lib.eqd_node_stage(G, L, None, nat.ptr(hin), dhp, nat.ptr(h0p), nat.ptr(proj), nat.ptr(aggr), nat.ptr(hf), None, None)
+    lib.eqd_node_stage(G, L, None, nat.ptr(hin), dhp, nat.ptr(h0p), nat.ptr(proj), nat.ptr(aggr), None, nat.ptr(hf), None,
+                       None)
     torch.cuda.synchronize()
     msg = f'layer {li}: aggr err {np.abs(aggr.cpu().numpy() - want_ag).max():.2e}  FFMA node h err {np.abs(hf.cpu().numpy() - want_h).max():.2e}'
     if lay.dh == 64:

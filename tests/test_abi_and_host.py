@@ -39,7 +39,7 @@ def test_header_constants_match_binding():
         assert int(re.search(rf'#define {name} (\d+)', h).group(1)) == val
 
 
-def test_struct_layouts_are_natural_c_layouts():
+def test_abi_v11_struct_layouts_are_natural_c_layouts():
     assert ctypes.sizeof(nat.EqdGraph) == 24 + 6 * 8 + 8 + 8
     assert nat.EqdGraph.seg_ptr.offset == 24 and nat.EqdGraph.node_tiles.offset == 80
     assert nat.EqdLayerParams.w_proj.offset == 8 and nat.EqdLayerParams.b_coor2.offset == 8 + 10 * 8
@@ -51,9 +51,8 @@ def test_struct_layouts_are_natural_c_layouts():
     assert not any(n.endswith('_host') for n, _ in nat.EqdLayerParams._fields_)
     assert ctypes.sizeof(nat.EqdHeadParams) == 5 * 8 + 8
     assert nat.EqdHeadParams.m_qk.offset == 32 and nat.EqdHeadParams.leaky_slope.offset == 40
-    assert ctypes.sizeof(nat.EqdForwardIO) == 18 * 8 + 8 + 16 and nat.EqdForwardIO.stage_events.offset == 17 * 8
-    assert nat.EqdForwardIO.train_stash.offset == 19 * 8 and nat.EqdForwardIO.train_stash_bytes.offset == 20 * 8
-    assert nat.EqdForwardIO.layer0_fp32.offset == 18 * 8
+    assert ctypes.sizeof(nat.EqdForwardIO) == 18 * 8 + 16 and nat.EqdForwardIO.stage_events.offset == 17 * 8
+    assert nat.EqdForwardIO.train_stash.offset == 18 * 8 and nat.EqdForwardIO.train_stash_bytes.offset == 19 * 8
 
 
 def _header_struct_fields(name):

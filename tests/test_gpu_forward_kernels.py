@@ -329,9 +329,10 @@ def _layer1_next(mod1, h_out, pn, kv, N, rep, tag):
 
 
 @pytest.mark.parametrize('kind', ['bench', 'ragged', 'long', 'sizes'])
-def test_layer0_node_stage_tc0_and_fp32_route_vs_fp64(kind, cuda_device):
+def test_layer0_node_stage_tc0_and_panelless_fp32_route_vs_fp64(kind, cuda_device):
     """eqd_node_stage_tc0 with p_next = layer 1 (h_out; Psrc | Pdst | Q of proj_next; layer 1's K/V blocks), and the
-    route of layer0_fp32: eqd_project (ldh 72), eqd_node_stage at dh 69, eqd_kv_blocks."""
+    fp32 CUDA-core route of a layer 0 without tensor-core panels: eqd_project (ldh 72), eqd_node_stage at dh 69 with its
+    attention output mu [n][72] (what the training stash keeps for such a layer), eqd_kv_blocks."""
     dev, lib = cuda_device, nat.load()
     _, plan = _fbatch(kind, dev)
     mod, lay, _ = _layer(0, dev)
@@ -362,20 +363,23 @@ def test_layer0_node_stage_tc0_and_fp32_route_vs_fp64(kind, cuda_device):
     def fp32():
         p = torch.full((N, 344), SENT, device=dev)
         nat.check(lib.eqd_project(G, L, nat.ptr(h0), 72, nat.ptr(p), None), 'eqd_project')
+        mu = torch.full((N, 72), SENT, device=dev)
         h_out = torch.full((N, 64), float('nan'), device=dev)
         pn = torch.full((N, 320), SENT, device=dev)
-        nat.check(lib.eqd_node_stage(G, L, Ln, nat.ptr(h0), 72, nat.ptr(h0), nat.ptr(p), nat.ptr(aggr), nat.ptr(h_out),
-                                     nat.ptr(pn), None), 'eqd_node_stage')
+        nat.check(lib.eqd_node_stage(G, L, Ln, nat.ptr(h0), 72, nat.ptr(h0), nat.ptr(p), nat.ptr(aggr), nat.ptr(mu),
+                                     nat.ptr(h_out), nat.ptr(pn), None), 'eqd_node_stage')
         kvf = torch.zeros(lib.eqd_kv_blocks_bytes(N), dtype=torch.uint8, device=dev)
         nat.check(lib.eqd_kv_blocks(G, nat.ptr(pn), 320, 192, 256, nat.ptr(kvf), None), 'eqd_kv_blocks')
-        return p, h_out, pn, kvf
+        return p, mu, h_out, pn, kvf
 
-    p, h_out, pn, kvf = _twice(fp32)
+    p, mu, h_out, pn, kvf = _twice(fp32)
     ref = fs.projections(mod, h069)
     for name, base in (('Psrc', 0), ('Pdst', 64), ('Q', 128), ('K', 200), ('V', 272)):
         w = 64 if name.startswith('P') else 69
         rep.rel(f'fp32 proj {name}', p[:, base:base + w], ref[name])
     mu_ref = fs.attention(seg, _d(p[:, 128:197]), _d(p[:, 200:269]), _d(p[:, 272:341]))
+    rep.rel('fp32 mu', mu[:, :69], mu_ref)
+    assert torch.equal(mu[:, 69:], torch.zeros(N, 3, device=dev))      # the padded V columns are 0
     rep.rel('fp32 h_out', h_out, fs.node_mlp(mod, h069, _d(aggr), mu_ref, h069))
     _layer1_next(mod1, h_out, pn, kvf, N, rep, 'fp32')
     rep.rel('fp32 proj_next K, V (fp32 columns)', pn[:, 192:320],

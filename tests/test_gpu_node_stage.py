@@ -65,8 +65,9 @@ def _rel_err(a, ref):
 
 
 @pytest.mark.parametrize('n_bulk', [0, 80])
-def test_node_stage_tensor_core_vs_fp32_twin(n_bulk, cuda_device):
-    """n_bulk = 80 adds 80 pairs of 200 + 200 nodes: 640 query tiles of 64 rows, more than the resident tile chains hold,
+def test_node_stage_tensor_core_vs_fp32_twin_with_mu(n_bulk, cuda_device):
+    """The tensor-core node stage against its fp32 CUDA-core twin, and the attention output mu of both (the fp32 twin
+    writes it when given a buffer) against fp64.  n_bulk = 80 adds 80 pairs of 200 + 200 nodes: 640 query tiles of 64 rows, more than the resident tile chains hold,
     so every chain runs several tiles and prefetches across them.  n_nodes is not a multiple of 64 in either case."""
     dev = cuda_device
     lib = nat.load()
@@ -90,8 +91,9 @@ def test_node_stage_tensor_core_vs_fp32_twin(n_bulk, cuda_device):
 
     h_ref = torch.full((N, 64), float('nan'), device=dev)
     pn_ref = torch.full((N, 320), float('nan'), device=dev)
-    assert lib.eqd_node_stage(G, L, Ln, nat.ptr(h), 64, nat.ptr(h0), nat.ptr(proj), nat.ptr(aggr), nat.ptr(h_ref),
-                              nat.ptr(pn_ref), None) == 0
+    mu_ff = torch.full((N, 64), float('nan'), device=dev)
+    assert lib.eqd_node_stage(G, L, Ln, nat.ptr(h), 64, nat.ptr(h0), nat.ptr(proj), nat.ptr(aggr), nat.ptr(mu_ff),
+                              nat.ptr(h_ref), nat.ptr(pn_ref), None) == 0
     mu = torch.full((N, 64), float('nan'), device=dev)
     h_tc = torch.full((N, 64), float('nan'), device=dev)
     pn_tc = torch.full((N, 320), float('nan'), device=dev)
@@ -109,6 +111,8 @@ def test_node_stage_tensor_core_vs_fp32_twin(n_bulk, cuda_device):
         mu_ref[seg[s]:seg[s + 1]] = torch.softmax(q @ k.t(), 1) @ v
     assert torch.isfinite(mu).all()
     assert _rel_err(mu, mu_ref) <= 1e-5
+    assert torch.isfinite(mu_ff).all()
+    assert _rel_err(mu_ff, mu_ref) <= 1e-5
 
     assert torch.isfinite(h_tc).all()
     assert _rel_err(h_tc, h_ref) <= 1e-5

@@ -11,6 +11,7 @@ coordinates (|coords| up to 64 A -> one ulp = 3.8e-6 A), so each is only known t
 additive term.  The per-pair errors of a build are written by scripts/parity_table.py.  The yardstick itself is one
 sample of fp32 rounding noise: the reference's fp32 evaluation of a pair changes with the BLAS thread count.
 """
+import copy
 import ctypes as C
 
 import numpy as np
@@ -330,31 +331,28 @@ def test_c_abi_rejects_bad_arguments(cuda_device):
                                nat.ptr(one), None) == -2                         # 48-wide layer
 
 
-def test_one_call_forward_equals_stage_by_stage_driver(models, cuda_device, monkeypatch):
-    """eqd_iegmn_forward (one C call, one workspace) chains exactly the kernels the Python driver launches one by
-    one: outputs are bitwise identical, for both checkpoints (5 shared layers / 8 layers) and a ragged batch."""
-    from equidock_public_b200 import engine as eng
-    for ds in ('db5', 'dips'):
-        names, pairs, _, _ = gio.load_pairs(ds)
-        outs = {}
-        for py in (False, True):
-            monkeypatch.setattr(eng, '_PY_FORWARD', py)
-            g = gio.make_batch([pairs[n] for n in names[:3]], cuda_device)
-            coors, kl, kr, rot, tr = models[ds](g, epoch=0)
-            outs[py] = (torch.cat(coors), torch.stack(rot), torch.stack(tr), torch.stack(kl), torch.stack(kr),
-                        g.nodes['ligand'].data['hv_iegmn_out'].clone(), g.nodes['receptor'].data['x_iegmn_out'].clone())
-        for a, b in zip(outs[False], outs[True]):
-            assert torch.equal(a, b)
+def _layer0_without_panels(model, monkeypatch):
+    """For the rest of the test, layer 0 of `model` hands the engine a copy of its eqd_layer with the tensor-core panels
+    (w_proj_tc, w_node_tc) set to NULL: by the ABI's rule that layer then runs on the fp32 CUDA-core kernels."""
+    lay0 = model.iegmn_original.iegmn_layers[0]
+    packed = lay0.packed
+
+    def without_panels(device):
+        p = copy.copy(packed(device))
+        p.struct = nat.EqdLayer.from_buffer_copy(p.struct)
+        p.struct.dev.w_proj_tc = p.struct.dev.w_node_tc = None
+        return p
+    monkeypatch.setattr(lay0, 'packed', without_panels)
 
 
-def test_layer0_tensor_core_path_vs_fp32_cuda_core_path(models, cuda_device, monkeypatch):
+def test_layer0_tensor_core_path_vs_panelless_fp32_path(models, cuda_device, monkeypatch):
     """The 69-wide layer 0 on the tensor cores (K = 80 panels, 64 TC + 5 fp32 attention channels) against the fp32
     CUDA-core kernels for the same layer: the two evaluate the same formulas with different roundings."""
-    from equidock_public_b200 import engine as eng
     names, pairs, outs, _ = gio.load_pairs('dips')
     res = {}
     for ffma in (False, True):
-        monkeypatch.setattr(eng, '_LAYER0_FFMA', ffma)
+        if ffma:
+            _layer0_without_panels(models['dips'], monkeypatch)
         g = gio.make_batch([pairs[n] for n in names], cuda_device)
         coors, _, _, rot, _ = models['dips'](g, epoch=0)
         res[ffma] = (coors, rot)
@@ -362,6 +360,49 @@ def test_layer0_tensor_core_path_vs_fp32_cuda_core_path(models, cuda_device, mon
         yard = np.abs(outs[n]['ref32']['ligand_coors'] - outs[n]['ref64']['ligand_coors']).max()
         d = (res[False][0][i] - res[True][0][i]).abs().max().item()
         assert d <= 2 * max(COORD_TOL, 2 * yard), (n, d, yard)
+
+
+def test_fp32_layer_writes_its_attention_output_to_the_training_stash(models, cuda_device, monkeypatch):
+    """A layer that eqd_iegmn_forward runs on the fp32 CUDA-core node stage still fills its slot mu[l] of the training
+    stash, which the backward reads: with layer 0 on the fp32 kernels and a stash that reads NaN everywhere beforehand,
+    stash mu[0] (and aggr[0]) equal bit for bit what eqd_iegmn_layer_forward computes from the stashed h0 and x[0]."""
+    from equidock_public_b200 import engine as eng
+    from equidock_public_b200.training import TrainEngine
+    model = models['dips']
+    _layer0_without_panels(model, monkeypatch)
+    forward = eng.IEGMNEngine.forward
+
+    def nan_stash(self, *args, train_stash=None, **kw):
+        train_stash.fill_(0xFF)      # every float of the stash is NaN until the forward writes it
+        return forward(self, *args, train_stash=train_stash, **kw)
+    monkeypatch.setattr(eng.IEGMNEngine, 'forward', nan_stash)
+    names, pairs, _, _ = gio.load_pairs('dips')
+    fwd = TrainEngine(model).forward(gio.make_batch([pairs[n] for n in names[:3]], cuda_device))
+    plan, stash, offs, lay = fwd['plan'], fwd['stash'], fwd['stash_offsets'], fwd['layers'][0]
+    assert lay.dh == nat.H0 and not lay.struct.dev.w_proj_tc and not lay.struct.dev.w_node_tc
+    N, dev = plan.N, cuda_device
+
+    def at(off, dt, cols):   # the [N][cols] tensor of the stash at byte offset `off`
+        return stash[off:off + N * cols * (torch.finfo(dt).bits // 8)].view(dt).view(N, cols)
+    h0, x0 = at(offs[0], torch.float32, nat.H0_PAD), at(offs[1], torch.float64, 3)
+    aggr_st, mu_st = at(offs[5], torch.float32, nat.HID), at(offs[7], torch.float32, nat.H0_PAD)
+
+    lib = nat.load()
+    G, L = C.byref(plan.struct), C.byref(lay.struct)
+    proj = torch.empty(N, 128 + 3 * nat.H0_PAD, dtype=torch.float32, device=dev)
+    aggr = torch.empty(N, nat.HID, dtype=torch.float32, device=dev)
+    h_out = torch.empty(N, nat.HID, dtype=torch.float32, device=dev)
+    mu = torch.full((N, nat.H0_PAD), float('nan'), dtype=torch.float32, device=dev)
+    x_out = torch.empty(N, 3, dtype=torch.float64, device=dev)
+    status = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
+    st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    nat.check(lib.eqd_project(G, L, nat.ptr(h0), nat.H0_PAD, nat.ptr(proj), st), 'eqd_project')
+    nat.check(lib.eqd_iegmn_layer_forward(G, L, None, nat.ptr(h0), nat.H0_PAD, nat.ptr(h0), nat.ptr(x0), nat.ptr(x0),
+                                          nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(mu), nat.ptr(h_out),
+                                          nat.ptr(x_out), nat.ptr(status), st), 'eqd_iegmn_layer_forward')
+    assert torch.isfinite(mu).all()
+    assert torch.equal(aggr_st, aggr)
+    assert torch.equal(mu_st, mu)
 
 
 @pytest.mark.timeout(180)
