@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # EQD_LIB_PATH: load another build of the same ABI instead (A/B runs of kernel variants, scripts/forward_ab.py)
 LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.so')
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
@@ -34,7 +34,7 @@ class EqdLayerParams(C.Structure):
                 ('b_coor2', _f32), ('w_edge_tc', _vp), ('w_node_tc', _vp), ('w_proj_tc', _vp),
                 ('w_node1', _vp), ('b_node1', _vp), ('node_ln_g', _vp), ('node_ln_b', _vp),
                 ('w_node2', _vp), ('b_node2', _vp),
-                ('skip_weight_h', _f32), ('x_connection_init', _f32), ('leaky_slope', _f32)]
+                ('skip_weight_h', _f32), ('x_connection_init', _f32), ('leaky_slope', _f32), ('mma_products', _i32)]
 
 
 class EqdLayerConsts(C.Structure):

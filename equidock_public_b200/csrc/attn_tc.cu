@@ -257,6 +257,8 @@ attention0_tc_kernel(eqd_graph g, const float* __restrict__ proj, int pw, const 
 // boundaries, so the next tile's first K and V chunks land during this tile's last chunk.  The next tile's Q rows are
 // cp.async'ed into the staging buffer during this tile.  The chunk walk (8-node blocks from the partner's first block)
 // does not depend on the query tile: every per-element sum has the order of the 128-row kernel it replaces.
+// P = 3 (bf16x3): pass 2's S and O GEMMs take the three leading products on two-term Q / P splits; pass 1 is hi-only in
+// both modes.  The K / V chunks are copied whole (their third split is not read).
 #define AT_CHAINS 2
 
 struct __align__(128) AtChainSmem {
@@ -272,6 +274,7 @@ struct AtTile {        // one 64-row query tile
   int blk_lo, nchunks; // first 8-node block of the walk, 64-key chunks
 };
 
+template <int P>
 __global__ void __launch_bounds__(AT_CHAINS * 128, 1)
 attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigned char* __restrict__ kv,
                       long kv_split_stride, float* __restrict__ mu) {
@@ -353,7 +356,7 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
     cp_async_wait<0>();
     wg_barrier(bar);
     unsigned qf[3][4][4];
-    staged_rows_to_a_split3(W.qs, t, qf);
+    staged_rows_to_a_split3<P>(W.qs, t, qf);
     wg_barrier(bar);   // the staging buffer is free
     auto k_desc = [&](int kb_) {
       return [&, kb_](int sp, int kk) { return b_desc_ex(k_saddr + (kb_ * 3 + sp) * AT_CHUNK_BYTES + kk * 256, 128, 1024); };
@@ -403,7 +406,7 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
         fill(W.v, W.v_bar, vfill, v_g, nxt.blk_lo);
       }
       float s[32];
-      wg_gemm6_rs_issue<64, 4>(s, qf, k_desc(kb_), false);
+      wg_gemm6_rs_issue<64, 4, 0, false, P>(s, qf, k_desc(kb_), false);
       wg_mma_wait(s);
       const int key0 = (cur.blk_lo + 8 * c) * 8 + fc;
 #pragma unroll
@@ -437,10 +440,10 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
           }
       }
       unsigned pf[3][4][4];
-      acc_to_a_split3<4>(s, pf);
+      acc_to_a_split3<4, P>(s, pf);
       const int vb_ = consume(W.v_bar, vcons);
       float o[32];
-      wg_gemm6_rs_issue<64, 4, 1>(o, pf, [&](int sp, int kk) {
+      wg_gemm6_rs_issue<64, 4, 1, false, P>(o, pf, [&](int sp, int kk) {
         return b_desc_ex(v_saddr + (vb_ * 3 + sp) * AT_CHUNK_BYTES + kk * 2048, 1024, 128); }, false);
       wg_mma_wait(o);
       // The tensor core truncates (round-toward-zero) every time it adds into an fp32 accumulator, a systematic bias that
@@ -470,22 +473,35 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
   cp_async_wait<0>();
 }
 
-}  // namespace eqd
-
-extern "C" int eqd_attention_tc(const eqd_graph* g, const float* proj, const void* kv, float* mu, void* stream) {
-  if (!g || !proj || !kv || !mu) return EQD_ERR_BAD_ARG;
-  if (reinterpret_cast<uintptr_t>(kv) & 15) return EQD_ERR_BAD_ARG;
-  if (g->n_node_tiles <= 0) return EQD_OK;
-  const size_t smem = AT_CHAINS * sizeof(eqd::AtChainSmem);
-  EQD_SET_SMEM(eqd::attention64_tc_kernel, smem);
+template <int P>
+static int launch_attention64_tc(const eqd_graph* g, const float* proj, const void* kv, float* mu, void* stream) {
+  const size_t smem = AT_CHAINS * sizeof(AtChainSmem);
+  EQD_SET_SMEM(attention64_tc_kernel<P>, smem);
   const int nht = 2 * g->n_node_tiles;
   int grid = (nht + AT_CHAINS - 1) / AT_CHAINS;
   if (grid > EQD_SMS) grid = EQD_SMS;
   const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
-  eqd::attention64_tc_kernel<<<grid, AT_CHAINS * 128, smem, (cudaStream_t)stream>>>(
+  attention64_tc_kernel<P><<<grid, AT_CHAINS * 128, smem, (cudaStream_t)stream>>>(
       *g, proj, reinterpret_cast<const unsigned char*>(kv), split_stride, mu);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
+}
+
+}  // namespace eqd
+
+// eqd_attention_tc with the product count of a layer's tensor-core GEMMs (6 or 3, eqd_mma_products); the node stage's
+// entry point, not part of the C ABI
+int eqd_attention_tc_products(const eqd_graph* g, const float* proj, const void* kv, float* mu, int products, void* stream) {
+  if (!g || !proj || !kv || !mu) return EQD_ERR_BAD_ARG;
+  if (reinterpret_cast<uintptr_t>(kv) & 15) return EQD_ERR_BAD_ARG;
+  if (products != 6 && products != 3) return EQD_ERR_UNSUPPORTED;
+  if (g->n_node_tiles <= 0) return EQD_OK;
+  return products == 3 ? eqd::launch_attention64_tc<3>(g, proj, kv, mu, stream)
+                       : eqd::launch_attention64_tc<6>(g, proj, kv, mu, stream);
+}
+
+extern "C" int eqd_attention_tc(const eqd_graph* g, const float* proj, const void* kv, float* mu, void* stream) {
+  return eqd_attention_tc_products(g, proj, kv, mu, 6, stream);
 }
 
 extern "C" int eqd_attention_tc0(const eqd_graph* g, const float* proj, const void* kv, const float* x5, float* mu,

@@ -41,6 +41,13 @@
     }                                                                                                          \
   } while (0)
 
+// Product count of a layer's tensor-core GEMMs (eqd_layer_params.mma_products): 6 for 0 or 6 (bf16x6), 3 for 3 on a
+// 64-wide layer (bf16x3); 0 for any other value, which the tensor-core launchers refuse with EQD_ERR_UNSUPPORTED.
+inline int eqd_mma_products(const eqd_layer_params* p) {
+  if (p->mma_products == 0 || p->mma_products == 6) return 6;
+  return p->mma_products == 3 && p->dh == EQD_HID ? 3 : 0;
+}
+
 namespace eqd {
 
 // LeakyReLU for 0 <= slope <= 1 (checked by the launchers): max(v, slope*v) is bit-identical to the select form

@@ -21,6 +21,7 @@
 // Rounding: every step is that of a row-per-thread epilogue on shared-memory operands: the split, the six products, their
 // order and the accumulation chain of every GEMM output, the Psrc/Pdst add order, the LayerNorm and phi summation chains
 // (chain_val), the two-chain mean aggregation and the fp64 coordinate update.
+// P = 3 (bf16x3, eqd_layer_params.mma_products): the same kernel with two-term A splits and the three leading products.
 #include "tc_common.cuh"
 
 namespace eqd {
@@ -60,6 +61,7 @@ struct TcSmem {
   unsigned long long w_bar;
 };
 
+template <int P>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ EdgeConsts cst_p,
                      const float* __restrict__ proj, const double* __restrict__ x_in, const double* __restrict__ x_orig,
@@ -242,9 +244,9 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
       }
       unsigned p0[12], p1[12], p2[12];
 #pragma unroll
-      for (int c = 0; c < 12; ++c) split3_pair(a1v[2 * c], a1v[2 * c + 1], p0[c], p1[c], p2[c]);
+      for (int c = 0; c < 12; ++c) split3_pair<P>(a1v[2 * c], a1v[2 * c + 1], p0[c], p1[c], p2[c]);
 #pragma unroll
-      for (int j = 0; j < 3; ++j) a_store8<TC_ROWS>(W.a, TC_A_SPLIT, r, half * 24 + 8 * j, p0 + 4 * j, p1 + 4 * j, p2 + 4 * j);
+      for (int j = 0; j < 3; ++j) a_store8<TC_ROWS, P>(W.a, TC_A_SPLIT, r, half * 24 + 8 * j, p0 + 4 * j, p1 + 4 * j, p2 + 4 * j);
     }
     tc_fence_before();
     // The A operand is complete and the he staging consumed.  The barrier also tells whether every node of the tile has
@@ -254,7 +256,7 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     unsigned af[3][4][4];
     {
       float v[32];
-      wg_gemm6_issue<64>(v, a_desc, [&](int sp, int kb) { return b_desc_ex(w_saddr + sp * TC_W1_SPLIT + kb * 2048, 1024, 128); },
+      wg_gemm6_issue<64, 0, P>(v, a_desc, [&](int sp, int kb) { return b_desc_ex(w_saddr + sp * TC_W1_SPLIT + kb * 2048, 1024, 128); },
                          3, false);
       if (has_next) prefetch(tile + tstride, buf ^ 1, e0n, e1n, off_ln, n_ln, off_rn);
       wg_mma_wait(v);
@@ -317,7 +319,7 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
           x1 = fmaf(__fmul_rn(__fadd_rn(x1, -mean[h]), rstd[h]), gj.y, bj.y);
         }
       }
-      acc_to_a_split3<4>(v, af);
+      acc_to_a_split3<4, P>(v, af);
     }
     if (has_next) {
       // The next tile's x[src] / x[dst] gathers go out two GEMMs before they are needed: my own index of the next tile
@@ -335,8 +337,8 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
           return b_desc_ex(w_saddr + TC_W23_BASE + sp * TC_W23_SPLIT + kb * 4096 + hn * 1024, 2048, 128); };
       };
       float m[32], hd[32];
-      wg_gemm6_rs_issue<64>(m, af, w23(0), false);
-      wg_gemm6_rs_issue<64>(hd, af, w23(1), false);
+      wg_gemm6_rs_issue<64, 4, 0, false, P>(m, af, w23(0), false);
+      wg_gemm6_rs_issue<64, 4, 0, false, P>(hd, af, w23(1), false);
       wg_mma_wait(m);
       wg_mma_wait(hd);   // (the second wait only pins hd behind the first)
       float u[32];   // LeakyReLU(hidden + b3)
@@ -435,6 +437,22 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
   __syncthreads();
 }
 
+template <int P>
+static int launch_edge_stage_tc(const eqd_graph* g, const eqd_layer* p_l, const float* proj, const double* x_in,
+                                const double* x_orig, float* aggr, double* x_out, int32_t* status, int tn, void* stream) {
+  const int ntiles = (g->n_nodes + tn - 1) / tn;
+  EdgeConsts cst;
+  memcpy(&cst, p_l->consts.edge, sizeof(cst));
+  size_t smem = sizeof(TcSmem) + 128;
+  EQD_SET_SMEM((edge_stage_tc_kernel<P>), smem);
+  int grid = (ntiles + TC_WGS - 1) / TC_WGS;
+  if (grid > EQD_SMS) grid = EQD_SMS;
+  edge_stage_tc_kernel<P><<<grid, TC_THREADS, smem, (cudaStream_t)stream>>>(*g, p_l->dev, cst, proj, x_in, x_orig, aggr,
+                                                                           x_out, status, tn);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
+}
+
 }  // namespace eqd
 
 extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const float* proj, const double* x_in,
@@ -442,6 +460,8 @@ extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const fl
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !proj || !x_in || !x_orig || !aggr || !x_out || !status) return EQD_ERR_BAD_ARG;
   if (!p->w_edge_tc) return EQD_ERR_BAD_ARG;
+  const int products = eqd_mma_products(p);
+  if (!products) return EQD_ERR_UNSUPPORTED;
   if (g->max_in_degree < 1 || g->max_in_degree > EQD_TM) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
   if ((reinterpret_cast<uintptr_t>(g->he_lig) | reinterpret_cast<uintptr_t>(g->he_rec) |
@@ -452,15 +472,6 @@ extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const fl
   if (g->n_nodes <= 0) return EQD_OK;
   int tn = TC_ROWS / g->max_in_degree;
   if (tn > TC_MAX_TN) tn = TC_MAX_TN;
-  int ntiles = (g->n_nodes + tn - 1) / tn;
-  eqd::EdgeConsts cst;
-  memcpy(&cst, p_l->consts.edge, sizeof(cst));
-  size_t smem = sizeof(eqd::TcSmem) + 128;
-  EQD_SET_SMEM((eqd::edge_stage_tc_kernel), smem);
-  int grid = (ntiles + TC_WGS - 1) / TC_WGS;
-  if (grid > EQD_SMS) grid = EQD_SMS;
-  eqd::edge_stage_tc_kernel<<<grid, TC_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, cst, proj, x_in, x_orig, aggr, x_out,
-                                                                             status, tn);
-  EQD_CUDA_LAUNCH_CHECK();
-  return EQD_OK;
+  return products == 3 ? eqd::launch_edge_stage_tc<3>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream)
+                       : eqd::launch_edge_stage_tc<6>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream);
 }

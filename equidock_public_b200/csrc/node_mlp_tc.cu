@@ -25,6 +25,7 @@ struct NmConsts { float b5[64], ln_g[64], ln_b[64], b6[64]; };
 // fragments; the skip line takes h from the registers of piece 0 and h' leaves by direct fragment stores (a quad writes
 // 32 contiguous bytes of a row).  Every element of h' takes the splits, products, order and epilogue of the 128-row kernel
 // this one replaced, with the same multiply-add contraction (pinned below with the _rn intrinsics).
+// P = 3 (bf16x3): two-term A splits and the three leading products in both GEMMs.
 #define NM_CHAINS 2
 #define NM_SLOTS 3   // staging buffers per chain: pieces are issued NM_SLOTS - 1 ahead
 
@@ -35,6 +36,7 @@ struct NmSmem {
   unsigned long long w_bar;
 };
 
+template <int P>
 __global__ void __launch_bounds__(NM_CHAINS * 128, 1)
 node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmConsts cst, const float* __restrict__ h_in,
                    const float* __restrict__ aggr, const float* __restrict__ mu, const float* __restrict__ h0,
@@ -106,9 +108,9 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
         for (int i = 0; i < 32; ++i) hs[i] = v[i];   // the skip operand
       }
       unsigned af[3][4][4];
-      acc_to_a_split3<4>(v, af);
+      acc_to_a_split3<4, P>(v, af);
       float d[32];
-      wg_gemm6_rs_issue<64, 4>(d, af, [&](int sp, int kb) {
+      wg_gemm6_rs_issue<64, 4, 0, false, P>(d, af, [&](int sp, int kb) {
         return b_desc_ex(w_saddr + (4 * pc + kb) * 2048 + sp * NM_W5_SPLIT, 1024, 128); }, false);
       wg_mma_wait(d);
 #pragma unroll
@@ -117,11 +119,11 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
     {
       unsigned a4[3][1][4];
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) split3_pair(x4[hh].x, x4[hh].y, a4[0][0][hh], a4[1][0][hh], a4[2][0][hh]);
+      for (int hh = 0; hh < 2; ++hh) split3_pair<P>(x4[hh].x, x4[hh].y, a4[0][0][hh], a4[1][0][hh], a4[2][0][hh]);
 #pragma unroll
       for (int sp = 0; sp < 3; ++sp) a4[sp][0][2] = a4[sp][0][3] = 0u;
       float d[32];
-      wg_gemm6_rs_issue<64, 1>(d, a4, [&](int sp, int kb) {
+      wg_gemm6_rs_issue<64, 1, 0, false, P>(d, a4, [&](int sp, int kb) {
         return b_desc_ex(w_saddr + 16 * 2048 + sp * NM_W5_SPLIT, 1024, 128); }, false);
       wg_mma_wait(d);
 #pragma unroll
@@ -180,11 +182,11 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
           x1 = __fmaf_rn(__fmul_rn(__fmaf_rn(msum[h], -0.5f, x1), rstd[h]), gj.y, bj.y);
         }
       }
-      acc_to_a_split3<4>(v, af);
+      acc_to_a_split3<4, P>(v, af);
     }
     {
       float d[32];
-      wg_gemm6_rs_issue<64, 4>(d, af, [&](int sp, int kb) {
+      wg_gemm6_rs_issue<64, 4, 0, false, P>(d, af, [&](int sp, int kb) {
         return b_desc_ex(w_saddr + NM_W6_BASE + sp * NM_W6_SPLIT + kb * 2048, 1024, 128); }, false);
       wg_mma_wait(d);
 #pragma unroll
@@ -384,6 +386,22 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
   }
 }
 
+template <int P>
+static int launch_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const float* h_in, const float* aggr,
+                              const float* mu, const float* h0, float* h_out, void* stream) {
+  NmConsts cst;
+  memcpy(&cst, p_l->consts.node, sizeof(cst));
+  const int ntiles = (g->n_nodes + 63) / 64;
+  const size_t smem = sizeof(NmSmem) + 128;
+  EQD_SET_SMEM(node_mlp_tc_kernel<P>, smem);
+  int grid = (ntiles + NM_CHAINS - 1) / NM_CHAINS;
+  if (grid > EQD_SMS) grid = EQD_SMS;
+  node_mlp_tc_kernel<P><<<grid, NM_CHAINS * 128, smem, (cudaStream_t)stream>>>(g->n_nodes, p_l->dev, cst, h_in, aggr, mu,
+                                                                             h0, h_out);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
+}
+
 }  // namespace eqd
 
 extern "C" int eqd_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const float* h_in, const float* aggr,
@@ -392,25 +410,19 @@ extern "C" int eqd_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const f
   if (!g || !p || !h_in || !aggr || !mu || !h0 || !h_out) return EQD_ERR_BAD_ARG;
   if (p->dh != 64 || p->dhp != 64) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
+  const int products = eqd_mma_products(p);
+  if (!products) return EQD_ERR_UNSUPPORTED;
   if (!p->w_node_tc || (reinterpret_cast<uintptr_t>(p->w_node_tc) & 15)) return EQD_ERR_BAD_ARG;
   if (g->n_nodes <= 0) return EQD_OK;
-  eqd::NmConsts cst;
-  memcpy(&cst, p_l->consts.node, sizeof(cst));
-  const int ntiles = (g->n_nodes + 63) / 64;
-  const size_t smem = sizeof(eqd::NmSmem) + 128;
-  EQD_SET_SMEM(eqd::node_mlp_tc_kernel, smem);
-  int grid = (ntiles + NM_CHAINS - 1) / NM_CHAINS;
-  if (grid > EQD_SMS) grid = EQD_SMS;
-  eqd::node_mlp_tc_kernel<<<grid, NM_CHAINS * 128, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h_in, aggr, mu, h0, h_out);
-  EQD_CUDA_LAUNCH_CHECK();
-  return EQD_OK;
+  return products == 3 ? eqd::launch_node_mlp_tc<3>(g, p_l, h_in, aggr, mu, h0, h_out, stream)
+                       : eqd::launch_node_mlp_tc<6>(g, p_l, h_in, aggr, mu, h0, h_out, stream);
 }
 
 extern "C" int eqd_node_mlp_tc0(const eqd_graph* g, const eqd_layer* p_l, const float* h0, const float* aggr,
                                 const float* mu, float* h_out, void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !h0 || !aggr || !mu || !h_out) return EQD_ERR_BAD_ARG;
-  if (p->dh != 69 || p->dhp != 72) return EQD_ERR_UNSUPPORTED;
+  if (p->dh != 69 || p->dhp != 72 || !eqd_mma_products(p)) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
   if (!p->w_node_tc || (reinterpret_cast<uintptr_t>(p->w_node_tc) & 15)) return EQD_ERR_BAD_ARG;
   if (g->n_nodes <= 0) return EQD_OK;
@@ -435,6 +447,7 @@ extern "C" int eqd_node_stage_tc0(const eqd_graph* g, const eqd_layer* p_l, cons
   const eqd_layer_params* p_next = p_next_l ? &p_next_l->dev : nullptr;
   if (!g || !p || !kv || !mu || !x5) return EQD_ERR_BAD_ARG;
   if (p_next && !proj_next) return EQD_ERR_BAD_ARG;
+  if (!eqd_mma_products(p)) return EQD_ERR_UNSUPPORTED;   // layer 0 runs bf16x6 only
   int rc = eqd_attention_tc0(g, proj, kv, x5, mu, stream);
   if (rc) return rc;
   rc = eqd_node_mlp_tc0(g, p_l, h0, aggr, mu, h_out, stream);
@@ -444,7 +457,9 @@ extern "C" int eqd_node_stage_tc0(const eqd_graph* g, const eqd_layer* p_l, cons
 }
 
 extern "C" int eqd_project_tc(const eqd_graph*, const eqd_layer*, const float*, float*, void*, void*);
-extern "C" int eqd_attention_tc(const eqd_graph*, const float*, const void*, float*, void*);
+int eqd_attention_tc_products(const eqd_graph*, const float*, const void*, float*, int, void*);
+
+// Attention and node MLP take this layer's product count, the next layer's projections that of p_next.
 
 extern "C" int eqd_node_stage_tc(const eqd_graph* g, const eqd_layer* p_l, const eqd_layer* p_next_l,
                                  const float* h_in, const float* h0, const float* proj, const float* aggr, void* kv,
@@ -453,7 +468,9 @@ extern "C" int eqd_node_stage_tc(const eqd_graph* g, const eqd_layer* p_l, const
   const eqd_layer_params* p_next = p_next_l ? &p_next_l->dev : nullptr;
   if (!g || !p || !kv || !mu) return EQD_ERR_BAD_ARG;
   if (p_next && !proj_next) return EQD_ERR_BAD_ARG;
-  int rc = eqd_attention_tc(g, proj, kv, mu, stream);
+  const int products = eqd_mma_products(p);
+  if (!products) return EQD_ERR_UNSUPPORTED;
+  int rc = eqd_attention_tc_products(g, proj, kv, mu, products, stream);
   if (rc) return rc;
   rc = eqd_node_mlp_tc(g, p_l, h_in, aggr, mu, h0, h_out, stream);
   if (rc) return rc;

@@ -176,6 +176,8 @@ project_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjCon
 // | Q (and K | V without K/V blocks) leave through the chain's staging tile as whole 256-byte rows; K and V go straight from
 // the fragments into the 8-node kv blocks (a quad writes 16 contiguous bytes of a block row, a warp 8 whole block rows).
 // Every output element takes the split, products, order and epilogue of the 128-row kernel it replaces.
+// P = 3 (bf16x3): two-term h splits and the three leading products.  The K / V blocks are written as full bf16x3 in both
+// modes, so the attention of either mode can read them.
 #define PJ_CHAINS 2
 #define PJ64_W_BYTES (5 * PjCfg<false>::GROUP_BYTES)
 #define PJ_OUT_LD 72   // fp32 row stride of the output staging tile (72 % 32 = 8: the fragment stores are conflict-free)
@@ -191,6 +193,7 @@ struct Pj64Smem {
   unsigned long long w_bar;
 };
 
+template <int P>
 __global__ void __launch_bounds__(PJ_CHAINS * 128, 1)
 project64_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjConsts cst, const float* __restrict__ h,
                     float* __restrict__ proj, unsigned char* __restrict__ kv, long kv_split_stride) {
@@ -222,19 +225,19 @@ project64_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ PjC
     cp_async_wait<0>();
     wg_barrier(bar);   // this tile's h rows have landed
     unsigned af[3][4][4];
-    staged_rows_to_a_split3(W.hs, t, af);
+    staged_rows_to_a_split3<P>(W.hs, t, af);
     wg_barrier(bar);   // the staging buffer is free
     if (tile + tstride < ntiles) stage_h(tile + tstride);
     auto group = [&](int grp) {
       return [&, grp](int s, int kb) { return b_desc_ex(w_saddr + grp * PjCfg<false>::GROUP_BYTES + s * PjCfg<false>::SPLIT_BYTES + kb * 2048, 1024, 128); };
     };
     float acc[2][32];
-    wg_gemm6_rs_issue<64, 4>(acc[0], af, group(0), false);
+    wg_gemm6_rs_issue<64, 4, 0, false, P>(acc[0], af, group(0), false);
 #pragma unroll
     for (int grp = 0; grp < 5; ++grp) {
       float (&d)[32] = acc[grp & 1];
       if (grp + 1 < 5) {
-        wg_gemm6_rs_issue<64, 4>(acc[(grp + 1) & 1], af, group(grp + 1), false);
+        wg_gemm6_rs_issue<64, 4, 0, false, P>(acc[(grp + 1) & 1], af, group(grp + 1), false);
         wg_mma_wait<1>(d);
       } else {
         wg_mma_wait(d);
@@ -340,34 +343,43 @@ static int launch_project_tc(const eqd_graph* g, const eqd_layer* p_l, const flo
   return EQD_OK;
 }
 
+template <int P>
+static int launch_project64_tc(const eqd_graph* g, const eqd_layer* p_l, const float* h, float* proj, void* kv,
+                               void* stream) {
+  eqd::PjConsts cst;
+  memset(&cst, 0, sizeof(cst));
+  memcpy(&cst, p_l->consts.proj_bias, 320 * sizeof(float));
+  const int ntiles = (g->n_nodes + 63) / 64;
+  const size_t smem = sizeof(eqd::Pj64Smem) + 128;
+  EQD_SET_SMEM(eqd::project64_tc_kernel<P>, smem);
+  int grid = (ntiles + PJ_CHAINS - 1) / PJ_CHAINS;
+  if (grid > EQD_SMS) grid = EQD_SMS;
+  const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
+  eqd::project64_tc_kernel<P><<<grid, PJ_CHAINS * 128, smem, (cudaStream_t)stream>>>(
+      g->n_nodes, p_l->dev, cst, h, proj, reinterpret_cast<unsigned char*>(kv), split_stride);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
+}
+
 extern "C" int eqd_project_tc(const eqd_graph* g, const eqd_layer* p_l, const float* h, float* proj, void* kv,
                               void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !h || !proj) return EQD_ERR_BAD_ARG;
   if (p->dh != 64 || p->dhp != 64) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
+  const int products = eqd_mma_products(p);
+  if (!products) return EQD_ERR_UNSUPPORTED;
   if (!p->w_proj_tc || (reinterpret_cast<uintptr_t>(p->w_proj_tc) & 15)) return EQD_ERR_BAD_ARG;
   if (g->n_nodes <= 0) return EQD_OK;
-  eqd::PjConsts cst;
-  memset(&cst, 0, sizeof(cst));
-  memcpy(&cst, p_l->consts.proj_bias, 320 * sizeof(float));
-  const int ntiles = (g->n_nodes + 63) / 64;
-  const size_t smem = sizeof(eqd::Pj64Smem) + 128;
-  EQD_SET_SMEM(eqd::project64_tc_kernel, smem);
-  int grid = (ntiles + PJ_CHAINS - 1) / PJ_CHAINS;
-  if (grid > EQD_SMS) grid = EQD_SMS;
-  const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
-  eqd::project64_tc_kernel<<<grid, PJ_CHAINS * 128, smem, (cudaStream_t)stream>>>(
-      g->n_nodes, *p, cst, h, proj, reinterpret_cast<unsigned char*>(kv), split_stride);
-  EQD_CUDA_LAUNCH_CHECK();
-  return EQD_OK;
+  return products == 3 ? launch_project64_tc<3>(g, p_l, h, proj, kv, stream)
+                       : launch_project64_tc<6>(g, p_l, h, proj, kv, stream);
 }
 
 extern "C" int eqd_project_tc0(const eqd_graph* g, const eqd_layer* p_l, const float* h0, float* proj, void* kv,
                                float* x5, void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !h0 || !proj || !kv || !x5) return EQD_ERR_BAD_ARG;
-  if (p->dh != 69 || p->dhp != 72) return EQD_ERR_UNSUPPORTED;
+  if (p->dh != 69 || p->dhp != 72 || !eqd_mma_products(p)) return EQD_ERR_UNSUPPORTED;
   return launch_project_tc<true>(g, p_l, h0, EQD_H0_PAD, proj, 128 + 3 * 72, kv, x5, stream);
 }
 

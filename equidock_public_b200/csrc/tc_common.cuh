@@ -12,6 +12,12 @@
 //       along K), SBO (along N).
 //   D : fp32 accumulator fragments of each warpgroup's 64 rows, stored to a row-major shared-memory tile
 //       (wg_store_d) from which every thread reads its own row.
+//
+// Product count P (template parameter of the GEMM and split helpers, default 6): P = 6 is bf16x6 as above; P = 3 is
+// "bf16x3", the opt-in mode of the 64-wide layers (eqd_layer_params.mma_products): only the two leading split terms of
+// each operand are used and the three products a1w0, a0w1, a0w0 are accumulated (same order, the product loop starts at
+// 3).  Each product then carries a relative error of about 2^-16 instead of 2^-24.  With P = 3 the helpers compute and
+// store no third A split; B operands keep their three splits in memory (the third is not read).
 #pragma once
 #include "common.cuh"
 
@@ -107,18 +113,19 @@ struct WgmmaRS<64, TB> {
   }
 };
 
-// bf16x6 GEMM of one 64-row slab on the calling warpgroup: d (+)= sum over the 6 split products (smallest terms
-// first) and k-blocks [0, kblocks) of A[split][kb] . B[split][kb]^T; a_desc(split, kb) / b_desc(split, kb) give the
-// operand descriptors.  hi_only: just the leading bf16 x bf16 product.  The _issue form returns with the MMAs in flight
-// (one commit group; wg_mma_wait completes them), wg_gemm6 with the MMAs complete.
-template <int N, int TB = 0, class AD, class BD>
+// bf16x6 GEMM of one 64-row slab on the calling warpgroup: d (+)= sum over the last P of the 6 split products (smallest
+// terms first) and k-blocks [0, kblocks) of A[split][kb] . B[split][kb]^T; a_desc(split, kb) / b_desc(split, kb) give
+// the operand descriptors.  hi_only: just the leading bf16 x bf16 product.  The _issue form returns with the MMAs in
+// flight (one commit group; wg_mma_wait completes them), wg_gemm6 with the MMAs complete.
+template <int N, int TB = 0, int P = 6, class AD, class BD>
 __device__ __forceinline__ void wg_gemm6_issue(float (&d)[N / 2], AD a_desc, BD b_desc, int kblocks, bool accumulate,
                                                bool hi_only = false) {
+  static_assert(P == 6 || P == 3, "bf16x6 or bf16x3");
   const int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
   int scale_d = accumulate ? 1 : 0;
 #pragma unroll
-  for (int pr = hi_only ? 5 : 0; pr < 6; ++pr)
+  for (int pr = hi_only ? 5 : 6 - P; pr < 6; ++pr)
     for (int kb = 0; kb < kblocks; ++kb) {
       Wgmma<N, TB>::mma(d, a_desc(pa[pr], kb), b_desc(pb[pr], kb), scale_d);
       scale_d = 1;
@@ -133,21 +140,22 @@ __device__ __forceinline__ void wg_mma_wait(float (&d)[M]) {
 #pragma unroll
   for (int i = 0; i < M; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <int N, int TB = 0, class AD, class BD>
+template <int N, int TB = 0, int P = 6, class AD, class BD>
 __device__ __forceinline__ void wg_gemm6(float (&d)[N / 2], AD a_desc, BD b_desc, int kblocks, bool accumulate,
                                          bool hi_only = false) {
-  wg_gemm6_issue<N, TB>(d, a_desc, b_desc, kblocks, accumulate, hi_only);
+  wg_gemm6_issue<N, TB, P>(d, a_desc, b_desc, kblocks, accumulate, hi_only);
   asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
 }
-// wg_gemm6_issue with A from registers: a[split][kb] are the bf16x3 A fragments (acc_to_a_split3), same product order;
-// HI_ONLY: just the leading bf16 x bf16 product.  Returns with the MMAs in flight (wg_mma_wait).
-template <int N, int KB, int TB = 0, bool HI_ONLY = false, class BD>
+// wg_gemm6_issue with A from registers: a[split][kb] are the bf16x3 A fragments (acc_to_a_split3), same product order
+// (P = 3: a[2] is not read); HI_ONLY: just the leading bf16 x bf16 product.  Returns with the MMAs in flight (wg_mma_wait).
+template <int N, int KB, int TB = 0, bool HI_ONLY = false, int P = 6, class BD>
 __device__ __forceinline__ void wg_gemm6_rs_issue(float (&d)[N / 2], const unsigned (&a)[3][KB][4], BD b_desc, bool accumulate) {
+  static_assert(P == 6 || P == 3, "bf16x6 or bf16x3");
   constexpr int pa[6] = {2, 0, 1, 1, 0, 0}, pb[6] = {0, 2, 1, 0, 1, 0};
   asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
   int scale_d = accumulate ? 1 : 0;
 #pragma unroll
-  for (int pr = HI_ONLY ? 5 : 0; pr < 6; ++pr)
+  for (int pr = HI_ONLY ? 5 : 6 - P; pr < 6; ++pr)
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb) {
       WgmmaRS<N, TB>::mma(d, a[pa[pr]][kb], b_desc(pb[pr], kb), scale_d);
@@ -163,14 +171,14 @@ template <int R>
 __device__ __forceinline__ unsigned long long a_desc_at(unsigned a_saddr, unsigned split_bytes, int wgi, int s, int kb) {
   return b_desc_ex(a_saddr + s * split_bytes + kb * (32 * R) + wgi * 1024, 16 * R, 128);
 }
-// 8 consecutive channels [c, c + 8) of `row` (c a multiple of 8), as three packed bf16x3 split rows
-template <int R>
+// 8 consecutive channels [c, c + 8) of `row` (c a multiple of 8), as three packed bf16x3 split rows (P = 3: two)
+template <int R, int P = 6>
 __device__ __forceinline__ void a_store8(unsigned char* a, unsigned split_bytes, int row, int c, const unsigned* p0,
                                          const unsigned* p1, const unsigned* p2) {
   unsigned char* base = a + (c >> 4) * (32 * R) + ((c >> 3) & 1) * (16 * R) + (row >> 3) * 128 + (row & 7) * 16;
   *reinterpret_cast<uint4*>(base) = make_uint4(p0[0], p0[1], p0[2], p0[3]);
   *reinterpret_cast<uint4*>(base + split_bytes) = make_uint4(p1[0], p1[1], p1[2], p1[3]);
-  *reinterpret_cast<uint4*>(base + 2 * split_bytes) = make_uint4(p2[0], p2[1], p2[2], p2[3]);
+  if constexpr (P == 6) *reinterpret_cast<uint4*>(base + 2 * split_bytes) = make_uint4(p2[0], p2[1], p2[2], p2[3]);
 }
 
 // wgmma m64nN accumulator fragment of warpgroup thread t -> rows [0, 64) of a row-major fp32 tile (ld floats per row)
@@ -190,13 +198,14 @@ __device__ __forceinline__ unsigned cvt_bf16x2(float hi, float lo) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(hi), "f"(lo));
   return d;
 }
-// (v0, v1) -> three packed bf16x2 words (v0 in the low half = even k)
+// (v0, v1) -> three packed bf16x2 words (v0 in the low half = even k); P = 3: the first two only (p2 is not written)
+template <int P = 6>
 __device__ __forceinline__ void split3_pair(float v0, float v1, unsigned& p0, unsigned& p1, unsigned& p2) {
   p0 = cvt_bf16x2(v1, v0);
   // v - hi, exact: hi is v rounded to bf16
   const float r0 = v0 - __uint_as_float(p0 << 16), r1 = v1 - __uint_as_float(p0 & 0xFFFF0000u);
   p1 = cvt_bf16x2(r1, r0);
-  p2 = cvt_bf16x2(r1 - __uint_as_float(p1 & 0xFFFF0000u), r0 - __uint_as_float(p1 << 16));
+  if constexpr (P == 6) p2 = cvt_bf16x2(r1 - __uint_as_float(p1 & 0xFFFF0000u), r0 - __uint_as_float(p1 << 16));
 }
 // 32 fp32 values = channels [c0, c0 + 32) of `row` -> bf16x3 -> A operand
 template <int R>
@@ -221,12 +230,12 @@ __device__ __forceinline__ void store_extra8_split3(unsigned char* a, unsigned s
 // m64nN fp32 accumulator fragment (N = 16 KB columns) -> bf16x3 A fragments of an RS wgmma whose K runs over those
 // columns.  The accumulator's (row, column) ownership is the A fragment's (row, k) ownership: d[8kb + 2i], d[8kb + 2i + 1]
 // hold (row g + 8 (i & 1), k = 16 kb + 8 (i >> 1) + 2 (lane & 3) + {0, 1}) = A register i of k-block kb.
-template <int KB>
+template <int KB, int P = 6>
 __device__ __forceinline__ void acc_to_a_split3(const float (&v)[8 * KB], unsigned (&a)[3][KB][4]) {
 #pragma unroll
   for (int kb = 0; kb < KB; ++kb)
 #pragma unroll
-    for (int i = 0; i < 4; ++i) split3_pair(v[8 * kb + 2 * i], v[8 * kb + 2 * i + 1], a[0][kb][i], a[1][kb][i], a[2][kb][i]);
+    for (int i = 0; i < 4; ++i) split3_pair<P>(v[8 * kb + 2 * i], v[8 * kb + 2 * i + 1], a[0][kb][i], a[1][kb][i], a[2][kb][i]);
 }
 // bf16x3 RS A fragments (k = 64 channels, 4 k-blocks) of warpgroup thread t from 64 fp32 rows of 64 channels staged in
 // shared memory by 16-byte chunks, chunk k4 of row r at position k4 ^ stage_swz(r) (the fragment loads are then free of
@@ -243,6 +252,7 @@ __device__ __forceinline__ void stage_rows64(float* rows, const float* src, int 
   }
   cp_async_commit();
 }
+template <int P = 6>
 __device__ __forceinline__ void staged_rows_to_a_split3(const float* rows, int t, unsigned (&a)[3][4][4]) {
   const int g = (t >> 5) * 16 + ((t & 31) >> 2), c = t & 3;
 #pragma unroll
@@ -251,7 +261,7 @@ __device__ __forceinline__ void staged_rows_to_a_split3(const float* rows, int t
     for (int i = 0; i < 4; ++i) {
       const int row = g + 8 * (i & 1), k4 = 4 * kb + 2 * (i >> 1) + (c >> 1);
       const float2 v = *reinterpret_cast<const float2*>(rows + row * 64 + ((k4 ^ stage_swz(row)) << 2) + 2 * (c & 1));
-      split3_pair(v.x, v.y, a[0][kb][i], a[1][kb][i], a[2][kb][i]);
+      split3_pair<P>(v.x, v.y, a[0][kb][i], a[1][kb][i], a[2][kb][i]);
     }
 }
 // The same staged values unsplit, in the m64n64 accumulator layout (the A fragments' ownership: v[8 kb + 2 i + e] is

@@ -64,6 +64,17 @@ def umma_bf16x3(w: torch.Tensor) -> torch.Tensor:
 # read by bench.py; the forward is always the one C call of IEGMNEngine.forward
 _PY_FORWARD = False
 
+# IEGMN.precision -> eqd_layer_params.mma_products of the 64-wide layers (layer 0 always runs bf16x6):
+#   'fp32'   : bf16x6 tensor-core GEMMs, fp32-level results (the default)
+#   'bf16x3' : three products on two-term bf16 splits, about 2^-16 relative error per product
+PRECISIONS = {'fp32': 0, 'bf16x3': 3}
+
+
+def check_precision(precision: str) -> str:
+    if precision not in PRECISIONS:
+        raise ValueError(f'precision must be one of {sorted(PRECISIONS)}, got {precision!r}')
+    return precision
+
 
 class PackedLayer:
     """One IEGMN_Layer's parameters repacked k-major for the kernels (see eqd_layer_params)."""
@@ -164,6 +175,19 @@ class PackedLayer:
         s.b_coor2 = float(sd['coors_mlp.4.bias'].detach().reshape(-1)[0].item())
         s.skip_weight_h, s.x_connection_init, s.leaky_slope = skip_weight_h, x_connection_init, leaky_slope
         self.struct = lay
+        self._descriptors = {}
+
+    def descriptor(self, mma_products: int = 0):
+        """The layer's eqd_layer with ``mma_products`` set: ``self.struct`` itself for 0 and for the 69-wide layer 0,
+        else a copy of it (sharing the device panels), cached while ``self.struct`` stays the same object."""
+        if mma_products == 0 or self.dh != nat.HID:
+            return self.struct
+        src, d = self._descriptors.get(mma_products, (None, None))
+        if src is not self.struct:
+            d = nat.EqdLayer.from_buffer_copy(self.struct)
+            d.dev.mma_products = mma_products
+            self._descriptors[mma_products] = (self.struct, d)
+        return d
 
 
 class PackedHead:
@@ -436,9 +460,11 @@ class IEGMNEngine:
 
     def forward(self, plan: GraphPlan, emb: torch.Tensor, layers: List[PackedLayer], head: PackedHead,
                 res_l, res_r, mu_l, mu_r, x_l, x_r, check_status: bool = True, log=None,
-                stage_timer=None, record_event: bool = True, train_stash=None) -> Dict[str, torch.Tensor]:
+                stage_timer=None, record_event: bool = True, train_stash=None,
+                mma_products: int = 0) -> Dict[str, torch.Tensor]:
         """One forward = ONE call into the library (eqd_iegmn_forward): the per-stage entry points are chained in C on
-        the current stream out of a single workspace allocation."""
+        the current stream out of a single workspace allocation.  ``mma_products`` (0 or 3, see ``PRECISIONS``) goes
+        to the descriptors of the 64-wide layers."""
         with torch.cuda.device(self.device):   # the raw launches below go to the CURRENT device: make it the model's
             lib, dev = self.lib, self.device
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
@@ -469,7 +495,7 @@ class IEGMNEngine:
                 io.train_stash, io.train_stash_bytes = train_stash.data_ptr(), int(train_stash.numel())
             events = stage_timer.new_forward(len(layers)) if stage_timer is not None else None
             io.stage_events = C.cast(events, C.c_void_p) if events is not None else None
-            larr = (C.POINTER(nat.EqdLayer) * len(layers))(*[C.pointer(l.struct) for l in layers])
+            larr = (C.POINTER(nat.EqdLayer) * len(layers))(*[C.pointer(l.descriptor(mma_products)) for l in layers])
             nat.check(lib.eqd_iegmn_forward(g, larr, len(layers), C.byref(head.struct), C.byref(io), nat.ptr(ws),
                                             plan.forward_ws_bytes, st), 'eqd_iegmn_forward')
             kab = lambda mask: nat.check(lib.eqd_kabsch_apply(

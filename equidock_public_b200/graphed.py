@@ -13,8 +13,9 @@ edge list or a bad residue index was flagged -- falls back to the eager path, wh
 control flow (rigid_docking_model.py:570-584).  The captured work is exactly the eager path's: same kernels, same
 order, same buffers.
 
-The graph is tied to the parameter version it was captured with (kernel parameter banks hold small per-layer
-vectors): ``launch()`` re-captures when a parameter changed.
+The graph is tied to the parameter version and the precision (``IEGMN.precision``) it was captured with (kernel
+parameter banks hold small per-layer vectors and the product count selects the kernels): ``launch()`` re-captures when
+either changed.
 """
 from __future__ import annotations
 
@@ -39,7 +40,7 @@ class GraphedForward:
         self._capture()
 
     def _param_key(self):
-        return tuple((p.data_ptr(), p._version) for p in self.model.parameters())
+        return tuple((p.data_ptr(), p._version) for p in self.model.parameters()) + (self.iegmn.precision,)
 
     def _capture(self):
         with torch.cuda.device(self.device):

@@ -41,7 +41,7 @@ except ImportError:  # DGL-free deployments use the package's own container
     fn = None
 
 from . import _native as nat
-from .engine import GraphPlan, IEGMNEngine, PackedHead, PackedLayer, UnsortedEdges, _sorted_copy
+from .engine import PRECISIONS, GraphPlan, IEGMNEngine, PackedHead, PackedLayer, UnsortedEdges, _sorted_copy, check_precision
 from .hetero_graph import LIGAND, LL, RECEPTOR, RR
 
 
@@ -354,6 +354,19 @@ class IEGMN(nn.Module):
                                             get_non_lin(args['nonlin'], args['leakyrelu_neg_slope']))
         self._head, self._head_key = None, None
         self.last_outputs = None
+        self._precision = 'fp32'
+
+    @property
+    def precision(self) -> str:
+        """Arithmetic of the tensor-core GEMMs of layers 1..L-1 at inference: ``'fp32'`` (default; bf16x6, fp32-level
+        agreement with an fp64 evaluation) or ``'bf16x3'`` (three products on two-term bf16 splits, about 2^-16 relative
+        error per product, half the tensor-core work).  Layer 0, the keypoint head and Kabsch are the same in both.  The
+        autograd paths refuse ``'bf16x3'``."""
+        return self._precision
+
+    @precision.setter
+    def precision(self, value: str):
+        self._precision = check_precision(value)
 
     def reset_parameters(self):
         for p in self.parameters():
@@ -386,9 +399,10 @@ class IEGMN(nn.Module):
         nl, nr = batch_hetero_graph.nodes[LIGAND].data, batch_hetero_graph.nodes[RECEPTOR].data
         plan = _plan_for(batch_hetero_graph, dev, self.graph_max_neighbor)
         emb32 = emb.detach().to(torch.float32).contiguous()
+        products = PRECISIONS[self.precision]
         call = lambda p, chk: eng.forward(p, emb32, layers, head, nl['res_feat'], nr['res_feat'], nl['mu_r_norm'],
                                           nr['mu_r_norm'], nl['new_x'], nr['x'], chk, self.log,
-                                          record_event=record_event)
+                                          record_event=record_event, mma_products=products)
         try:
             out = call(plan, check_status)
         except UnsortedEdges:
@@ -456,6 +470,15 @@ class Rigid_Body_Docking_Net(nn.Module):
             raise NotImplementedError("fine_tune=True is outside the CUDA engine's scope (both checkpoints: fine_F)")
         self.iegmn_original = IEGMN(args, n_lays=args['iegmn_n_lays'], fine_tune=False, log=log)
         self.list_iegmns = [('finetune', self.iegmn_original)]
+
+    @property
+    def precision(self) -> str:
+        """``IEGMN.precision`` of the model's IEGMN: ``'fp32'`` (default) or ``'bf16x3'``."""
+        return self.iegmn_original.precision
+
+    @precision.setter
+    def precision(self, value: str):
+        self.iegmn_original.precision = value
 
     def reset_parameters(self):
         for p in self.parameters():

@@ -510,11 +510,21 @@ class _HotPath(torch.autograd.Function):
         return (None, *in_grads, *eng.layout.views(flat))
 
 
+def check_fp32_precision(model):
+    """The CUDA backward recomputes every layer from the stash in fp32 arithmetic: under ``precision='bf16x3'`` its
+    gradients would not belong to the forward that ran, so training and autograd refuse that mode."""
+    precision = getattr(model, 'iegmn_original', model).precision
+    if precision != 'fp32':
+        raise NotImplementedError(f"precision={precision!r} is an inference mode: autograd and training need "
+                                  "precision='fp32' (the CUDA backward recomputes the forward in fp32)")
+
+
 def autograd_forward(model, graph, log=None):
     """Runs the model's hot path as ONE autograd node and returns (raw outputs dict, the six differentiable outputs:
     ligand coordinates, keypoints, rotations, translations, last-layer coordinates (N,3) f64, last-layer features).
     ``model`` is a Rigid_Body_Docking_Net or an IEGMN module."""
     from .rigid_docking_model import graph_inputs
+    check_fp32_precision(model)
     eng = getattr(model, '_eqd_train_engine', None)
     if eng is None or eng.device != getattr(model, 'iegmn_original', model).residue_emb_layer.weight.device:
         eng = TrainEngine(model)
@@ -682,6 +692,7 @@ class DataParallelTrainer:
     def __init__(self, model, lr: float, weight_decay: float = 0.0, clip: float = 100.0, betas=(0.9, 0.999), eps: float = 1e-8,
                  pocket_ot_loss_weight: float = 1.0, intersection_loss_weight: float = 10.0, intersection_sigma: float = 25.0,
                  intersection_surface_ct: float = 10.0, world: int = 1, group=None):
+        check_fp32_precision(model)
         self.model = model.train()
         self.engine = TrainEngine(model)
         self.layout = self.engine.layout
@@ -711,6 +722,7 @@ class DataParallelTrainer:
 
     def step(self, graph, targets) -> Dict:
         from .losses import device_losses
+        check_fp32_precision(self.model)
         dev, eng = self.device, self.engine
         with torch.cuda.device(dev):
             compute = torch.cuda.current_stream(dev)

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define EQD_ABI_VERSION 11
+#define EQD_ABI_VERSION 12
 
 #define EQD_EDGE_FEATS 27     /* input_edge_feats_dim, protein_utils.py:71-86 + :373-389 */
 #define EQD_N_RBF 15          /* all_sigmas_dist = 1.5**s, rigid_docking_model.py:116 */
@@ -122,6 +122,15 @@ typedef struct eqd_layer_params {
   float skip_weight_h;        /* args['skip_weight_h'] (applied only when dh == 64, :332-337) */
   float x_connection_init;    /* args['x_connection_init'] (:286-292) */
   float leaky_slope;          /* args['leakyrelu_neg_slope'] */
+  /* Products per GEMM of the tensor-core kernels of this layer (edge stage, projections, attention, node MLP):
+   *   0 or 6 : bf16x6, the default.  Operands split into three bf16 terms, six products: fp32-level results (about 1e-4 A
+   *            on the output coordinates against an fp64 evaluation).
+   *   3      : bf16x3, 64-wide layers only (dh == 64).  Two-term splits, the products a1w0, a0w1, a0w0: each product
+   *            carries a relative error of at most about 2^-16 instead of 2^-24, so a GEMM output sum_k a_k w_k is off by
+   *            up to about 2^-16 * sum_k |a_k w_k|, for half the tensor-core work.
+   * Any other value, or 3 on the 69-wide layer 0, makes the tensor-core entry points return EQD_ERR_UNSUPPORTED.  The fp32
+   * CUDA-core kernels ignore the field.  It fills what was tail padding: sizeof and every other offset are unchanged. */
+  int32_t mma_products;
 } eqd_layer_params;
 
 /* Launch-time constants of the tensor-core kernels, BY VALUE in host memory: the launcher copies them into the kernel's
