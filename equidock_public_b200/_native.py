@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # EQD_LIB_PATH: load another build of the same ABI instead (A/B runs of kernel variants, scripts/forward_ab.py)
 LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.so')
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
@@ -56,6 +56,22 @@ class EqdForwardIO(C.Structure):
 
 class EqdHeadParams(C.Structure):
     _fields_ = [('w_mean', _vp), ('b_mean', _vp), ('w_key', _vp), ('w_query', _vp), ('m_qk', _vp), ('leaky_slope', _f32)]
+
+
+class EqdPairArchive(C.Structure):
+    """eqd_pair_archive: device pointers of a pair archive uploaded once (datasets.DevicePairDataset)."""
+    _fields_ = [('n_pairs', _i32)] + [(n, _vp) for n in (
+        'lig_node_ptr', 'rec_node_ptr', 'lig_edge_ptr', 'rec_edge_ptr', 'pocket_ptr', 'lig_res_feat', 'rec_res_feat',
+        'lig_x', 'rec_x', 'lig_mu_r_norm', 'rec_mu_r_norm', 'lig_src', 'lig_dst', 'rec_src', 'rec_dst', 'lig_he', 'rec_he',
+        'lig_new_x', 'pocket_coors', 'bound_lig', 'bound_rec', 'lig_centroid')]
+
+
+class EqdBatchOut(C.Structure):
+    """eqd_batch_out: the device arrays one eqd_assemble_batch call writes."""
+    _fields_ = [(n, _vp) for n in ('res_feat', 'x', 'new_x', 'mu_r_norm', 'row_ptr', 'col_src', 'edge_dst', 'he_lig', 'he_rec',
+                                   'seg_ptr',
+                                   'node_tiles', 'pocket_ptr', 'pocket_lig', 'pocket_rec', 'bound_lig', 'bound_rec', 'rot',
+                                   'trans')]
 
 
 # symbol -> (restype, argtypes); every symbol include/eqd_iegmn.h declares must be listed here
@@ -104,6 +120,8 @@ PROTOTYPES = {
     'eqd_graph_build_workspace_bytes': (C.c_size_t, [_i32]),
     'eqd_graph_build_knn': (C.c_int, [_i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     'eqd_graph_build_edges': (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'eqd_assemble_batch': (C.c_int, [C.POINTER(EqdPairArchive), _i32, _vp, _i32, C.c_uint64, C.c_uint64, _i32, _f32, _i32,
+                                     C.POINTER(EqdBatchOut), _vp]),
     'eqd_rmsd_meter': (C.c_int, [_G, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_sqnorm_partials': (C.c_int, [_vp, C.c_int64, _vp, _i32, _vp]),
     'eqd_clip_adam': (C.c_int, [_vp, _vp, _vp, _vp, C.c_int64, _vp, _i32, _f32, _f32, _f32, _f32, _f32, _f32, _i32, _f32, _vp, _vp]),

@@ -327,6 +327,41 @@ class GraphPlan:
         return True
 
     @classmethod
+    def from_device_arrays(cls, n_lig: Sequence[int], n_rec: Sequence[int], E_l: int, E: int, col_src, edge_dst, row_ptr,
+                           he_l, he_r, seg_ptr, node_tiles, seg_ptr_host, device, max_in_degree: int = 10, keep=()) -> 'GraphPlan':
+        """Plan over topology arrays the device already holds in the engine's layout (graph_build.build_graphs,
+        datasets.DevicePairDataset): no copy, no check, no sync.  ``col_src`` / ``edge_dst`` are global node ids grouped by
+        destination, ``row_ptr`` [N+1] their CSR.  ``he_l`` / ``he_r``: 16-byte aligned edge features with one readable
+        row past the end, either one buffer [E+1][27] for both edge types passed twice (n_lig_edges = E) or the ligand
+        rows [E_l+1][27] and the receptor rows [E_r+1][27] (n_lig_edges = E_l).  ``seg_ptr`` [2B+1] / ``node_tiles`` [T][2] int32 on the device, ``seg_ptr_host`` the same
+        offsets on the host, ``device`` the device the plan reports.  ``keep`` holds tensors the plan's pointers depend on."""
+        plan = cls.__new__(cls)
+        B, dev = len(n_lig), device
+        plan.n_pairs, plan.forward_ws_bytes = B, None
+        plan.n_lig_list, plan.n_rec_list = [int(v) for v in n_lig], [int(v) for v in n_rec]
+        N_l, N = sum(plan.n_lig_list), sum(plan.n_lig_list) + sum(plan.n_rec_list)
+        plan.N_l, plan.N_r, plan.N, plan.device = N_l, N - N_l, N, dev
+        plan.E_l, plan.E_r, plan.E = int(E_l), int(E) - int(E_l), int(E)
+        plan.col_src, plan.edge_dst, plan.row_ptr = col_src, edge_dst, row_ptr
+        plan.unsorted = torch.zeros((), dtype=torch.bool, device=dev)
+        plan.unsorted_i32 = torch.zeros(1, dtype=torch.int32, device=dev)
+        plan._arange = None
+        plan.edge_perm = None
+        plan.he_l, plan.he_r = he_l, he_r
+        plan.seg_ptr_host, plan.n_node_tiles = seg_ptr_host, int(node_tiles.numel()) // 2
+        plan.seg_ptr, plan.node_tiles = seg_ptr, node_tiles
+        gs = nat.EqdGraph()
+        gs.n_pairs, gs.n_nodes, gs.n_lig_nodes = B, N, N_l
+        gs.n_edges, gs.n_lig_edges, gs.max_in_degree = plan.E, plan.E if he_r is he_l else plan.E_l, int(max_in_degree)
+        gs.seg_ptr, gs.row_ptr = seg_ptr.data_ptr(), row_ptr.data_ptr()
+        gs.col_src, gs.edge_dst = col_src.data_ptr(), edge_dst.data_ptr()
+        gs.he_lig, gs.he_rec = he_l.data_ptr(), he_r.data_ptr()
+        gs.n_node_tiles, gs.node_tiles = plan.n_node_tiles, node_tiles.data_ptr()
+        plan.struct = gs
+        plan._keep = keep
+        return plan
+
+    @classmethod
     def from_graph(cls, graph, device, max_in_degree: int = 10) -> 'GraphPlan':
         """From a batched DGL heterograph (train_utils.py:61-100) or a ``PairGraphBatch``."""
         n_l = graph.batch_num_nodes(LIGAND).tolist()

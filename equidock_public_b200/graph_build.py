@@ -149,32 +149,13 @@ def build_graphs(rb: ResidueBatch, device, cutoff: float = 30.0, max_neighbor: i
     g._ndata[RECEPTOR] = {'res_feat': d['res_feat'][N_l:], 'x': x[N_l:], 'mu_r_norm': mu[N_l:]}
     if sync_sizes:
         g._edata[LL]['he'], g._edata[RR]['he'] = he[:E_l], he[E_l:E]
-    # plan over the device-built arrays (no copies; the whole edge list is addressed through `he_lig`)
-    plan = GraphPlan.__new__(GraphPlan)
-    plan.n_pairs, plan.forward_ws_bytes = B, None
-    plan.n_lig_list, plan.n_rec_list = list(rb.n_lig), list(rb.n_rec)
-    plan.N_l, plan.N_r, plan.N, plan.device = N_l, N - N_l, N, dev
-    plan.E_l, plan.E_r, plan.E = E_l, E - E_l, E
-    plan.col_src, plan.edge_dst, plan.row_ptr = col_src, edge_dst, row_ptr
-    plan.unsorted = torch.zeros((), dtype=torch.bool, device=dev)
-    plan.unsorted_i32 = torch.zeros(1, dtype=torch.int32, device=dev)
-    plan._arange = None
-    plan.he_l, plan.he_r = he, he
     seg = np.zeros(2 * B + 1, dtype=np.int64)
     seg[1:] = np.cumsum(np.asarray(list(rb.n_lig) + list(rb.n_rec), dtype=np.int64))
     tiles = [(s, n0) for s in range(2 * B) for n0 in range(int(seg[s]), int(seg[s + 1]), nat.TILE_ROWS)]
-    plan.seg_ptr_host, plan.n_node_tiles = seg, len(tiles)
     small = torch.from_numpy(np.concatenate([seg.astype(np.int32), np.asarray(tiles, dtype=np.int32).reshape(-1)])).to(dev, non_blocking=True)
-    plan.seg_ptr, plan.node_tiles, plan._small = small[:2 * B + 1], small[2 * B + 1:], small
-    gs = nat.EqdGraph()
-    gs.n_pairs, gs.n_nodes, gs.n_lig_nodes = B, N, N_l
-    gs.n_edges, gs.n_lig_edges, gs.max_in_degree = E, E, int(max_neighbor)      # n_lig_edges = E: every edge row lives in `he_lig`
-    gs.seg_ptr, gs.row_ptr = plan.seg_ptr.data_ptr(), row_ptr.data_ptr()
-    gs.col_src, gs.edge_dst = col_src.data_ptr(), edge_dst.data_ptr()
-    gs.he_lig, gs.he_rec = he.data_ptr(), he.data_ptr()
-    gs.n_node_tiles, gs.node_tiles = plan.n_node_tiles, plan.node_tiles.data_ptr()
-    plan.struct = gs
-    plan._keep = (ws, deg, d)
+    plan = GraphPlan.from_device_arrays(rb.n_lig, rb.n_rec, E_l, E, col_src, edge_dst, row_ptr, he, he, small[:2 * B + 1],
+                                        small[2 * B + 1:], seg, dev, int(max_neighbor), keep=(ws, deg, d))
+    plan._small = small
     g._eqd_plan = plan
     return g
 

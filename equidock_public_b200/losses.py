@@ -29,6 +29,19 @@ class PocketBatch:
         self.max_pocket = max(sizes) if sizes else 0
         self.pocket_ptr = torch.tensor(ptr, dtype=torch.int32, device=device)
 
+    @classmethod
+    def from_device_arrays(cls, bound_lig: torch.Tensor, bound_rec: torch.Tensor, pocket_lig: torch.Tensor,
+                           pocket_rec: torch.Tensor, pocket_ptr: torch.Tensor, pocket_sizes: Sequence[int]) -> 'PocketBatch':
+        """Over arrays already on the device in this class's layout (f32 (n,3) contiguous, ``pocket_ptr`` (B+1,) int32):
+        no copy, no sync.  ``pocket_sizes`` are the per-pair pocket sizes, known on the host."""
+        self = cls.__new__(cls)
+        self.bound_lig, self.bound_rec, self.pocket_lig, self.pocket_rec = bound_lig, bound_rec, pocket_lig, pocket_rec
+        sizes = [int(s) for s in pocket_sizes]
+        self.n_pocket_total = sum(sizes)
+        self.max_pocket = max(sizes) if sizes else 0
+        self.pocket_ptr = pocket_ptr
+        return self
+
 
 def device_losses(plan, pred_lig: torch.Tensor, keypts: torch.Tensor, tgt: PocketBatch, pocket_ot_loss_weight: float,
                   intersection_loss_weight: float, intersection_sigma: float, intersection_surface_ct: float) -> Dict:

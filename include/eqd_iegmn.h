@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define EQD_ABI_VERSION 12
+#define EQD_ABI_VERSION 13
 
 #define EQD_EDGE_FEATS 27     /* input_edge_feats_dim, protein_utils.py:71-86 + :373-389 */
 #define EQD_N_RBF 15          /* all_sigmas_dist = 1.5**s, rigid_docking_model.py:116 */
@@ -459,6 +459,77 @@ int eqd_graph_build_knn(int32_t n_prot, int32_t n_nodes, int32_t max_protein_nod
                         float* mu_r_norm, void* stream);
 int eqd_graph_build_edges(int32_t n_nodes, const int32_t* row_ptr, const int32_t* deg, const void* workspace,
                           int32_t* col_src, int32_t* edge_dst, float* he, void* stream);
+
+/* ---- training minibatches assembled on the device from a device-resident pair archive --------------------------------
+ * eqd_pair_archive: the ragged arrays of a pair archive (formats.save_pairs) in device memory, uploaded once.  Node, edge
+ * and pocket offsets per pair are int64 [n_pairs+1]; src / dst are protein-local node ids with every protein's edges
+ * grouped by ascending destination (checked by the caller when the archive is uploaded); he arrays are 16-byte aligned
+ * and readable up to the next 16-byte boundary past their end.  lig_centroid [n_pairs][3] fp64 is the mean of every
+ * ligand's `x`, derived once at upload: the centre the ligand is re-posed about.
+ * eqd_batch_out: the arrays of one batch, caller-allocated, in engine order (ligand proteins of the B pairs, then their
+ * receptor proteins; N = N_l + N_r nodes, E = E_l + E_r edges, P pocket points, T node tiles).  col_src / edge_dst are
+ * global batch node ids, row_ptr is the CSR of the whole batch, he_lig [E_l+1][27] / he_rec [E_r+1][27] the edge
+ * features of the two edge types (eqd_graph.he_lig / he_rec with n_lig_edges = E_l; each 16-byte aligned, the last row
+ * readable and not written), node_tiles the (segment, first node) tiles of eqd_graph.
+ * rot [B][9] / trans [B][3] fp64 receive the rigid motion applied to each pair's ligand (identity when re-posing is off).
+ * ---------------------------------------------------------------------------------------------------------------------- */
+typedef struct eqd_pair_archive {
+  int32_t n_pairs;
+  const int64_t* lig_node_ptr;   /* [n_pairs+1] */
+  const int64_t* rec_node_ptr;
+  const int64_t* lig_edge_ptr;   /* [n_pairs+1] */
+  const int64_t* rec_edge_ptr;
+  const int64_t* pocket_ptr;     /* [n_pairs+1] label/pocket_ptr */
+  const uint8_t* lig_res_feat;   /* [n][1] residue type 0..20 */
+  const uint8_t* rec_res_feat;
+  const float* lig_x;            /* [n][3] */
+  const float* rec_x;
+  const float* lig_mu_r_norm;    /* [n][5] */
+  const float* rec_mu_r_norm;
+  const int32_t* lig_src;        /* [e] */
+  const int32_t* lig_dst;
+  const int32_t* rec_src;
+  const int32_t* rec_dst;
+  const float* lig_he;           /* [e][27] */
+  const float* rec_he;
+  const float* lig_new_x;        /* [n][3] */
+  const float* pocket_coors;     /* [p][3] label/pocket_coors */
+  const float* bound_lig;        /* [n_lig][3] */
+  const float* bound_rec;        /* [n_rec][3] */
+  const double* lig_centroid;    /* [n_pairs][3] */
+} eqd_pair_archive;
+
+typedef struct eqd_batch_out {
+  float* res_feat;               /* [N][1] */
+  float* x;                      /* [N][3] */
+  float* new_x;                  /* [N_l][3] */
+  float* mu_r_norm;              /* [N][5] */
+  int32_t* row_ptr;              /* [N+1] */
+  int32_t* col_src;              /* [E] */
+  int32_t* edge_dst;             /* [E] */
+  float* he_lig;                 /* [E_l+1][27] */
+  float* he_rec;                 /* [E_r+1][27] */
+  int32_t* seg_ptr;              /* [2B+1] */
+  int32_t* node_tiles;           /* [T][2] */
+  int32_t* pocket_ptr;           /* [B+1] */
+  float* pocket_lig;             /* [P][3] */
+  float* pocket_rec;             /* [P][3] */
+  float* bound_lig;              /* [N_l][3] */
+  float* bound_rec;              /* [N_r][3] */
+  double* rot;                   /* [B][9] */
+  double* trans;                 /* [B][3] */
+} eqd_batch_out;
+
+/* Gathers B pairs (repeats allowed) of the archive into `out`.  `offsets` (device int32, built by the caller from the
+ * per-pair sizes it keeps on the host) = [ pair index [B] | node offsets [2B+1] | edge offsets [2B+1] | pocket offsets
+ * [B+1] | node-tile offsets [2B+1] ], per segment in engine order (pocket offsets per pair).  max_segment_edges (host
+ * value) sizes the grid.  With `repose` != 0 the ligand of batch slot b is moved by a random rigid motion drawn from
+ * Philox4x32-10 (key = seed, counter = (slot0 + b, draw, step)): R from a unit quaternion of four normals, t = a unit
+ * normal direction x U(0, translation_interval) (synthetic.random_rigid); new_x = R (x - centroid) + t and the ligand
+ * pocket points = R (pocket - centroid) + t, in fp64.  Otherwise new_x and pocket_lig are copies.  Needs no workspace. */
+int eqd_assemble_batch(const eqd_pair_archive* archive, int32_t n_batch, const int32_t* offsets, int32_t max_segment_edges,
+                       uint64_t seed, uint64_t step, int32_t slot0, float translation_interval, int32_t repose,
+                       const eqd_batch_out* out, void* stream);
 
 /* ---- batched RMSD meter (Meter_Unbound_Bound.update_rmsd, src/utils/eval.py:19-42; Kabsch src/utils/protein_utils.py:31-64) ----
  * out[b] = {complex RMSD after superimposing the predicted complex on the true one, ligand RMSD, receptor RMSD}, fp64.
