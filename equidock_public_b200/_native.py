@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # EQD_LIB_PATH: load another build of the same ABI instead (A/B runs of kernel variants, scripts/forward_ab.py)
 LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.so')
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
@@ -42,9 +42,26 @@ class EqdLayerConsts(C.Structure):
     _fields_ = [('edge', _f32 * 64 * 5), ('node', _f32 * 304), ('proj_bias', _f32 * 320)]
 
 
+class EqdDropout(C.Structure):
+    """eqd_dropout: training-mode dropout of one layer or of the keypoint head (all zero = off)."""
+    _fields_ = [('seed', C.c_uint64), ('p', _f32), ('scale', _f32), ('threshold', C.c_uint32), ('layer', _i32),
+                ('rank', _i32), ('reserved', _i32)]
+
+
+def dropout_descriptor(p: float, seed: int, layer: int, rank: int = 0) -> EqdDropout:
+    """The eqd_dropout of probability ``p`` (0 < p <= 1) for one layer (or the head, layer = n_layers) of one forward."""
+    import numpy as np
+    d = EqdDropout()
+    d.seed, d.p, d.layer, d.rank = int(seed) & 0xFFFFFFFFFFFFFFFF, float(p), int(layer), int(rank)
+    d.threshold = min(int(round(float(p) * 2.0 ** 32)), 0xFFFFFFFF)
+    d.scale = 0.0 if p >= 1.0 else float(np.float32(1.0 / (1.0 - float(p))))
+    return d
+
+
 class EqdLayer(C.Structure):
-    """eqd_layer: what the entry points take -- `dev` (device pointers + scalars, passed to kernels by value) + `consts`."""
-    _fields_ = [('dev', EqdLayerParams), ('consts', EqdLayerConsts)]
+    """eqd_layer: what the entry points take -- `dev` (device pointers + scalars, passed to kernels by value) + `consts`,
+    and `dropout` (training-mode dropout; zero = off)."""
+    _fields_ = [('dev', EqdLayerParams), ('consts', EqdLayerConsts), ('dropout', EqdDropout)]
 
 
 class EqdForwardIO(C.Structure):
@@ -113,6 +130,7 @@ PROTOTYPES = {
     'eqd_bwd_embed': (C.c_int, [_G, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_bwd_head_workspace_bytes': (C.c_size_t, [_i32, _i32, _i32]),
     'eqd_bwd_head': (C.c_int, [_G, _H] + [_vp] * 9 + [C.c_size_t] + [_vp] * 6),
+    'eqd_bwd_head_dropout': (C.c_int, [_G, _H, C.POINTER(EqdDropout)] + [_vp] * 9 + [C.c_size_t] + [_vp] * 6),
     'eqd_bwd_layer_inputs': (C.c_int, [_G, _L] + [_vp] * 5),
     'eqd_bwd_inputs': (C.c_int, [_G] + [_vp] * 11),
     'eqd_losses_workspace_bytes': (C.c_size_t, [_i32, _i32]),
@@ -129,6 +147,7 @@ PROTOTYPES = {
     'eqd_event_destroy': (None, [_vp]),
     'eqd_event_elapsed_ms': (C.c_float, [_vp, _vp]),
     'eqd_keypoints': (C.c_int, [_G, _H, _vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
+    'eqd_keypoints_dropout': (C.c_int, [_G, _H, C.POINTER(EqdDropout), _vp, _vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     'eqd_kabsch_apply': (C.c_int, [_G, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
 }
 

@@ -7,23 +7,11 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace eqd {
 
 #define BA_THREADS 256
-
-// Philox4x32-10 (Salmon et al., SC'11): counter c, key k.
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-    k.x += 0x9E3779B9u;
-    k.y += 0xBB67AE85u;
-  }
-  return c;
-}
 
 // 53-bit uniform in [0, 1) from two 32-bit words
 __device__ __forceinline__ double u01(uint32_t hi, uint32_t lo) {

@@ -13,6 +13,7 @@
 // over IN-edges, dx = (1 - eta) dx' + sum_out dx_rel - sum_in dx_rel: fixed summation order, no atomics.
 // Restated in oracle/backward_manual.py::edge_bwd / edge_gather.
 #include "bwd_common.cuh"
+#include "philox.cuh"
 
 namespace eqd {
 
@@ -37,12 +38,15 @@ struct EdgeBwdSmem {
   int src[EQD_TM], dst[EQD_TM];
 };
 
+// DROP: the forward applied dropout sites 0 / 1 of `dr` to z1 / z3; the same masks and scale enter the chain rule
+// (dz = d(dropout output) * mask * scale).
+template <bool DROP>
 __global__ void __launch_bounds__(EQD_THREADS)
 bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin, const float* __restrict__ w3lin,
                 const float* __restrict__ proj, const double* __restrict__ x_in, const float* __restrict__ daggr,
                 const double* __restrict__ dx_out, float* __restrict__ ein_out, float* __restrict__ n1_out,
                 float* __restrict__ msg_out, float* __restrict__ dz3_out, float* __restrict__ dmsg_out,
-                float* __restrict__ dz1_out, double* __restrict__ dxrel_out, float* __restrict__ vec_partial) {
+                float* __restrict__ dz1_out, double* __restrict__ dxrel_out, float* __restrict__ vec_partial, eqd_dropout dr) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   EdgeBwdSmem& s = *reinterpret_cast<EdgeBwdSmem*>(smem_raw);
   const int tid = threadIdx.x, ty = tid >> 3, tx = tid & 7;
@@ -147,6 +151,7 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
       }
     }
     gemm_nn<false>(acc, accx, s.bufE + ty * 8 * BE_LD1, BE_LD1, s.w1, 64, BE_K1, tx);
+    if (DROP) dropout_tile<false>(acc, accx, dr, 0, e0 + ty * 8, tx);
     unsigned pos_lo = 0, pos_hi = 0;
     float nrm[8][8];
 #pragma unroll
@@ -189,6 +194,18 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
     // ---- z3 = W3 msg + b3, c3 = lrelu(z3), phi; dz3 = dphi w4 lrelu'(z3); dw4 += c3 dphi ----
     acc_set_bias(acc, s.b3, tx);
     gemm_nn<false>(acc, accx, s.bufA + ty * 8 * BE_LD, BE_LD, s.w3, 64, 64, tx);
+    float keep[8][8];   // DROP: mask * scale of z3 (the same factor then carries dz3 back through the dropout)
+    if (DROP) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) keep[i][j] = 1.f;
+      dropout_tile<false>(keep, accx, dr, 1, e0 + ty * 8, tx);
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[i][j] *= keep[i][j];
+    }
     {
       float w4r[8];
 #pragma unroll
@@ -204,6 +221,7 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
           v = fmaf(c3, w4r[j], v);
           w4sum[j] = fmaf(c3, dph, w4sum[j]);
           acc[i][j] = dph * w4r[j] * lrelu_grad_from_post(c3, slope);     // dz3
+          if (DROP) acc[i][j] *= keep[i][j];
         }
         v = row_sum8(v);
         if (tx == 0) s.phi[r] = v + p.b_coor2;
@@ -264,6 +282,7 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
         acc[i][j] = rstd * (acc[i][j] - m1 - nhat[j] * m2) * (pos ? 1.f : slope);
       }
     }
+    if (DROP) dropout_tile<false>(acc, accx, dr, 0, e0 + ty * 8, tx);   // dz1 = d(dropout output) * mask * scale
     __syncthreads();   // bufA (dmsg) no longer read
     store_tile_smem<false>(s.bufA, BE_LD, acc, accx, ty, tx);
     store_tile_global(dz1_out, e0, 64, ne, acc, ty, tx);
@@ -354,10 +373,17 @@ extern "C" int eqd_bwd_edge(const eqd_graph* g, const eqd_layer* p_l, const floa
   if (n_partials_out) *n_partials_out = grid > 0 ? grid : 0;
   if (g->n_edges <= 0) return EQD_OK;
   size_t smem = sizeof(eqd::EdgeBwdSmem);
-  EQD_SET_SMEM((eqd::bwd_edge_kernel), smem);
-  eqd::bwd_edge_kernel<<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, w2lin, w3lin, proj, x_in, daggr, dx_out,
-                                                                         ein_out, n1_out, msg_out, dz3_out, dmsg_out,
-                                                                         dz1_out, dxrel_out, vec_partial);
+  if (p_l->dropout.p > 0.f) {
+    EQD_SET_SMEM((eqd::bwd_edge_kernel<true>), smem);
+    eqd::bwd_edge_kernel<true><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(
+        *g, *p, w2lin, w3lin, proj, x_in, daggr, dx_out, ein_out, n1_out, msg_out, dz3_out, dmsg_out, dz1_out, dxrel_out,
+        vec_partial, p_l->dropout);
+  } else {
+    EQD_SET_SMEM((eqd::bwd_edge_kernel<false>), smem);
+    eqd::bwd_edge_kernel<false><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(
+        *g, *p, w2lin, w3lin, proj, x_in, daggr, dx_out, ein_out, n1_out, msg_out, dz3_out, dmsg_out, dz1_out, dxrel_out,
+        vec_partial, p_l->dropout);
+  }
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }

@@ -8,6 +8,7 @@
 // operands of the weight-gradient reductions (n5 = LN output, du) plus per-CTA partials of dgamma / dbeta.
 // Restated in oracle/backward_manual.py::node_mlp_bwd.
 #include "bwd_common.cuh"
+#include "philox.cuh"
 
 namespace eqd {
 
@@ -20,14 +21,16 @@ struct NodeBwdCfg {
   static constexpr size_t SMEM = (size_t)(3 * BUF + WB + 16 * 64 + EQD_TM) * sizeof(float);
 };
 
-template <bool EXTRA>
+// DROP: the forward applied dropout site 2 of `dr` to u5; du = d(dropout output) * mask * scale.
+template <bool EXTRA, bool DROP>
 __global__ void __launch_bounds__(EQD_THREADS)
 bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w_node1_lin /*[dhp][2dhp+136]*/,
                     const float* __restrict__ w_node2_lin /*[64][dhp]*/, const float* __restrict__ h_in, int ldh,
                     const float* __restrict__ aggr, const float* __restrict__ mu, int ldmu,
                     const float* __restrict__ h0, const float* __restrict__ dh_out, float* __restrict__ dh_in,
                     float* __restrict__ daggr, float* __restrict__ dmu, float* __restrict__ dh0_acc,
-                    float* __restrict__ n5_out, float* __restrict__ du_out, float* __restrict__ vec_partial) {
+                    float* __restrict__ n5_out, float* __restrict__ du_out, float* __restrict__ vec_partial,
+                    eqd_dropout dr) {
   using C = NodeBwdCfg<EXTRA>;
   constexpr int DHP = C::DHP, LD = C::LD;
   extern __shared__ __align__(16) float smem[];
@@ -79,6 +82,7 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
       __syncthreads();
       gemm_nn_stream<EXTRA>(acc, accx, bufA + ty * 8 * LD, LD, 8, w5 + (long)(2 * DHP + 128) * DHP, DHP, DHP, wbuf, tid);
     }
+    if (DROP) dropout_tile<EXTRA>(acc, accx, dr, 2, node0 + ty * 8, tx);
     // ---------------- LeakyReLU + LayerNorm statistics; keep n-hat (smem), sign bits (registers) ----------------
     unsigned pos_lo = 0, pos_hi = 0, pos_x = 0;
     const float inv_n = 1.f / (float)p.dh;
@@ -181,6 +185,7 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
       }
       if (EXTRA) accx[i] = xvalid ? rstd * (accx[i] - m1 - nhx * m2) * (((pos_x >> i) & 1u) ? 1.f : slope) : 0.f;
     }
+    if (DROP) dropout_tile<EXTRA>(acc, accx, dr, 2, node0 + ty * 8, tx);
     __syncthreads();   // everyone is done with bufA (A operand of the W6 product)
     store_tile_smem<EXTRA>(bufA, LD, acc, accx, ty, tx);     // du: A operand of the four input-gradient products
     // du -> global (D operand of dW5 = inp^T . du, and of db5)
@@ -293,19 +298,23 @@ extern "C" int eqd_bwd_node_mlp(const eqd_graph* g, const eqd_layer* p_l, const 
   if (n_partials_out) *n_partials_out = grid > 0 ? grid : 0;
   if (g->n_nodes <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  if (extra) {
-    size_t smem = eqd::NodeBwdCfg<true>::SMEM;
-    EQD_SET_SMEM((eqd::bwd_node_mlp_kernel<true>), smem);
-    eqd::bwd_node_mlp_kernel<true><<<grid, EQD_THREADS, smem, st>>>(g->n_nodes, *p, w_node1_lin, w_node2_lin, h_in, ldh, aggr,
-                                                                   mu, ldmu, h0, dh_out, dh_in, daggr, dmu, dh0_acc, n5_out,
-                                                                   du_out, vec_partial);
+  const eqd_dropout& dr = p_l->dropout;
+#define EQD_BWD_NODE_LAUNCH(EXTRA, DROP)                                                                                 \
+  do {                                                                                                                \
+    size_t smem = eqd::NodeBwdCfg<EXTRA>::SMEM;                                                                       \
+    EQD_SET_SMEM((eqd::bwd_node_mlp_kernel<EXTRA, DROP>), smem);                                                      \
+    eqd::bwd_node_mlp_kernel<EXTRA, DROP><<<grid, EQD_THREADS, smem, st>>>(g->n_nodes, *p, w_node1_lin, w_node2_lin, h_in, \
+                                                                           ldh, aggr, mu, ldmu, h0, dh_out, dh_in, daggr, \
+                                                                           dmu, dh0_acc, n5_out, du_out, vec_partial, dr); \
+  } while (0)
+  if (dr.p > 0.f) {
+    if (extra) EQD_BWD_NODE_LAUNCH(true, true);
+    else EQD_BWD_NODE_LAUNCH(false, true);
   } else {
-    size_t smem = eqd::NodeBwdCfg<false>::SMEM;
-    EQD_SET_SMEM((eqd::bwd_node_mlp_kernel<false>), smem);
-    eqd::bwd_node_mlp_kernel<false><<<grid, EQD_THREADS, smem, st>>>(g->n_nodes, *p, w_node1_lin, w_node2_lin, h_in, ldh,
-                                                                    aggr, mu, ldmu, h0, dh_out, dh_in, daggr, dmu, dh0_acc,
-                                                                    n5_out, du_out, vec_partial);
+    if (extra) EQD_BWD_NODE_LAUNCH(true, false);
+    else EQD_BWD_NODE_LAUNCH(false, false);
   }
+#undef EQD_BWD_NODE_LAUNCH
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }

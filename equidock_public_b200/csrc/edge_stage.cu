@@ -6,6 +6,7 @@
 // by the projection stage (Psrc, Pdst(+bias)); only the 27+15 per-edge columns are a GEMM here.
 // Per-edge activations never leave the SM.
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace eqd {
 
@@ -26,10 +27,12 @@ struct EdgeSmem {
   int rp[EQD_TM + 1];
 };
 
+// DROP: training-mode dropout sites 0 (z1) and 1 (z3) of eqd_dropout `dr`, applied before their LeakyReLU.
+template <bool DROP>
 __global__ void __launch_bounds__(EQD_THREADS, 2)
 edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ proj, const double* __restrict__ x_in,
                   const double* __restrict__ x_orig, float* __restrict__ aggr, double* __restrict__ x_out,
-                  int* __restrict__ status, int tn /* destination nodes per tile */) {
+                  int* __restrict__ status, int tn /* destination nodes per tile */, eqd_dropout dr) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   EdgeSmem& s = *reinterpret_cast<EdgeSmem*>(smem_raw);
   const int tid = threadIdx.x, ty = tid >> 3, tx = tid & 7;
@@ -127,6 +130,7 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
       }
     }
     gemm_nn<false>(acc, accx, s.buf + ty * 8 * EDGE_LD1, EDGE_LD1, s.w1, 64, EDGE_K1, tx);
+    if (DROP) dropout_tile<false>(acc, accx, dr, 0, e0 + ty * 8, tx);
     lrelu_layernorm<false>(acc, accx, s.ln_g, s.ln_b, 64, p.leaky_slope, tx);  // edge_mlp.2-3
     __syncthreads();  // everyone is done reading the [he|rbf] operand
     store_tile_smem<false>(s.buf, EDGE_LD, acc, accx, ty, tx);
@@ -142,6 +146,7 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
     // ---- coors_mlp: Linear, LeakyReLU, Linear(64->1) -> phi ------------------------------------
     acc_set_bias(acc, s.b3, tx);
     gemm_nn<false>(acc, accx, s.buf + ty * 8 * EDGE_LD, EDGE_LD, s.w3, 64, 64, tx);
+    if (DROP) dropout_tile<false>(acc, accx, dr, 1, e0 + ty * 8, tx);
     {
       float w4r[8];
 #pragma unroll
@@ -194,10 +199,16 @@ extern "C" int eqd_edge_stage_ffma(const eqd_graph* g, const eqd_layer* p_l, con
   if (tn > EQD_TM) tn = EQD_TM;
   int ntiles = (g->n_nodes + tn - 1) / tn;
   size_t smem = sizeof(eqd::EdgeSmem);
-  EQD_SET_SMEM((eqd::edge_stage_kernel), smem);
   int grid = ntiles < EQD_SMS * 2 ? ntiles : EQD_SMS * 2;
-  eqd::edge_stage_kernel<<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, proj, x_in, x_orig, aggr, x_out,
-                                                                           status, tn);
+  if (p_l->dropout.p > 0.f) {
+    EQD_SET_SMEM((eqd::edge_stage_kernel<true>), smem);
+    eqd::edge_stage_kernel<true><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, proj, x_in, x_orig, aggr,
+                                                                                  x_out, status, tn, p_l->dropout);
+  } else {
+    EQD_SET_SMEM((eqd::edge_stage_kernel<false>), smem);
+    eqd::edge_stage_kernel<false><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, proj, x_in, x_orig, aggr,
+                                                                                   x_out, status, tn, p_l->dropout);
+  }
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }

@@ -467,8 +467,8 @@ extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const fl
   if ((reinterpret_cast<uintptr_t>(g->he_lig) | reinterpret_cast<uintptr_t>(g->he_rec) |
        reinterpret_cast<uintptr_t>(p->w_edge_tc)) & 15)
     return EQD_ERR_BAD_ARG;  // bulk copies need 16-byte aligned bases
-  // a node's in-edges must fit one 64-row warpgroup tile; larger bounds run on the fp32 kernel
-  if (g->max_in_degree > TC_ROWS) return eqd_edge_stage_ffma(g, p_l, proj, x_in, x_orig, aggr, x_out, status, stream);
+  // a node's in-edges must fit one 64-row warpgroup tile; larger bounds, and training-mode dropout, run on the fp32 kernel
+  if (g->max_in_degree > TC_ROWS || p_l->dropout.p > 0.f) return eqd_edge_stage_ffma(g, p_l, proj, x_in, x_orig, aggr, x_out, status, stream);
   if (g->n_nodes <= 0) return EQD_OK;
   int tn = TC_ROWS / g->max_in_degree;
   if (tn > TC_MAX_TN) tn = TC_MAX_TN;

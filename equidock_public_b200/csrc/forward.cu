@@ -137,7 +137,10 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
   if (rc) return rc;
   const eqd_layer* l0_l = layers[0];
   const eqd_layer_params* l0 = &l0_l->dev;
-  const bool tc0 = l0->dh == EQD_H0 && l0->w_proj_tc && l0->w_node_tc;
+  // training-mode dropout runs the whole stack on the fp32 CUDA-core kernels (the tensor-core node stages have no dropout)
+  bool drop = false;
+  for (int li = 0; li < n_layers; ++li) drop = drop || layers[li]->dropout.p > 0.f;
+  const bool tc0 = l0->dh == EQD_H0 && l0->w_proj_tc && l0->w_node_tc && !drop;
   if (tc0) rc = eqd_project_tc0(g, l0_l, h0, pa, kv, x5, stream);
   else rc = eqd_project(g, l0_l, h0, l0->dh == EQD_H0 ? EQD_H0_PAD : EQD_HID, pa, stream);
   if (rc) return rc;
@@ -165,13 +168,13 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
     if (rc) return rc;
     stage_event(li, 1);
     stage_event(li, 2);
-    if (lp->dh == EQD_HID && lp->w_node_tc && (!lpn || lpn->w_proj_tc)) {
+    if (lp->dh == EQD_HID && lp->w_node_tc && !drop && (!lpn || lpn->w_proj_tc)) {
       rc = eqd_node_stage_tc(g, lp_l, lpn_l, h_in, h0, pa, aggr, kv, mu, h_out, pb, stream);
     } else if (li == 0 && tc0 && (!lpn || lpn->w_proj_tc)) {
       rc = eqd_node_stage_tc0(g, lp_l, lpn_l, h0, pa, aggr, kv, x5, mu, h_out, pb, stream);
     } else {   // fp32 CUDA-core node stage (fused projections); the next layer's tensor-core attention needs K/V blocks
       rc = eqd_node_stage(g, lp_l, lpn_l, h_in, ldh, h0, pa, aggr, sb ? mu : nullptr, h_out, pb, stream);
-      if (!rc && lpn && lpn->dh == EQD_HID && lpn->w_node_tc) rc = eqd_kv_blocks(g, pb, 320, 192, 256, kv, stream);
+      if (!rc && lpn && lpn->dh == EQD_HID && lpn->w_node_tc && !drop) rc = eqd_kv_blocks(g, pb, 320, 192, 256, kv, stream);
     }
     if (rc) return rc;
     stage_event(li, 3);
@@ -180,7 +183,9 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
     ldh = EQD_HID;
     x_in = x_out;
   }
-  rc = eqd_keypoints(g, hp, h_in, x_in, w + c.head, c.head_bytes, keypts, ymean, cov, stream);
+  eqd_dropout head_drop = layers[n_layers - 1]->dropout;   // site 3: the last layer's descriptor, layer = n_layers
+  head_drop.layer = n_layers;
+  rc = eqd_keypoints_dropout(g, hp, &head_drop, h_in, x_in, w + c.head, c.head_bytes, keypts, ymean, cov, stream);
   if (rc) return rc;
   return eqd_kabsch_apply(g, cov, ymean, io->x_lig, nullptr, io->rot, io->trans, io->ligand_out, io->sing, io->status, stream);
 }

@@ -10,6 +10,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "philox.cuh"
 #include "svd3.cuh"
 
 namespace eqd {
@@ -20,8 +21,10 @@ namespace eqd {
 #define HEAD_JC 64    // nodes per staged chunk
 
 // ---- partial column sums of LeakyReLU(W_m h + b_m) over each node tile (:525, :529) -------------
+// DROP: training-mode dropout site 3 of eqd_dropout `dr` on W_m h + b_m, before the LeakyReLU.
+template <bool DROP>
 __global__ void __launch_bounds__(EQD_THREADS, 2)
-head_mean_kernel(eqd_graph g, eqd_head_params hp, const float* __restrict__ h, float* __restrict__ part) {
+head_mean_kernel(eqd_graph g, eqd_head_params hp, const float* __restrict__ h, float* __restrict__ part, eqd_dropout dr) {
   extern __shared__ __align__(16) float smem[];
   constexpr int LD = 68;
   float* A = smem;                   // [128][68]
@@ -37,6 +40,7 @@ head_mean_kernel(eqd_graph g, eqd_head_params hp, const float* __restrict__ h, f
     float acc[8][8], accx[8];
     acc_set_bias(acc, hp.b_mean, tx);
     gemm_nn_stream<false>(acc, accx, A + ty * 8 * LD, LD, EQD_HID, hp.w_mean, EQD_HID, EQD_HID, wbuf, tid);
+    if (DROP) dropout_tile<false>(acc, accx, dr, 3, node0 + ty * 8, tx);
     float colsum[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) colsum[j] = 0.f;
@@ -383,6 +387,12 @@ extern "C" int eqd_head_fold(const eqd_head_params* hp, double* m_qk, void* stre
 extern "C" int eqd_keypoints(const eqd_graph* g, const eqd_head_params* hp, const float* h, const double* x,
                              void* workspace, size_t workspace_bytes, double* keypts, double* ymean, double* cov,
                              void* stream) {
+  return eqd_keypoints_dropout(g, hp, nullptr, h, x, workspace, workspace_bytes, keypts, ymean, cov, stream);
+}
+
+extern "C" int eqd_keypoints_dropout(const eqd_graph* g, const eqd_head_params* hp, const eqd_dropout* dropout,
+                                     const float* h, const double* x, void* workspace, size_t workspace_bytes,
+                                     double* keypts, double* ymean, double* cov, void* stream) {
   if (!g || !hp || !h || !x || !workspace || !keypts || !ymean || !cov) return EQD_ERR_BAD_ARG;
   if (!hp->m_qk || (reinterpret_cast<uintptr_t>(hp->m_qk) & 15)) return EQD_ERR_BAD_ARG;   // eqd_head_fold() output
   if (workspace_bytes < eqd_workspace_bytes(g->n_nodes, g->n_node_tiles, g->n_pairs)) return EQD_ERR_WORKSPACE;
@@ -397,9 +407,15 @@ extern "C" int eqd_keypoints(const eqd_graph* g, const eqd_head_params* hp, cons
   const int nseg = 2 * g->n_pairs;
   {
     size_t smem = (size_t)(EQD_TM * 68 + 2 * EQD_WCHUNK * EQD_WLD) * sizeof(float);
-    EQD_SET_SMEM((eqd::head_mean_kernel), smem);
     int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
-    eqd::head_mean_kernel<<<grid, EQD_THREADS, smem, st>>>(*g, *hp, h, part);
+    const eqd_dropout dr = dropout ? *dropout : eqd_dropout{};
+    if (dr.p > 0.f) {
+      EQD_SET_SMEM((eqd::head_mean_kernel<true>), smem);
+      eqd::head_mean_kernel<true><<<grid, EQD_THREADS, smem, st>>>(*g, *hp, h, part, dr);
+    } else {
+      EQD_SET_SMEM((eqd::head_mean_kernel<false>), smem);
+      eqd::head_mean_kernel<false><<<grid, EQD_THREADS, smem, st>>>(*g, *hp, h, part, dr);
+    }
     EQD_CUDA_LAUNCH_CHECK();
   }
   {
@@ -725,10 +741,11 @@ __global__ void head_dqbar_kernel(int n_pairs, eqd_head_params hp, const double*
 }
 
 // warp per node: pre = W_m h + b_m; dpre = dqbar[seg] / n_seg * lrelu'(pre) -> dpre_out (D operand of dW_m);
-// dh[n] += W_m^T dpre
+// dh[n] += W_m^T dpre.  DROP: pre is replaced by its dropout output d = m * scale * pre (site 3), dpre = ... lrelu'(d) m scale.
+template <bool DROP>
 __global__ void head_mean_bwd_kernel(eqd_graph g, eqd_head_params hp, const int* __restrict__ node_seg,
                                      const float* __restrict__ h, const double* __restrict__ dqbar,
-                                     float* __restrict__ dpre_out, float* __restrict__ dh) {
+                                     float* __restrict__ dpre_out, float* __restrict__ dh, eqd_dropout dr) {
   __shared__ float hs[8][64], dp[8][64];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x * 8 + w;
@@ -743,8 +760,22 @@ __global__ void head_mean_bwd_kernel(eqd_graph g, eqd_head_params hp, const int*
     p0 = fmaf(hs[w][d], hp.w_mean[d * 64 + lane], p0);
     p1 = fmaf(hs[w][d], hp.w_mean[d * 64 + lane + 32], p1);
   }
-  const float g0 = (float)dqbar[(long)s * 64 + lane] * inv_n * (p0 > 0.f ? 1.f : hp.leaky_slope);
-  const float g1 = (float)dqbar[(long)s * 64 + lane + 32] * inv_n * (p1 > 0.f ? 1.f : hp.leaky_slope);
+  float f0 = 1.f, f1 = 1.f;
+  if (DROP) {
+    const uint4 a = dropout_words(dr, 3, n, lane >> 2), b = dropout_words(dr, 3, n, 8 + (lane >> 2));
+    const int k = lane & 3;
+    const uint32_t wa = k == 0 ? a.x : k == 1 ? a.y : k == 2 ? a.z : a.w, wb = k == 0 ? b.x : k == 1 ? b.y : k == 2 ? b.z : b.w;
+    f0 = dropout_apply(1.f, wa, dr);
+    f1 = dropout_apply(1.f, wb, dr);
+    p0 *= f0;
+    p1 *= f1;
+  }
+  float g0 = (float)dqbar[(long)s * 64 + lane] * inv_n * (p0 > 0.f ? 1.f : hp.leaky_slope);
+  float g1 = (float)dqbar[(long)s * 64 + lane + 32] * inv_n * (p1 > 0.f ? 1.f : hp.leaky_slope);
+  if (DROP) {
+    g0 *= f0;
+    g1 *= f1;
+  }
   dpre_out[(long)n * 64 + lane] = g0;
   dpre_out[(long)n * 64 + lane + 32] = g1;
   dp[w][lane] = g0;
@@ -783,6 +814,15 @@ extern "C" int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const
                             const double* cov, const float* x_lig_in, const float* dcoors, const double* dkeypts,
                             const float* drot, const float* dtrans, void* workspace, size_t workspace_bytes, float* dh,
                             double* dx, float* dpre, float* g_wkey, float* g_wquery, void* stream) {
+  return eqd_bwd_head_dropout(g, hp, nullptr, h, x, cov, x_lig_in, dcoors, dkeypts, drot, dtrans, workspace,
+                              workspace_bytes, dh, dx, dpre, g_wkey, g_wquery, stream);
+}
+
+extern "C" int eqd_bwd_head_dropout(const eqd_graph* g, const eqd_head_params* hp, const eqd_dropout* dropout,
+                                    const float* h, const double* x, const double* cov, const float* x_lig_in,
+                                    const float* dcoors, const double* dkeypts, const float* drot, const float* dtrans,
+                                    void* workspace, size_t workspace_bytes, float* dh, double* dx, float* dpre,
+                                    float* g_wkey, float* g_wquery, void* stream) {
   if (!g || !hp || !h || !x || !cov || !x_lig_in || !workspace || !dh || !dx || !dpre || !g_wkey || !g_wquery)
     return EQD_ERR_BAD_ARG;
   if (workspace_bytes < eqd_bwd_head_workspace_bytes(g->n_nodes, g->n_node_tiles, g->n_pairs)) return EQD_ERR_WORKSPACE;
@@ -805,7 +845,7 @@ extern "C" int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const
   double* a = reinterpret_cast<double*>(take(2 * B * EQD_HEADS * 64 * 8));
   double* dqbar = reinterpret_cast<double*>(take(2 * B * 64 * 8));
   // recompute qbar, u, keypoints and their means (cov_scratch is discarded: the caller's cov may carry the guard's noise)
-  int rc = eqd_keypoints(g, hp, h, x, fwd_ws, fwd_bytes, keypts, ymean, cov_scratch, stream);
+  int rc = eqd_keypoints_dropout(g, hp, dropout, h, x, fwd_ws, fwd_bytes, keypts, ymean, cov_scratch, stream);
   if (rc) return rc;
   const double* qbar = reinterpret_cast<const double*>(fwd_ws + ws_part_bytes(g->n_node_tiles) + ws_tile_ptr_bytes(g->n_pairs));
   const double* u = reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(qbar) + ws_qbar_bytes(g->n_pairs));
@@ -825,7 +865,11 @@ extern "C" int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const
   EQD_CUDA_LAUNCH_CHECK();
   eqd::head_dqbar_kernel<<<2 * g->n_pairs, 64, 0, st>>>(g->n_pairs, *hp, a, dqbar);
   EQD_CUDA_LAUNCH_CHECK();
-  eqd::head_mean_bwd_kernel<<<(unsigned)((N + 7) / 8), 256, 0, st>>>(*g, *hp, node_seg, h, dqbar, dpre, dh);
+  const eqd_dropout dr = dropout ? *dropout : eqd_dropout{};
+  if (dr.p > 0.f)
+    eqd::head_mean_bwd_kernel<true><<<(unsigned)((N + 7) / 8), 256, 0, st>>>(*g, *hp, node_seg, h, dqbar, dpre, dh, dr);
+  else
+    eqd::head_mean_bwd_kernel<false><<<(unsigned)((N + 7) / 8), 256, 0, st>>>(*g, *hp, node_seg, h, dqbar, dpre, dh, dr);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }

@@ -408,6 +408,7 @@ extern "C" int eqd_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const f
                                const float* mu, const float* h0, float* h_out, void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !h_in || !aggr || !mu || !h0 || !h_out) return EQD_ERR_BAD_ARG;
+  if (p_l->dropout.p > 0.f) return EQD_ERR_UNSUPPORTED;   // dropout runs on the fp32 node stage (eqd_node_stage)
   if (p->dh != 64 || p->dhp != 64) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
   const int products = eqd_mma_products(p);
@@ -422,6 +423,7 @@ extern "C" int eqd_node_mlp_tc0(const eqd_graph* g, const eqd_layer* p_l, const 
                                 const float* mu, float* h_out, void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !h0 || !aggr || !mu || !h_out) return EQD_ERR_BAD_ARG;
+  if (p_l->dropout.p > 0.f) return EQD_ERR_UNSUPPORTED;   // dropout runs on the fp32 node stage (eqd_node_stage)
   if (p->dh != 69 || p->dhp != 72 || !eqd_mma_products(p)) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
   if (!p->w_node_tc || (reinterpret_cast<uintptr_t>(p->w_node_tc) & 15)) return EQD_ERR_BAD_ARG;

@@ -7,6 +7,7 @@
 //   3. writes h' and, when a next layer exists, that layer's projections of h' (Psrc, Pdst, Q, K, V)
 //      so h' is never re-read from HBM for them; with mu != NULL also mu (the per-layer backward reads it).
 #include "common.cuh"
+#include "philox.cuh"
 
 namespace eqd {
 
@@ -24,12 +25,13 @@ struct NodeCfg {
   static constexpr size_t SMEM = (size_t)(2 * BUF + KVW) * sizeof(float);
 };
 
-template <bool EXTRA>
+// DROP: training-mode dropout site 2 (u5) of eqd_dropout `dr`, applied before the LeakyReLU.
+template <bool EXTRA, bool DROP>
 __global__ void __launch_bounds__(EQD_THREADS, 2)
 node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_next, const float* __restrict__ h_in,
                   int ldh, const float* __restrict__ h0, const float* __restrict__ proj,
                   const float* __restrict__ aggr, float* __restrict__ h_out, float* __restrict__ proj_next,
-                  float* __restrict__ mu_out) {
+                  float* __restrict__ mu_out, eqd_dropout dr) {
   using C = NodeCfg<EXTRA>;
   constexpr int DHP = C::DHP, LD = C::LD, KC = C::KC;
   extern __shared__ __align__(16) float smem[];
@@ -153,6 +155,7 @@ node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_
     __syncthreads();
     gemm_nn_stream<EXTRA>(acc, accx, bufB + ty * 8 * LD, LD, 8, w5 + (long)(2 * DHP + 128) * DHP, DHP, DHP, wbuf,
                           tid);
+    if (DROP) dropout_tile<EXTRA>(acc, accx, dr, 2, node0 + ty * 8, tx);
     lrelu_layernorm<EXTRA>(acc, accx, p.node_ln_g, p.node_ln_b, p.dh, p.leaky_slope, tx);
     store_tile_smem<EXTRA>(bufA, LD, acc, accx, ty, tx);
     __syncthreads();
@@ -204,19 +207,23 @@ extern "C" int eqd_node_stage(const eqd_graph* g, const eqd_layer* p_l, const eq
   eqd_layer_params pn = p_next ? *p_next : *p;
   int has_next = p_next ? 1 : 0;
   cudaStream_t st = (cudaStream_t)stream;
-  if (extra) {
-    size_t smem = eqd::NodeCfg<true>::SMEM;
-    EQD_SET_SMEM((eqd::node_stage_kernel<true>), smem);
-    int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
-    eqd::node_stage_kernel<true><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr,
-                                                                  h_out, proj_next, mu);
+  const eqd_dropout& dr = p_l->dropout;
+  const int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
+#define EQD_NODE_STAGE_LAUNCH(EXTRA, DROP)                                                                              \
+  do {                                                                                                                \
+    size_t smem = eqd::NodeCfg<EXTRA>::SMEM;                                                                          \
+    EQD_SET_SMEM((eqd::node_stage_kernel<EXTRA, DROP>), smem);                                                        \
+    eqd::node_stage_kernel<EXTRA, DROP><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr, \
+                                                                         h_out, proj_next, mu, dr);                   \
+  } while (0)
+  if (dr.p > 0.f) {
+    if (extra) EQD_NODE_STAGE_LAUNCH(true, true);
+    else EQD_NODE_STAGE_LAUNCH(false, true);
   } else {
-    size_t smem = eqd::NodeCfg<false>::SMEM;
-    EQD_SET_SMEM((eqd::node_stage_kernel<false>), smem);
-    int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
-    eqd::node_stage_kernel<false><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr,
-                                                                   h_out, proj_next, mu);
+    if (extra) EQD_NODE_STAGE_LAUNCH(true, false);
+    else EQD_NODE_STAGE_LAUNCH(false, false);
   }
+#undef EQD_NODE_STAGE_LAUNCH
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }

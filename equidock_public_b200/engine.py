@@ -70,6 +70,34 @@ _PY_FORWARD = False
 PRECISIONS = {'fp32': 0, 'bf16x3': 3}
 
 
+def draw_dropout(p: float, rank: int = 0):
+    """The dropout of one training-mode forward: (p, seed, rank) with a 64-bit seed drawn from torch's default CPU
+    generator (so ``torch.manual_seed`` reproduces the masks), or None when ``p == 0``."""
+    if not p > 0:
+        return None
+    seed = int(torch.empty((), dtype=torch.int64).random_(-2 ** 63, 2 ** 63 - 1)) & 0xFFFFFFFFFFFFFFFF
+    return float(p), seed, int(rank)
+
+
+def with_dropout(descs, dropout, first_layer: int = 0):
+    """Copies of eqd_layer descriptors with the dropout of one forward (``dropout`` = draw_dropout's tuple) set, layer
+    positions ``first_layer``, ``first_layer + 1``, ...; the descriptors themselves when ``dropout`` is None."""
+    if dropout is None:
+        return list(descs)
+    p, seed, rank = dropout
+    out = []
+    for li, d in enumerate(descs):
+        c = nat.EqdLayer.from_buffer_copy(d)
+        c.dropout = nat.dropout_descriptor(p, seed, first_layer + li, rank)
+        out.append(c)
+    return out
+
+
+def head_dropout(dropout, n_layers: int):
+    """The keypoint head's eqd_dropout for a forward over ``n_layers`` layers (layer position n_layers), or None."""
+    return None if dropout is None else nat.dropout_descriptor(dropout[0], dropout[1], n_layers, dropout[2])
+
+
 def check_precision(precision: str) -> str:
     if precision not in PRECISIONS:
         raise ValueError(f'precision must be one of {sorted(PRECISIONS)}, got {precision!r}')
@@ -496,10 +524,11 @@ class IEGMNEngine:
     def forward(self, plan: GraphPlan, emb: torch.Tensor, layers: List[PackedLayer], head: PackedHead,
                 res_l, res_r, mu_l, mu_r, x_l, x_r, check_status: bool = True, log=None,
                 stage_timer=None, record_event: bool = True, train_stash=None,
-                mma_products: int = 0) -> Dict[str, torch.Tensor]:
+                mma_products: int = 0, dropout=None) -> Dict[str, torch.Tensor]:
         """One forward = ONE call into the library (eqd_iegmn_forward): the per-stage entry points are chained in C on
         the current stream out of a single workspace allocation.  ``mma_products`` (0 or 3, see ``PRECISIONS``) goes
-        to the descriptors of the 64-wide layers."""
+        to the descriptors of the 64-wide layers.  ``dropout`` (draw_dropout's tuple, None = off) turns on training-mode
+        dropout; the descriptors it ran with are returned as ``dropout_layers`` / ``dropout_head`` for the backward."""
         with torch.cuda.device(self.device):   # the raw launches below go to the CURRENT device: make it the model's
             lib, dev = self.lib, self.device
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
@@ -530,7 +559,8 @@ class IEGMNEngine:
                 io.train_stash, io.train_stash_bytes = train_stash.data_ptr(), int(train_stash.numel())
             events = stage_timer.new_forward(len(layers)) if stage_timer is not None else None
             io.stage_events = C.cast(events, C.c_void_p) if events is not None else None
-            larr = (C.POINTER(nat.EqdLayer) * len(layers))(*[C.pointer(l.descriptor(mma_products)) for l in layers])
+            descs = with_dropout([l.descriptor(mma_products) for l in layers], dropout)
+            larr = (C.POINTER(nat.EqdLayer) * len(layers))(*[C.pointer(d) for d in descs])
             nat.check(lib.eqd_iegmn_forward(g, larr, len(layers), C.byref(head.struct), C.byref(io), nat.ptr(ws),
                                             plan.forward_ws_bytes, st), 'eqd_iegmn_forward')
             kab = lambda mask: nat.check(lib.eqd_kabsch_apply(
@@ -547,6 +577,8 @@ class IEGMNEngine:
             out = {'status_lease': lease, 'ligand_coors': lig_out, 'keypts': keyp, 'rotation': rot,
                    'translation': trans, 'h': h_fin, 'x64': x_fin, 'cov': cov, 'sing': sing, 'status': status,
                    'unsorted': plan.unsorted, 'kabsch': kab, 'status_host': status_host, 'status_event': status_event, '_keep': (ws, ymean, x_l)}
+            if dropout is not None:
+                out.update(dropout_layers=descs, dropout_head=head_dropout(dropout, len(layers)))
             if check_status:
                 self.resolve_status(plan, out, kab, log)
             return out

@@ -184,7 +184,7 @@ class ResidueGraphedForward:
     graph (k-NN edges, 27 edge features, surface features) never exists on the host."""
 
     def __init__(self, model, rb: ResidueBatch, device, cutoff: float = 30.0, max_neighbor: int = 10):
-        from .graphed import GraphedForward
+        from .graphed import GraphedForward, refuse_dropout_capture
         self.model, self.device = model, torch.device(device)
         self.cutoff, self.max_neighbor = cutoff, max_neighbor
         self.buffers = GraphBuffers(rb, device, max_neighbor)
@@ -196,6 +196,7 @@ class ResidueGraphedForward:
         class _Captured(GraphedForward):
             def _capture(self_inner):
                 # identical to GraphedForward._capture, with the graph build recorded in front of the forward
+                refuse_dropout_capture(self_inner.iegmn)
                 with torch.cuda.device(self_inner.device):
                     cur = torch.cuda.current_stream(self_inner.device)
                     self_inner.stream.wait_stream(cur)

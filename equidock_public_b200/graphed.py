@@ -26,6 +26,15 @@ import torch
 from . import _native as nat
 
 
+def refuse_dropout_capture(iegmn):
+    """A captured graph replays the kernel parameters of its capture, dropout seed included: every replay would apply the
+    same masks.  Capture therefore refuses a model in training mode with dropout > 0 (launch() re-captures, and so
+    refuses, when the model is switched to training mode after capture)."""
+    if iegmn.training and iegmn.iegmn_layers[0].dropout_p > 0:
+        raise NotImplementedError('CUDA-graph capture of a training-mode forward with dropout > 0 would replay one '
+                                  'set of dropout masks: call model.eval(), or run the model eagerly')
+
+
 class GraphedForward:
     def __init__(self, model, device_batch):
         self.model, self.batch = model, device_batch
@@ -40,9 +49,11 @@ class GraphedForward:
         self._capture()
 
     def _param_key(self):
-        return tuple((p.data_ptr(), p._version) for p in self.model.parameters()) + (self.iegmn.precision,)
+        return tuple((p.data_ptr(), p._version) for p in self.model.parameters()) + (self.iegmn.precision,
+                                                                                     self.iegmn.training)
 
     def _capture(self):
+        refuse_dropout_capture(self.iegmn)
         with torch.cuda.device(self.device):
             cur = torch.cuda.current_stream(self.device)
             self.stream.wait_stream(cur)

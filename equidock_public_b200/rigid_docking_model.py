@@ -17,7 +17,9 @@ checkpoints load with ``strict=True``.  The graph argument may be a batched DGL 
 
 Scope of this engine: forward AND backward of the configuration the shipped checkpoints use
 (``nonlin='lkyrelu'``, ``layer_norm='LN'``, ``layer_norm_coors='0'``, ``final_h_layer_norm='0'``,
-``cross_msgs``, ``use_dist_in_layers``, ``rot_model='kb_att'``, ``fine_tune=False``, dropout inactive).
+``cross_msgs``, ``use_dist_in_layers``, ``rot_model='kb_att'``, ``fine_tune=False``).  ``dropout > 0`` is applied in
+training mode, as ``nn.Dropout`` does, with masks from a counter-based generator seeded per forward from torch's default
+CPU generator (``engine.draw_dropout``): same distribution as torch's, a different random stream.
 Anything else raises ``NotImplementedError``; a missing CUDA library raises -- there is no CPU path.
 In training mode (``model.train()`` with grad enabled), and in any mode when one of the graph's ``new_x`` / ``x`` /
 ``mu_r_norm`` / ``he`` requires grad, the outputs of ``Rigid_Body_Docking_Net.forward`` are autograd-connected: the whole
@@ -41,7 +43,8 @@ except ImportError:  # DGL-free deployments use the package's own container
     fn = None
 
 from . import _native as nat
-from .engine import PRECISIONS, GraphPlan, IEGMNEngine, PackedHead, PackedLayer, UnsortedEdges, _sorted_copy, check_precision
+from .engine import (PRECISIONS, GraphPlan, IEGMNEngine, PackedHead, PackedLayer, UnsortedEdges, _sorted_copy, check_precision,
+                     draw_dropout, with_dropout)
 from .hetero_graph import LIGAND, LL, RECEPTOR, RR
 
 
@@ -246,9 +249,10 @@ class IEGMN_Layer(nn.Module):
             self._packed_key = key
         return self._packed
 
-    def _check_mode(self):
-        if self.training and self.dropout_p > 0:
-            raise NotImplementedError('dropout > 0 in training mode is not implemented in the CUDA engine')
+    def dropout_now(self, rank: int = 0):
+        """The dropout of one call of this layer (or of a stack it leads): engine.draw_dropout's (p, seed, rank) in
+        training mode with dropout > 0, else None (no draw from the generator)."""
+        return draw_dropout(self.dropout_p, rank) if self.training else None
 
     def forward(self, hetero_graph, coors_ligand, h_feats_ligand, original_ligand_node_features,
                 original_edge_feats_ligand, orig_coors_ligand, coors_receptor, h_feats_receptor,
@@ -259,7 +263,6 @@ class IEGMN_Layer(nn.Module):
         per-layer backward (``training.layer_backward``): gradients reach the layer's parameters and all ten tensor
         inputs."""
         import ctypes as C
-        self._check_mode()
         inputs = (coors_ligand, h_feats_ligand, original_ligand_node_features, original_edge_feats_ligand,
                   orig_coors_ligand, coors_receptor, h_feats_receptor, original_receptor_node_features,
                   original_edge_feats_receptor, orig_coors_receptor)
@@ -286,7 +289,8 @@ class IEGMN_Layer(nn.Module):
         x_out = torch.empty(N, 3, **f64)
         status = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
         st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        g, lp = C.byref(plan.struct), C.byref(lay.struct)
+        desc = with_dropout([lay.struct], self.dropout_now())[0]   # each call is its own forward: own seed, layer 0
+        g, lp = C.byref(plan.struct), C.byref(desc)
         nat.check(eng.lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
         nat.check(eng.lib.eqd_iegmn_layer_forward(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
                                                   nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), None,
@@ -385,14 +389,14 @@ class IEGMN(nn.Module):
             self._head_key = key
         return self._head
 
-    def run_engine(self, batch_hetero_graph, check_status=True, record_event=True):
+    def run_engine(self, batch_hetero_graph, check_status=True, record_event=True, dropout='draw'):
         """The whole hot path on the device; returns the engine's raw output dict.  With ``check_status=False`` the
         per-pair status words are left pending (``resolve(out)`` finishes the call).  ``record_event=False`` is for
-        CUDA-graph capture (``graphed.GraphedForward``), which records its own completion event per replay."""
+        CUDA-graph capture (``graphed.GraphedForward``), which records its own completion event per replay.
+        ``dropout``: 'draw' = draw this forward's dropout in training mode (engine.draw_dropout), else the tuple of a
+        forward being re-run."""
         emb = self.residue_emb_layer.weight
         dev = emb.device
-        for lay in self.iegmn_layers:
-            lay._check_mode()
         eng = IEGMNEngine(dev)
         layers = [lay.packed(dev) for lay in self.iegmn_layers]
         head = self.packed_head(dev)
@@ -400,15 +404,17 @@ class IEGMN(nn.Module):
         plan = _plan_for(batch_hetero_graph, dev, self.graph_max_neighbor)
         emb32 = emb.detach().to(torch.float32).contiguous()
         products = PRECISIONS[self.precision]
+        if isinstance(dropout, str):
+            dropout = self.iegmn_layers[0].dropout_now() if self.training else None
         call = lambda p, chk: eng.forward(p, emb32, layers, head, nl['res_feat'], nr['res_feat'], nl['mu_r_norm'],
                                           nr['mu_r_norm'], nl['new_x'], nr['x'], chk, self.log,
-                                          record_event=record_event, mma_products=products)
+                                          record_event=record_event, mma_products=products, dropout=dropout)
         try:
             out = call(plan, check_status)
         except UnsortedEdges:
             plan = _sorted_plan(batch_hetero_graph, dev, self.graph_max_neighbor)
             out = call(plan, True)
-        out['plan'], out['engine'], out['graph'] = plan, eng, batch_hetero_graph
+        out['plan'], out['engine'], out['graph'], out['dropout'] = plan, eng, batch_hetero_graph, dropout
         return out
 
     def resolve(self, out):
@@ -417,8 +423,8 @@ class IEGMN(nn.Module):
         try:
             out['engine'].resolve_status(out['plan'], out, out['kabsch'], self.log)
             return out
-        except UnsortedEdges:
-            return self.run_engine(out['graph'], True)
+        except UnsortedEdges:     # re-run sorted: the same forward, so the same dropout seed
+            return self.run_engine(out['graph'], True, dropout=out['dropout'])
 
     def forward(self, batch_hetero_graph, epoch):
         """Returns ``[T list, b list, Y_ligand list, Y_receptor list]`` like the reference (:602) and

@@ -21,7 +21,7 @@ import numpy as np
 import torch
 
 from . import _native as nat
-from .engine import GraphPlan, IEGMNEngine, PackedHead, PackedLayer, _StatusLease, _upload_blob, _host_f32
+from .engine import GraphPlan, IEGMNEngine, PackedHead, PackedLayer, _StatusLease, _upload_blob, _host_f32, with_dropout
 
 _f32 = torch.float32
 
@@ -218,7 +218,7 @@ def _reduce(lib, src_t, nch, stride, mp, flat, st):
 
 
 def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack, ws: BackwardWorkspace, h_in, x_in, aggr,
-                   mu, h0, dh_out, dx_out, dh_in, dx_in, flat, st, dhe=None, dx_orig=None, capture=None, li=None):
+                   mu, h0, dh_out, dx_out, dh_in, dx_in, flat, st, dhe=None, dx_orig=None, capture=None, li=None, desc=None):
     """Backward of ONE IEGMN_Layer, the fixed kernel sequence eqd_project (recompute) -> eqd_bwd_node_mlp ->
     eqd_bwd_attention -> eqd_bwd_edge -> (eqd_bwd_layer_inputs) -> eqd_bwd_edge_gather -> eqd_bwd_project, with the weight
     gradients of each stage through eqd_tn_gemm + eqd_grad_reduce.
@@ -228,11 +228,12 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
     and dx_out [N][3] f64 of the layer's output features and coordinates.  Writes dh_in [N][dhp] and dx_in [N][3] f64
     (overwritten), adds the gradient w.r.t. h0 into ws.dh0 and the parameter gradients into `flat` (through the index maps
     of `tp`).  With dhe [E][27] f32 / dx_orig [N][3] f64 given, it also adds the gradients w.r.t. the edge features and the
-    original coordinates there (eqd_bwd_layer_inputs); without them that kernel is not launched.
+    original coordinates there (eqd_bwd_layer_inputs); without them that kernel is not launched.  ``desc`` is the eqd_layer
+    the forward ran with when it differs from ``lp_obj.struct`` (training-mode dropout: the backward replays its masks).
     Returns (dh_in, dx_in, ws.dh0, dhe, dx_orig)."""
     g = C.byref(plan.struct)
     N, E = plan.N, plan.E
-    lp = C.byref(lp_obj.struct)
+    lp = C.byref(desc if desc is not None else lp_obj.struct)
     dh, dhp, pw = tp.dh, tp.dhp, tp.pw
     ldh = nat.H0_PAD if dh == nat.H0 else nat.HID
     ldmu = nat.H0_PAD if dh == nat.H0 else nat.HID
@@ -306,6 +307,7 @@ class TrainEngine:
         self._maps: Dict[int, dict] = {}
         self._ws: Optional[BackwardWorkspace] = None
         self._head_maps = None
+        self.rank = 0        # data-parallel rank: an input of the dropout masks (DataParallelTrainer sets it)
 
     # ---- packs ----------------------------------------------------------------------------------------------------
     def layer_pack(self, lay_module) -> LayerTrainPack:
@@ -334,15 +336,14 @@ class TrainEngine:
     def forward(self, graph, log=None):
         from .rigid_docking_model import _plan_for, _sorted_plan, UnsortedEdges
         iegmn, dev, lib = self.iegmn, self.device, self.lib
-        for lay in iegmn.iegmn_layers:
-            lay._check_mode()
         plan = _plan_for(graph, dev, iegmn.graph_max_neighbor)
+        dropout = iegmn.iegmn_layers[0].dropout_now(self.rank) if iegmn.training else None
         try:
-            return self._forward_plan(graph, plan, log)
+            return self._forward_plan(graph, plan, log, dropout)
         except UnsortedEdges:
-            return self._forward_plan(graph, _sorted_plan(graph, dev, iegmn.graph_max_neighbor), log)
+            return self._forward_plan(graph, _sorted_plan(graph, dev, iegmn.graph_max_neighbor), log, dropout)
 
-    def _forward_plan(self, graph, plan, log):
+    def _forward_plan(self, graph, plan, log, dropout=None):
         from .hetero_graph import LIGAND, RECEPTOR
         iegmn, dev, lib = self.iegmn, self.device, self.lib
         layers = [lay.packed(dev) for lay in iegmn.iegmn_layers]
@@ -358,7 +359,7 @@ class TrainEngine:
             eng = IEGMNEngine(dev)
             emb32 = iegmn.residue_emb_layer.weight.detach().to(_f32).contiguous()
             out = eng.forward(plan, emb32, layers, head, nl['res_feat'], nr['res_feat'], nl['mu_r_norm'], nr['mu_r_norm'],
-                              nl['new_x'], nr['x'], True, log, train_stash=stash)
+                              nl['new_x'], nr['x'], True, log, train_stash=stash, dropout=dropout)
         out.update(plan=plan, engine=eng, graph=graph, stash=stash, stash_offsets=list(offs), layers=layers, head=head,
                    res_l=nl['res_feat'].to(_f32).contiguous(), res_r=nr['res_feat'].to(_f32).contiguous(),
                    x_lig_in=nl['new_x'].to(_f32).contiguous())
@@ -406,11 +407,13 @@ class TrainEngine:
             gq = flat[off['iegmn_original.att_mlp_query_ROT.0.weight']:]
             dh_cur, dh_nxt = ws.dh
             dx_cur, dx_nxt = ws.dx
-            nat.check(lib.eqd_bwd_head(g, C.byref(fwd['head'].struct), nat.ptr(fwd['h']), nat.ptr(fwd['x64']),
+            hd = fwd.get('dropout_head')
+            nat.check(lib.eqd_bwd_head_dropout(g, C.byref(fwd['head'].struct), C.byref(hd) if hd is not None else None,
+                                       nat.ptr(fwd['h']), nat.ptr(fwd['x64']),
                                        nat.ptr(fwd['cov']), nat.ptr(fwd['x_lig_in']), nat.ptr(d_coors), nat.ptr(d_keypts),
                                        nat.ptr(d_rot), nat.ptr(d_trans), nat.ptr(ws.head_ws), ws.head_ws_bytes,
                                        nat.ptr(dh_cur), nat.ptr(dx_cur), nat.ptr(ws.dpre), nat.ptr(gk), nat.ptr(gq), st),
-                      'eqd_bwd_head')
+                      'eqd_bwd_head_dropout')
             # eqd_bwd_head overwrote dh / dx: add the gradients that reach the last layer's outputs directly
             if d_x_out is not None:
                 dx_cur.add_(d_x_out.detach().to(device=dev, dtype=torch.float64))
@@ -443,8 +446,10 @@ class TrainEngine:
                 h_in = h0_ptr if li == 0 else sp(so[3] + li * so[4])
                 x_in = sp(so[1] + li * so[2])
                 aggr, mu = sp(so[5] + li * so[6]), sp(so[7] + li * so[8])
+                descs = fwd.get('dropout_layers')
                 layer_backward(lib, plan, fwd['layers'][li], self.layer_pack(lm), ws, h_in, x_in, aggr, mu, h0_ptr,
-                               dh_cur, dx_cur, dh_nxt, dx_nxt, flat, st, dhe, dx_orig, capture, li)
+                               dh_cur, dx_cur, dh_nxt, dx_nxt, flat, st, dhe, dx_orig, capture, li,
+                               desc=descs[li] if descs is not None else None)
                 dh_cur, dh_nxt = dh_nxt, dh_cur
                 dx_cur, dx_nxt = dx_nxt, dx_cur
                 if on_bucket_done and first_use[id(lm)] == li:   # a shared module completes at its FIRST use
@@ -590,9 +595,10 @@ class _LayerFn(torch.autograd.Function):
         aggr, mu, h_out = torch.empty(N, nat.HID, **f32), torch.empty(N, dhp, **f32), torch.empty(N, nat.HID, **f32)
         x_out = torch.empty(N, 3, **f64)
         status = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
+        desc = with_dropout([lay.struct], module.dropout_now())[0]   # each call is its own forward: own seed, layer 0
         with torch.cuda.device(dev):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            g, lp = C.byref(plan.struct), C.byref(lay.struct)
+            g, lp = C.byref(plan.struct), C.byref(desc)
             nat.check(lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
             nat.check(lib.eqd_iegmn_layer_forward(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
                                                   nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(mu),
@@ -600,14 +606,14 @@ class _LayerFn(torch.autograd.Function):
                       'eqd_iegmn_layer_forward')
         if int(status[plan.n_pairs].item()) & nat.STATUS_DEGREE_OVERFLOW:
             raise nat.NativeLibraryError(f'IEGMN_Layer.forward: in-degree above {plan.struct.max_in_degree}')
-        ctx.saved = (plan, lay, layout, tp, h, h0, x_in, aggr, mu)
+        ctx.saved = (plan, lay, layout, tp, h, h0, x_in, aggr, mu, desc)
         ctx.input_meta = [(t.dtype, t.device) for t in (x_l, h_l, h0_l, he_l, xo_l, x_r, h_r, h0_r, he_r, xo_r)]
         ctx.set_materialize_grads(False)    # a loss on only one of the two outputs launches nothing for the other
         return x_out, h_out
 
     @staticmethod
     def backward(ctx, d_x, d_h):
-        plan, lay, layout, tp, h, h0, x_in, aggr, mu = ctx.saved
+        plan, lay, layout, tp, h, h0, x_in, aggr, mu, desc = ctx.saved
         n_in = len(ctx.input_meta)
         if d_x is None and d_h is None:
             return (None,) * (1 + n_in + len(layout.params))
@@ -635,7 +641,7 @@ class _LayerFn(torch.autograd.Function):
             flat = torch.zeros(layout.total, dtype=_f32, device=dev)
             ws.dh0.zero_()
             layer_backward(lib, plan, lay, tp, ws, h, x_in, aggr, mu, h0, dh_out, dx_out, dh_in, dx_in, flat, st, dhe,
-                           dx_orig)
+                           dx_orig, desc=desc)
             dh0 = ws.dh0[:, :nat.H0].clone() if need[2] or need[7] else None
             if dhe is not None:
                 dhe_l, dhe_r = dhe[:E_l], dhe[E_l:E]
@@ -712,6 +718,9 @@ class DataParallelTrainer:
         self.loss_args = (pocket_ot_loss_weight, intersection_loss_weight, intersection_sigma, intersection_surface_ct)
         self.steps = 0
         self.comm = torch.cuda.Stream(dev) if self.world > 1 else None
+        if self.world > 1:
+            import torch.distributed as dist
+            self.engine.rank = dist.get_rank(group)
         self.lib = nat.load()
 
     def invalidate_packed(self):

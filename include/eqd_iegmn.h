@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define EQD_ABI_VERSION 13
+#define EQD_ABI_VERSION 14
 
 #define EQD_EDGE_FEATS 27     /* input_edge_feats_dim, protein_utils.py:71-86 + :373-389 */
 #define EQD_N_RBF 15          /* all_sigmas_dist = 1.5**s, rigid_docking_model.py:116 */
@@ -146,12 +146,37 @@ typedef struct eqd_layer_consts {
   float proj_bias[320];
 } eqd_layer_consts;
 
+/* Training-mode dropout (nn.Dropout(p) of the reference's IEGMN_Layer and keypoint head), host VALUES.  All zero = off,
+ * which is what every inference descriptor holds.  Four sites, each applied to a Linear output before its LeakyReLU:
+ *   site 0  edge_mlp.1          z1 = edge_mlp.0 output        row = global edge id (destination-sorted), col < 64
+ *   site 1  coors_mlp.1         z3 = coors_mlp.0 output       row = global edge id, col < 64
+ *   site 2  node_mlp.1          u5 = node_mlp.0 output        row = global node id, col < dh (69 in layer 0, else 64)
+ *   site 3  mlp_h_mean_ROT.1    W_m h + b_m of the head       row = global node id, col < 64  (layer = n_layers)
+ * Element (row, col) of a site is kept iff
+ *   philox4x32_10(counter = (row, col >> 2, (layer << 2) | site, rank), key = (lo32(seed), hi32(seed)))[col & 3] >= threshold
+ * and a kept element becomes z * scale, a dropped one 0.  threshold = round(p * 2^32) (at most 2^32 - 1), scale =
+ * float32(1 / (1 - p)), and scale = 0 for p = 1 (nothing kept).  Each element is kept independently with probability
+ * 1 - p up to a quantisation of 2^-32; the backward entry points replay the same masks from the same descriptor.    */
+typedef struct eqd_dropout {
+  uint64_t seed;
+  float p;                    /* 0 = off */
+  float scale;
+  uint32_t threshold;
+  int32_t layer;              /* position in the stack 0..L-1 (layers that share weights still differ) */
+  int32_t rank;               /* data-parallel rank, or 0 */
+  int32_t reserved;           /* 0 */
+} eqd_dropout;
+
 /* One IEGMN layer as the entry points take it: a HOST-resident descriptor.  `dev` holds device pointers and scalars only
  * and is what kernels receive by value (a binding may keep or upload it wholesale); `consts` holds host VALUES.  Entry
- * points of the fp32 FFMA path and of the backward read `dev` only.                                                 */
+ * points of the fp32 FFMA path and of the backward read `dev` only, plus `dropout` (sites 0-2) where it is on.
+ * Dropout runs on the fp32 CUDA-core kernels: eqd_edge_stage routes a layer with dropout on to eqd_edge_stage_ffma,
+ * eqd_iegmn_forward runs its node stage with eqd_node_stage, and the tensor-core node-stage entry points refuse it
+ * (EQD_ERR_UNSUPPORTED).                                                                                            */
 typedef struct eqd_layer {
   eqd_layer_params dev;
   eqd_layer_consts consts;
+  eqd_dropout dropout;
 } eqd_layer;
 
 /* ---- keypoint read-out parameters (IEGMN.__init__ :427-438), reference layouts ------------- */
@@ -287,6 +312,11 @@ int eqd_head_fold(const eqd_head_params* hp, double* m_qk /*[50][64][64]*/, void
 int eqd_keypoints(const eqd_graph* g, const eqd_head_params* hp, const float* h /*[n][64]*/,
                   const double* x /*[n][3] last-layer coords*/, void* workspace, size_t workspace_bytes,
                   double* keypts, double* ymean, double* cov, void* stream);
+/* The same with dropout site 3 (see eqd_dropout; NULL or p == 0 = eqd_keypoints).  eqd_iegmn_forward uses the last
+ * layer's dropout descriptor with layer = n_layers.                                                                   */
+int eqd_keypoints_dropout(const eqd_graph* g, const eqd_head_params* hp, const eqd_dropout* dropout, const float* h,
+                          const double* x, void* workspace, size_t workspace_bytes, double* keypts, double* ymean,
+                          double* cov, void* stream);
 
 /* Kabsch + rigid transform (:571-589, 657-665): SVD of cov, guard test, T = U diag(1,1,sign det A) V^T,
  * b = ymean_rec - T ymean_lig; ligand_out[n] = T new_x[n] + b for every ligand node.
@@ -405,6 +435,12 @@ int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const float* h, 
                  const float* x_lig_in, const float* dcoors, const double* dkeypts, const float* drot,
                  const float* dtrans, void* workspace, size_t workspace_bytes, float* dh, double* dx, float* dpre,
                  float* g_wkey, float* g_wquery, void* stream);
+/* The same for a forward that ran eqd_keypoints_dropout with `dropout` (replays its site-3 mask; NULL = eqd_bwd_head). */
+int eqd_bwd_head_dropout(const eqd_graph* g, const eqd_head_params* hp, const eqd_dropout* dropout, const float* h,
+                         const double* x, const double* cov, const float* x_lig_in, const float* dcoors,
+                         const double* dkeypts, const float* drot, const float* dtrans, void* workspace,
+                         size_t workspace_bytes, float* dh, double* dx, float* dpre, float* g_wkey, float* g_wquery,
+                         void* stream);
 
 /* ---- gradients w.r.t. the graph's input tensors (optional: the parameter gradients neither need nor change them) ----
  * eqd_bwd_layer_inputs, once per layer right after eqd_bwd_edge (any layer order; each output element is accumulated by
