@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import sys
+import threading
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -269,61 +270,73 @@ def _aligned_he(he, device):
     return own
 
 
+def node_tiles_for(n_lig: Sequence[int], n_rec: Sequence[int], device):
+    """Segment offsets and node tiles of a batch whose proteins (ligand proteins of all pairs, then receptor proteins)
+    have ``n_lig`` / ``n_rec`` nodes: (seg_ptr_host int64 [2B+1], seg_ptr int32 [2B+1], node_tiles int32 [T][2] flat =
+    (segment, first node) of every TILE_ROWS-row tile).  The two device arrays are views of ONE small upload."""
+    seg = np.zeros(len(n_lig) + len(n_rec) + 1, dtype=np.int64)
+    seg[1:] = np.cumsum(np.asarray(list(n_lig) + list(n_rec), dtype=np.int64))
+    tiles = [(s, n0) for s in range(len(seg) - 1) for n0 in range(int(seg[s]), int(seg[s + 1]), nat.TILE_ROWS)]
+    small = torch.from_numpy(np.concatenate([seg.astype(np.int32), np.asarray(tiles, dtype=np.int32).reshape(-1)]))
+    small = small.to(device, non_blocking=True)
+    return seg, small[:len(seg)], small[len(seg):]
+
+
 class GraphPlan:
     """Batch topology in the engine's layout (see the numbering comment in eqd_iegmn.h)."""
 
     def __init__(self, n_lig: Sequence[int], n_rec: Sequence[int], src_l, dst_l, src_r, dst_r, he_l, he_r,
                  device, max_in_degree: int = 10):
-        n_lig = [int(v) for v in n_lig]
-        n_rec = [int(v) for v in n_rec]
         assert len(n_lig) == len(n_rec) and len(n_lig) > 0
-        self.n_pairs = len(n_lig)
-        self.forward_ws_bytes = None   # eqd_forward_workspace_bytes(), filled on first use
-        self.n_lig_list, self.n_rec_list = n_lig, n_rec
-        self.N_l, self.N_r = sum(n_lig), sum(n_rec)
-        self.N = self.N_l + self.N_r
-        self.device = device
+        N_l = sum(int(v) for v in n_lig)
+        N = N_l + sum(int(v) for v in n_rec)
         i32 = dict(dtype=torch.int32, device=device)
         src_l, dst_l = src_l.to(**i32), dst_l.to(**i32)
         src_r, dst_r = src_r.to(**i32), dst_r.to(**i32)
-        self.E_l, self.E_r = int(src_l.shape[0]), int(src_r.shape[0])
-        self.E = self.E_l + self.E_r
-        self.col_src = torch.cat([src_l, src_r + self.N_l]).contiguous()
-        self.edge_dst = torch.cat([dst_l, dst_r + self.N_l]).contiguous()
+        E_l, E = int(src_l.shape[0]), int(src_l.shape[0]) + int(src_r.shape[0])
+        col_src = torch.cat([src_l, src_r + N_l]).contiguous()
+        edge_dst = torch.cat([dst_l, dst_r + N_l]).contiguous()
         # CSR by destination; the kernels assume edges arrive grouped by ascending destination
         # (protein_utils.py:339-346 emits them that way).  `unsorted` stays on the device and is
         # read together with the per-pair status (one sync per forward).
-        d64 = self.edge_dst.long()
-        self.unsorted = ((d64[1:] < d64[:-1]).any() if self.E > 1 else torch.zeros((), dtype=torch.bool, device=device))
-        self.unsorted_i32 = self.unsorted.to(torch.int32).reshape(1)
-        self._arange = None
+        d64 = edge_dst.long()
+        unsorted = (d64[1:] < d64[:-1]).any() if E > 1 else None
         # row_ptr[n] = first edge whose destination is >= n.  searchsorted on the (sorted) destination list needs no
         # host sync -- torch.bincount would block the CPU on the previous batch and break the copy/compute overlap.
-        self.row_ptr = torch.searchsorted(self.edge_dst, torch.arange(self.N + 1, **i32), out_int32=True).contiguous()
-        self.he_l, self.he_r = _aligned_he(he_l, device), _aligned_he(he_r, device)
-        assert self.he_l.shape == (self.E_l, nat.EDGE_FEATS) and self.he_r.shape == (self.E_r, nat.EDGE_FEATS)
-        self.edge_perm = None   # (ligand, receptor) caller edge ids of a plan built from a sorted copy (_sorted_copy)
-        seg = np.zeros(2 * self.n_pairs + 1, dtype=np.int64)
-        seg[1:] = np.cumsum(np.asarray(n_lig + n_rec, dtype=np.int64))
-        tiles = []
-        for s in range(2 * self.n_pairs):
-            for n0 in range(int(seg[s]), int(seg[s + 1]), nat.TILE_ROWS):
-                tiles.append((s, n0))
-        self.seg_ptr_host = seg
-        self.n_node_tiles = len(tiles)
-        small = torch.from_numpy(np.concatenate([seg.astype(np.int32),
-                                                 np.asarray(tiles, dtype=np.int32).reshape(-1)]))
-        small = small.to(device, non_blocking=True)
-        self.seg_ptr = small[:2 * self.n_pairs + 1]
-        self.node_tiles = small[2 * self.n_pairs + 1:]
-        self._small = small
+        row_ptr = torch.searchsorted(edge_dst, torch.arange(N + 1, **i32), out_int32=True).contiguous()
+        he_l, he_r = _aligned_he(he_l, device), _aligned_he(he_r, device)
+        assert he_l.shape == (E_l, nat.EDGE_FEATS) and he_r.shape == (E - E_l, nat.EDGE_FEATS)
+        self._finish(n_lig, n_rec, E_l, E, E_l, col_src, edge_dst, row_ptr, he_l, he_r, *node_tiles_for(n_lig, n_rec, device),
+                     device, max_in_degree, unsorted)
+
+    def _finish(self, n_lig, n_rec, E_l, E, n_lig_edges, col_src, edge_dst, row_ptr, he_l, he_r, seg_ptr_host, seg_ptr,
+                node_tiles, device, max_in_degree, unsorted=None, keep=()):
+        """Sets the size attributes and fills the eqd_graph descriptor from topology arrays in the engine's layout.
+        ``n_lig_edges`` is the number of edges whose features are rows of ``he_l`` (the rest are rows of ``he_r``);
+        ``unsorted`` = None: the edges are known to be grouped by destination."""
+        self.n_pairs = len(n_lig)
+        self.forward_ws_bytes = None   # eqd_forward_workspace_bytes(), filled on first use
+        self.n_lig_list, self.n_rec_list = [int(v) for v in n_lig], [int(v) for v in n_rec]
+        self.N_l, self.N_r = sum(self.n_lig_list), sum(self.n_rec_list)
+        self.N = self.N_l + self.N_r
+        self.device = device
+        self.E_l, self.E_r, self.E = int(E_l), int(E) - int(E_l), int(E)
+        self.col_src, self.edge_dst, self.row_ptr = col_src, edge_dst, row_ptr
+        self.unsorted = unsorted if unsorted is not None else torch.zeros((), dtype=torch.bool, device=device)
+        self.unsorted_i32 = self.unsorted.to(torch.int32).reshape(1)
+        self._arange = None
+        self.he_l, self.he_r = he_l, he_r
+        self.edge_perm = None   # (ligand, receptor) caller edge ids of a plan built from a sorted copy (from_graph)
+        self.seg_ptr_host, self.seg_ptr, self.node_tiles = seg_ptr_host, seg_ptr, node_tiles
+        self.n_node_tiles = int(node_tiles.numel()) // 2
+        self._keep = keep
         g = nat.EqdGraph()
         g.n_pairs, g.n_nodes, g.n_lig_nodes = self.n_pairs, self.N, self.N_l
-        g.n_edges, g.n_lig_edges, g.max_in_degree = self.E, self.E_l, int(max_in_degree)
-        g.seg_ptr, g.row_ptr = self.seg_ptr.data_ptr(), self.row_ptr.data_ptr()
-        g.col_src, g.edge_dst = self.col_src.data_ptr(), self.edge_dst.data_ptr()
-        g.he_lig, g.he_rec = self.he_l.data_ptr(), self.he_r.data_ptr()
-        g.n_node_tiles, g.node_tiles = self.n_node_tiles, self.node_tiles.data_ptr()
+        g.n_edges, g.n_lig_edges, g.max_in_degree = self.E, int(n_lig_edges), int(max_in_degree)
+        g.seg_ptr, g.row_ptr = seg_ptr.data_ptr(), row_ptr.data_ptr()
+        g.col_src, g.edge_dst = col_src.data_ptr(), edge_dst.data_ptr()
+        g.he_lig, g.he_rec = he_l.data_ptr(), he_r.data_ptr()
+        g.n_node_tiles, g.node_tiles = self.n_node_tiles, node_tiles.data_ptr()
         self.struct = g
 
     def refresh(self, graph) -> bool:
@@ -363,54 +376,61 @@ class GraphPlan:
         row past the end, either one buffer [E+1][27] for both edge types passed twice (n_lig_edges = E) or the ligand
         rows [E_l+1][27] and the receptor rows [E_r+1][27] (n_lig_edges = E_l).  ``seg_ptr`` [2B+1] / ``node_tiles`` [T][2] int32 on the device, ``seg_ptr_host`` the same
         offsets on the host, ``device`` the device the plan reports.  ``keep`` holds tensors the plan's pointers depend on."""
-        plan = cls.__new__(cls)
-        B, dev = len(n_lig), device
-        plan.n_pairs, plan.forward_ws_bytes = B, None
-        plan.n_lig_list, plan.n_rec_list = [int(v) for v in n_lig], [int(v) for v in n_rec]
-        N_l, N = sum(plan.n_lig_list), sum(plan.n_lig_list) + sum(plan.n_rec_list)
-        plan.N_l, plan.N_r, plan.N, plan.device = N_l, N - N_l, N, dev
-        plan.E_l, plan.E_r, plan.E = int(E_l), int(E) - int(E_l), int(E)
-        plan.col_src, plan.edge_dst, plan.row_ptr = col_src, edge_dst, row_ptr
-        plan.unsorted = torch.zeros((), dtype=torch.bool, device=dev)
-        plan.unsorted_i32 = torch.zeros(1, dtype=torch.int32, device=dev)
-        plan._arange = None
-        plan.edge_perm = None
-        plan.he_l, plan.he_r = he_l, he_r
-        plan.seg_ptr_host, plan.n_node_tiles = seg_ptr_host, int(node_tiles.numel()) // 2
-        plan.seg_ptr, plan.node_tiles = seg_ptr, node_tiles
-        gs = nat.EqdGraph()
-        gs.n_pairs, gs.n_nodes, gs.n_lig_nodes = B, N, N_l
-        gs.n_edges, gs.n_lig_edges, gs.max_in_degree = plan.E, plan.E if he_r is he_l else plan.E_l, int(max_in_degree)
-        gs.seg_ptr, gs.row_ptr = seg_ptr.data_ptr(), row_ptr.data_ptr()
-        gs.col_src, gs.edge_dst = col_src.data_ptr(), edge_dst.data_ptr()
-        gs.he_lig, gs.he_rec = he_l.data_ptr(), he_r.data_ptr()
-        gs.n_node_tiles, gs.node_tiles = plan.n_node_tiles, node_tiles.data_ptr()
-        plan.struct = gs
-        plan._keep = keep
+        plan = object.__new__(cls)
+        plan._finish(n_lig, n_rec, E_l, E, E if he_r is he_l else E_l, col_src, edge_dst, row_ptr, he_l, he_r, seg_ptr_host,
+                     seg_ptr, node_tiles, device, max_in_degree, keep=keep)
         return plan
 
     @classmethod
-    def from_graph(cls, graph, device, max_in_degree: int = 10) -> 'GraphPlan':
-        """From a batched DGL heterograph (train_utils.py:61-100) or a ``PairGraphBatch``."""
+    def from_graph(cls, graph, device, max_in_degree: int = 10, he=None, sort: bool = False) -> 'GraphPlan':
+        """From a batched DGL heterograph (train_utils.py:61-100) or a ``PairGraphBatch``.  ``he`` = (ligand, receptor)
+        edge features to use in place of the graph's.  ``sort`` is the slow path for graphs whose edges are not grouped by
+        destination: the plan holds a stable destination-sorted copy, and ``edge_perm`` its (ligand, receptor)
+        permutations: sorted edge i is the caller's edge perm[i]."""
         n_l = graph.batch_num_nodes(LIGAND).tolist()
         n_r = graph.batch_num_nodes(RECEPTOR).tolist()
-        src_l, dst_l = graph.edges(etype=LL)
-        src_r, dst_r = graph.edges(etype=RR)
-        return cls(n_l, n_r, src_l, dst_l, src_r, dst_r, graph.edges[LL].data['he'], graph.edges[RR].data['he'],
-                   device, max_in_degree)
+        he_l, he_r = he if he is not None else (graph.edges[LL].data['he'], graph.edges[RR].data['he'])
+        sides = [(*graph.edges(etype=LL), he_l), (*graph.edges(etype=RR), he_r)]
+        perms = None
+        if sort:
+            sides = [tuple(t.to(device) for t in side) for side in sides]
+            perms = tuple(torch.sort(d.long(), stable=True).indices for _, d, _ in sides)
+            sides = [tuple(t[perm] for t in side) for side, perm in zip(sides, perms)]
+        (src_l, dst_l, he_l), (src_r, dst_r, he_r) = sides
+        plan = cls(n_l, n_r, src_l, dst_l, src_r, dst_r, he_l, he_r, device, max_in_degree)
+        plan.edge_perm = perms
+        return plan
+
+    def caller_edge_order(self, dhe):
+        """Edge gradients [E][27] in the plan's edge order -> (ligand, receptor) in the caller's edge order."""
+        dhe_l, dhe_r = dhe[:self.E_l], dhe[self.E_l:self.E]
+        if self.edge_perm is not None:     # the plan holds a destination-sorted copy: sorted edge i = perm[i]
+            dhe_l = torch.empty_like(dhe_l).index_copy_(0, self.edge_perm[0].to(dhe.device), dhe_l)
+            dhe_r = torch.empty_like(dhe_r).index_copy_(0, self.edge_perm[1].to(dhe.device), dhe_r)
+        return dhe_l, dhe_r
 
 
-def _sorted_copy(plan_args):
-    """Slow path for graphs whose edges are not grouped by destination: stable sort + permute.  Returns the sorted
-    GraphPlan arguments and the (ligand, receptor) permutations: sorted edge i is the caller's edge perm[i]."""
-    n_l, n_r, src_l, dst_l, src_r, dst_r, he_l, he_r, device, mid = plan_args
-    out, perms = [], []
-    for s, d, he in ((src_l, dst_l, he_l), (src_r, dst_r, he_r)):
-        perm = torch.sort(d.long(), stable=True).indices
-        out.append((s[perm], d[perm], he[perm]))
-        perms.append(perm)
-    (sl, dl, hl), (sr, dr, hr) = out
-    return (n_l, n_r, sl, dl, sr, dr, hl, hr, device, mid), tuple(perms)
+def plan_for(graph, device, max_in_degree, sort: bool = False) -> GraphPlan:
+    """GraphPlan of a graph object, cached on it (the topology of a batch never changes).  ``sort`` builds (and caches)
+    the destination-sorted plan of ``GraphPlan.from_graph`` instead."""
+    cached = getattr(graph, '_eqd_plan', None)
+    if not sort and cached is not None and cached.device == device and cached.struct.max_in_degree == max_in_degree:
+        return cached
+    plan = GraphPlan.from_graph(graph, device, max_in_degree, sort=sort)
+    try:
+        graph._eqd_plan = plan
+    except AttributeError:
+        pass
+    return plan
+
+
+def retry_sorted(graph, plan: GraphPlan, run):
+    """``run(plan)``; when that finds the edges not grouped by destination (UnsortedEdges), ``run`` once more with the
+    graph's destination-sorted plan."""
+    try:
+        return run(plan)
+    except UnsortedEdges:
+        return run(plan_for(graph, plan.device, plan.struct.max_in_degree, sort=True))
 
 
 class _StatusPool:
@@ -420,7 +440,6 @@ class _StatusPool:
     page-locked memory per call (cudaHostAlloc) would stall the CPU for tens of milliseconds every few steps."""
 
     def __init__(self):
-        import threading
         self.free, self.lock = [], threading.Lock()
 
     def take(self, n: int) -> torch.Tensor:
@@ -628,6 +647,41 @@ class IEGMNEngine:
                     sys.exit(1)
                 if int(out['status'][b].item()) & nat.STATUS_SVD_DEGENERATE == 0:
                     break
+
+
+def run_layer(plan: GraphPlan, lay: PackedLayer, desc, inputs, keep_mu: bool):
+    """One IEGMN_Layer call on the device: eqd_project + eqd_iegmn_layer_forward with the eqd_layer ``desc`` (``lay``'s
+    descriptor, or its copy with this call's dropout).  ``inputs`` are the ten floating-point tensors of
+    IEGMN_Layer.forward in its argument order (the edge features are the plan's).  Returns the staged inputs and the
+    outputs in global node order: h [N][dhp] f32, h0 [N][72] f32, x_in [N][3] f64, aggr [N][64] f32, mu [N][dhp] f32 (None
+    unless ``keep_mu``), h_out [N][64] f32, x_out [N][3] f64."""
+    x_l, h_l, h0_l, _, xo_l, x_r, h_r, h0_r, _, xo_r = inputs
+    dev = x_l.device
+    lib = IEGMNEngine(dev).lib
+    N, dhp = plan.N, lay.dhp
+    f32, f64 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.float64, device=dev)
+    h = torch.zeros(N, dhp, **f32)
+    h[:, :lay.dh] = torch.cat([h_l, h_r]).to(**f32)
+    h0 = torch.zeros(N, nat.H0_PAD, **f32)
+    h0[:, :nat.H0] = torch.cat([h0_l, h0_r]).to(**f32)
+    x_in = torch.cat([x_l, x_r]).to(**f64).contiguous()
+    x_orig = torch.cat([xo_l, xo_r]).to(**f64).contiguous()
+    proj = torch.empty(N, 128 + 3 * dhp, **f32)
+    aggr, h_out = torch.empty(N, nat.HID, **f32), torch.empty(N, nat.HID, **f32)
+    mu = torch.empty(N, dhp, **f32) if keep_mu else None
+    x_out = torch.empty(N, 3, **f64)
+    status = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        g, lp = C.byref(plan.struct), C.byref(desc)
+        nat.check(lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
+        nat.check(lib.eqd_iegmn_layer_forward(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
+                                              nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(mu),
+                                              nat.ptr(h_out), nat.ptr(x_out), nat.ptr(status), st),
+                  'eqd_iegmn_layer_forward')
+    if int(status[plan.n_pairs].item()) & nat.STATUS_DEGREE_OVERFLOW:
+        raise nat.NativeLibraryError(f'IEGMN_Layer.forward: in-degree above {plan.struct.max_in_degree}')
+    return h, h0, x_in, aggr, mu, h_out, x_out
 
 
 class UnsortedEdges(RuntimeError):

@@ -11,14 +11,16 @@ attached, so ``model(graph, epoch)`` / ``model.graphed(graph)`` run on it direct
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, List, Sequence, Tuple
+from types import SimpleNamespace
+from typing import Dict, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from . import _native as nat
-from .engine import GraphPlan
-from .hetero_graph import LIGAND, LL, RECEPTOR, RR, PairGraphBatch
+from .engine import GraphPlan, node_tiles_for
+from .graphed import GraphedForward
+from .hetero_graph import CROSS_LR, CROSS_RL, LIGAND, LL, RECEPTOR, RR, PairGraphBatch
 
 MAXK = 16
 
@@ -54,7 +56,6 @@ class ResidueBatch:
 
 
 def _edge_counts(ne_l, ne_r, B):
-    from .hetero_graph import CROSS_LR, CROSS_RL
     z = torch.zeros(B, dtype=torch.int64)
     return {LL: torch.tensor(ne_l, dtype=torch.int64), RR: torch.tensor(ne_r, dtype=torch.int64), CROSS_RL: z, CROSS_LR: z.clone()}
 
@@ -100,39 +101,22 @@ def build_graphs(rb: ResidueBatch, device, cutoff: float = 30.0, max_neighbor: i
     ``sync_sizes=True`` reads the edge counts back (one small D2H) so that the result is a fully formed PairGraphBatch;
     ``False`` keeps everything asynchronous: edge buffers stay sized for N x max_neighbor edges and the attached GraphPlan
     serves the forward pass (inference) without the host ever learning E."""
-    lib = nat.load()
     dev = torch.device(device)
-    if buffers is not None:
-        dev_inputs = buffers.inputs          # already uploaded by the caller (GraphBuffers.upload)
-    d = dev_inputs or {k: v.to(dev, non_blocking=True) for k, v in rb.t.items()}
     N, B = rb.N, rb.n_pairs
     N_l = sum(rb.n_lig)
-    i32 = dict(dtype=torch.int32, device=dev)
-    f32 = dict(dtype=torch.float32, device=dev)
+    e_cap = N * int(max_neighbor)
+    if buffers is None:
+        i32, f32 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.float32, device=dev)
+        buffers = SimpleNamespace(
+            inputs=dev_inputs or {k: v.to(dev, non_blocking=True) for k, v in rb.t.items()},
+            ws=torch.empty(int(nat.load().eqd_graph_build_workspace_bytes(N)), dtype=torch.uint8, device=dev),
+            deg=torch.empty(N, **i32), x=torch.empty(N, 3, **f32), mu=torch.empty(N, 5, **f32),
+            row_ptr=torch.zeros(N + 1, **i32), col_src=torch.empty(e_cap, **i32), edge_dst=torch.empty(e_cap, **i32),
+            he=torch.empty(e_cap + 1, 27, **f32))                  # +1 row: readable past the end for the TMA over-read
+    rebuild_in_place(rb, buffers, cutoff, max_neighbor)     # (the inputs of a GraphBuffers were uploaded by the caller)
+    d, x, mu = buffers.inputs, buffers.x, buffers.mu
+    row_ptr, col_src, edge_dst, he = buffers.row_ptr, buffers.col_src, buffers.edge_dst, buffers.he
     with torch.cuda.device(dev):
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        ws_bytes = int(lib.eqd_graph_build_workspace_bytes(N))
-        if buffers is not None:
-            ws, deg, x, mu = buffers.ws, buffers.deg, buffers.x, buffers.mu
-        else:
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-            deg = torch.empty(N, **i32)
-            x = torch.empty(N, 3, **f32)
-            mu = torch.empty(N, 5, **f32)
-        nat.check(lib.eqd_graph_build_knn(2 * B, N, rb.max_protein_nodes, nat.ptr(d['seg_ptr']), nat.ptr(d['atom_ptr']),
-                                          nat.ptr(d['atoms']), nat.ptr(d['nca_c']), nat.ptr(d['bound_ca']), float(cutoff),
-                                          int(max_neighbor), nat.ptr(ws), ws_bytes, nat.ptr(deg), nat.ptr(x), nat.ptr(mu), st),
-                  'eqd_graph_build_knn')
-        e_cap = N * int(max_neighbor)
-        if buffers is not None:
-            row_ptr, col_src, edge_dst, he = buffers.row_ptr, buffers.col_src, buffers.edge_dst, buffers.he
-        else:
-            row_ptr = torch.zeros(N + 1, **i32)
-            col_src, edge_dst = torch.empty(e_cap, **i32), torch.empty(e_cap, **i32)
-            he = torch.empty(e_cap + 1, 27, **f32)                  # +1 row: readable past the end for the TMA over-read
-        torch.cumsum(deg, 0, dtype=torch.int32, out=row_ptr[1:])    # exclusive prefix sum: an index op
-        nat.check(lib.eqd_graph_build_edges(N, nat.ptr(row_ptr), nat.ptr(deg), nat.ptr(ws), nat.ptr(col_src), nat.ptr(edge_dst),
-                                            nat.ptr(he), st), 'eqd_graph_build_edges')
         if sync_sizes:       # ONE small D2H: the edge offsets at the 2B + 1 protein boundaries
             bounds = row_ptr[d['seg_ptr'].long()].cpu().tolist()
             E_l, E = int(bounds[B]), int(bounds[2 * B])
@@ -149,19 +133,15 @@ def build_graphs(rb: ResidueBatch, device, cutoff: float = 30.0, max_neighbor: i
     g._ndata[RECEPTOR] = {'res_feat': d['res_feat'][N_l:], 'x': x[N_l:], 'mu_r_norm': mu[N_l:]}
     if sync_sizes:
         g._edata[LL]['he'], g._edata[RR]['he'] = he[:E_l], he[E_l:E]
-    seg = np.zeros(2 * B + 1, dtype=np.int64)
-    seg[1:] = np.cumsum(np.asarray(list(rb.n_lig) + list(rb.n_rec), dtype=np.int64))
-    tiles = [(s, n0) for s in range(2 * B) for n0 in range(int(seg[s]), int(seg[s + 1]), nat.TILE_ROWS)]
-    small = torch.from_numpy(np.concatenate([seg.astype(np.int32), np.asarray(tiles, dtype=np.int32).reshape(-1)])).to(dev, non_blocking=True)
-    plan = GraphPlan.from_device_arrays(rb.n_lig, rb.n_rec, E_l, E, col_src, edge_dst, row_ptr, he, he, small[:2 * B + 1],
-                                        small[2 * B + 1:], seg, dev, int(max_neighbor), keep=(ws, deg, d))
-    plan._small = small
-    g._eqd_plan = plan
+    seg, seg_ptr, node_tiles = node_tiles_for(rb.n_lig, rb.n_rec, dev)
+    g._eqd_plan = GraphPlan.from_device_arrays(rb.n_lig, rb.n_rec, E_l, E, col_src, edge_dst, row_ptr, he, he, seg_ptr,
+                                               node_tiles, seg, dev, int(max_neighbor), keep=(buffers.ws, buffers.deg, d))
     return g
 
 
 def rebuild_in_place(rb: ResidueBatch, buffers: GraphBuffers, cutoff: float = 30.0, max_neighbor: int = 10):
-    """The three kernels + prefix sum of ``build_graphs`` writing into existing buffers (nothing allocated: capturable)."""
+    """The three graph kernels + one prefix sum (an index op), from ``buffers.inputs`` into the output tensors of
+    ``buffers`` (nothing allocated: capturable)."""
     lib = nat.load()
     d = buffers.inputs
     dev = buffers.x.device
@@ -184,36 +164,14 @@ class ResidueGraphedForward:
     graph (k-NN edges, 27 edge features, surface features) never exists on the host."""
 
     def __init__(self, model, rb: ResidueBatch, device, cutoff: float = 30.0, max_neighbor: int = 10):
-        from .graphed import GraphedForward, refuse_dropout_capture
         self.model, self.device = model, torch.device(device)
         self.cutoff, self.max_neighbor = cutoff, max_neighbor
         self.buffers = GraphBuffers(rb, device, max_neighbor)
         self.rb = rb
         self.buffers.upload(rb)
         self.graph = build_graphs(rb, device, cutoff, max_neighbor, sync_sizes=False, buffers=self.buffers)
-        outer = self
-
-        class _Captured(GraphedForward):
-            def _capture(self_inner):
-                # identical to GraphedForward._capture, with the graph build recorded in front of the forward
-                refuse_dropout_capture(self_inner.iegmn)
-                with torch.cuda.device(self_inner.device):
-                    cur = torch.cuda.current_stream(self_inner.device)
-                    self_inner.stream.wait_stream(cur)
-                    with torch.cuda.stream(self_inner.stream):
-                        for _ in range(2):
-                            rebuild_in_place(outer.rb, outer.buffers, outer.cutoff, outer.max_neighbor)
-                            self_inner.iegmn.resolve(self_inner.iegmn.run_engine(self_inner.batch, check_status=False))
-                    self_inner.stream.synchronize()
-                    self_inner.plan = self_inner.batch._eqd_plan
-                    self_inner.key = self_inner._param_key()
-                    self_inner.graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(self_inner.graph, stream=self_inner.stream):
-                        rebuild_in_place(outer.rb, outer.buffers, outer.cutoff, outer.max_neighbor)
-                        self_inner.raw = self_inner.iegmn.run_engine(self_inner.batch, check_status=False, record_event=False)
-                    cur.wait_stream(self_inner.stream)
-
-        self.gf = _Captured(model, self.graph)
+        self.gf = GraphedForward(model, self.graph, before_forward=lambda: rebuild_in_place(
+            self.rb, self.buffers, self.cutoff, self.max_neighbor))
 
     def upload(self, rb: ResidueBatch, stream=None):
         if not self.buffers.matches(rb):

@@ -36,8 +36,10 @@ def refuse_dropout_capture(iegmn):
 
 
 class GraphedForward:
-    def __init__(self, model, device_batch):
-        self.model, self.batch = model, device_batch
+    def __init__(self, model, device_batch, before_forward=lambda: None):
+        """``before_forward()`` is run (and recorded) in front of every forward of a capture: work on the capture stream
+        that produces the batch's tensors in place (``graph_build.ResidueGraphedForward``: the graph build)."""
+        self.model, self.batch, self.before_forward = model, device_batch, before_forward
         self.iegmn = model.iegmn_original
         self.device = self.iegmn.residue_emb_layer.weight.device
         if self.device.type != 'cuda':
@@ -61,12 +63,14 @@ class GraphedForward:
                 # eager warm-up on the capture stream: builds / caches the plan, the packed weights and every
                 # one-time attribute, and proves the batch is servable before anything is recorded
                 for _ in range(2):
+                    self.before_forward()
                     self.iegmn.resolve(self.iegmn.run_engine(self.batch, check_status=False))
             self.stream.synchronize()
             self.plan = self.batch._eqd_plan
             self.key = self._param_key()
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph, stream=self.stream):
+                self.before_forward()
                 self.raw = self.iegmn.run_engine(self.batch, check_status=False, record_event=False)
             cur.wait_stream(self.stream)
 

@@ -43,8 +43,8 @@ except ImportError:  # DGL-free deployments use the package's own container
     fn = None
 
 from . import _native as nat
-from .engine import (PRECISIONS, GraphPlan, IEGMNEngine, PackedHead, PackedLayer, UnsortedEdges, _sorted_copy, check_precision,
-                     draw_dropout, with_dropout)
+from .engine import (PRECISIONS, GraphPlan, IEGMNEngine, PackedHead, PackedLayer, check_precision, draw_dropout, plan_for,
+                     retry_sorted, run_layer, with_dropout)
 from .hetero_graph import LIGAND, LL, RECEPTOR, RR
 
 
@@ -117,54 +117,16 @@ def _check_layer_args(args):
                                       '(the configuration of both shipped checkpoints)')
 
 
-def _plan_for(graph, device, max_in_degree):
-    """GraphPlan of a graph object, cached on it (the topology of a batch never changes)."""
-    cached = getattr(graph, '_eqd_plan', None)
-    if cached is not None and cached.device == device and cached.struct.max_in_degree == max_in_degree:
-        return cached
-    plan = GraphPlan.from_graph(graph, device, max_in_degree)
-    try:
-        graph._eqd_plan = plan
-    except AttributeError:
-        pass
-    return plan
-
-
-def _sorted_plan(graph, device, max_in_degree):
-    src_l, dst_l = graph.edges(etype=LL)
-    src_r, dst_r = graph.edges(etype=RR)
-    args = (graph.batch_num_nodes(LIGAND).tolist(), graph.batch_num_nodes(RECEPTOR).tolist(), src_l.to(device),
-            dst_l.to(device), src_r.to(device), dst_r.to(device), graph.edges[LL].data['he'].to(device),
-            graph.edges[RR].data['he'].to(device), device, max_in_degree)
-    sorted_args, perms = _sorted_copy(args)
-    plan = GraphPlan(*sorted_args)
-    plan.edge_perm = perms        # scatters edge gradients back to the caller's edge order (training.TrainEngine)
-    try:
-        graph._eqd_plan = plan
-    except AttributeError:
-        pass
-    return plan
-
-
 def _layer_plan(graph, device, max_in_degree, he_l, he_r):
     """GraphPlan of an IEGMN_Layer call under autograd: the graph's cached plan when ``he_l`` / ``he_r`` are the tensors it
     was built from, else one built with the caller's edge features.  Edges not grouped by destination get a
     destination-sorted copy whose ``edge_perm`` maps edge gradients back to the caller's order."""
-    plan = _plan_for(graph, device, max_in_degree)
+    plan = plan_for(graph, device, max_in_degree)
     if plan.edge_perm is None and bool(plan.unsorted.item()):
-        plan = _sorted_plan(graph, device, max_in_degree)
+        plan = plan_for(graph, device, max_in_degree, sort=True)
     if plan.edge_perm is None and he_l.data_ptr() == plan.he_l.data_ptr() and he_r.data_ptr() == plan.he_r.data_ptr():
         return plan
-    src_l, dst_l = graph.edges(etype=LL)
-    src_r, dst_r = graph.edges(etype=RR)
-    args = (plan.n_lig_list, plan.n_rec_list, src_l.to(device), dst_l.to(device), src_r.to(device), dst_r.to(device),
-            he_l.detach().to(device), he_r.detach().to(device), device, max_in_degree)
-    if plan.edge_perm is None:
-        return GraphPlan(*args)
-    sorted_args, perms = _sorted_copy(args)
-    plan = GraphPlan(*sorted_args)
-    plan.edge_perm = perms
-    return plan
+    return GraphPlan.from_graph(graph, device, max_in_degree, (he_l.detach(), he_r.detach()), sort=plan.edge_perm is not None)
 
 
 def _wants_autograd(module, tensors):
@@ -187,6 +149,14 @@ def _module_state(module):
 
 def _version_key(module):
     return tuple((p.data_ptr(), p._version) for p in module.parameters())
+
+
+def _reset_parameters(module):
+    for p in module.parameters():
+        if p.dim() > 1:
+            torch.nn.init.xavier_normal_(p, gain=1.)
+        else:
+            torch.nn.init.zeros_(p)
 
 
 class IEGMN_Layer(nn.Module):
@@ -233,12 +203,7 @@ class IEGMN_Layer(nn.Module):
             raise NotImplementedError('CUDA engine widths: input_edge_feats_dim=27, hidden 64, node input 69')
         self._packed, self._packed_key = None, None
 
-    def reset_parameters(self):
-        for p in self.parameters():
-            if p.dim() > 1:
-                torch.nn.init.xavier_normal_(p, gain=1.)
-            else:
-                torch.nn.init.zeros_(p)
+    reset_parameters = _reset_parameters
 
     def packed(self, device) -> PackedLayer:
         """Kernel-layout copy of the parameters, rebuilt only when a parameter changed."""
@@ -262,52 +227,25 @@ class IEGMN_Layer(nn.Module):
         ``force_autograd``, or when an input requires grad, the call is one autograd node whose backward is the CUDA
         per-layer backward (``training.layer_backward``): gradients reach the layer's parameters and all ten tensor
         inputs."""
-        import ctypes as C
         inputs = (coors_ligand, h_feats_ligand, original_ligand_node_features, original_edge_feats_ligand,
                   orig_coors_ligand, coors_receptor, h_feats_receptor, original_receptor_node_features,
                   original_edge_feats_receptor, orig_coors_receptor)
-        if _wants_autograd(self, inputs):
-            return self._forward_autograd(hetero_graph, inputs)
         dev = coors_ligand.device
-        eng = IEGMNEngine(dev)
-        plan = _plan_for(hetero_graph, dev, self.graph_max_neighbor)
-        if original_edge_feats_ligand.data_ptr() != plan.he_l.data_ptr():  # caller scaled / replaced he
-            plan = GraphPlan(plan.n_lig_list, plan.n_rec_list, *hetero_graph.edges(etype=LL),
-                             *hetero_graph.edges(etype=RR), original_edge_feats_ligand, original_edge_feats_receptor,
-                             dev, self.graph_max_neighbor)
-        lay = self.packed(dev)
-        N, dhp = plan.N, lay.dhp
-        f32, f64 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.float64, device=dev)
-        h = torch.zeros(N, dhp, **f32)
-        h[:, :lay.dh] = torch.cat([h_feats_ligand, h_feats_receptor]).to(**f32)
-        h0 = torch.zeros(N, nat.H0_PAD, **f32)
-        h0[:, :nat.H0] = torch.cat([original_ligand_node_features, original_receptor_node_features]).to(**f32)
-        x_in = torch.cat([coors_ligand, coors_receptor]).to(**f64).contiguous()
-        x_orig = torch.cat([orig_coors_ligand, orig_coors_receptor]).to(**f64).contiguous()
-        proj = torch.empty(N, 128 + 3 * dhp, **f32)
-        aggr, h_out = torch.empty(N, nat.HID, **f32), torch.empty(N, nat.HID, **f32)
-        x_out = torch.empty(N, 3, **f64)
-        status = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        desc = with_dropout([lay.struct], self.dropout_now())[0]   # each call is its own forward: own seed, layer 0
-        g, lp = C.byref(plan.struct), C.byref(desc)
-        nat.check(eng.lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
-        nat.check(eng.lib.eqd_iegmn_layer_forward(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
-                                                  nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), None,
-                                                  nat.ptr(h_out), nat.ptr(x_out), nat.ptr(status), st),
-                  'eqd_iegmn_layer_forward')
-        if int(status[plan.n_pairs].item()) & nat.STATUS_DEGREE_OVERFLOW or bool(plan.unsorted.item()):
-            raise nat.NativeLibraryError('IEGMN_Layer.forward: edges must be grouped by destination with in-degree '
-                                         f'<= {self.graph_max_neighbor}')
+        if _wants_autograd(self, inputs):
+            from .training import layer_autograd
+            plan = _layer_plan(hetero_graph, dev, self.graph_max_neighbor, inputs[3], inputs[8])
+            x_out, h_out = layer_autograd(self, plan, inputs)
+        else:
+            plan = plan_for(hetero_graph, dev, self.graph_max_neighbor)
+            if original_edge_feats_ligand.data_ptr() != plan.he_l.data_ptr():  # caller scaled / replaced he
+                plan = GraphPlan.from_graph(hetero_graph, dev, self.graph_max_neighbor,
+                                            (original_edge_feats_ligand, original_edge_feats_receptor))
+            lay = self.packed(dev)
+            desc = with_dropout([lay.struct], self.dropout_now())[0]   # each call is its own forward: own seed, layer 0
+            h_out, x_out = run_layer(plan, lay, desc, inputs, keep_mu=False)[5:]
+            if bool(plan.unsorted.item()):
+                raise nat.NativeLibraryError('IEGMN_Layer.forward: edges must be grouped by destination')
         x_out = x_out.to(coors_ligand.dtype)
-        return x_out[:plan.N_l], h_out[:plan.N_l], x_out[plan.N_l:], h_out[plan.N_l:]
-
-    def _forward_autograd(self, hetero_graph, inputs):
-        from .training import layer_autograd
-        dev = inputs[0].device
-        plan = _layer_plan(hetero_graph, dev, self.graph_max_neighbor, inputs[3], inputs[8])
-        x_out, h_out = layer_autograd(self, plan, inputs)
-        x_out = x_out.to(inputs[0].dtype)
         return x_out[:plan.N_l], h_out[:plan.N_l], x_out[plan.N_l:], h_out[plan.N_l:]
 
     def __repr__(self):
@@ -372,12 +310,7 @@ class IEGMN(nn.Module):
     def precision(self, value: str):
         self._precision = check_precision(value)
 
-    def reset_parameters(self):
-        for p in self.parameters():
-            if p.dim() > 1:
-                torch.nn.init.xavier_normal_(p, gain=1.)
-            else:
-                torch.nn.init.zeros_(p)
+    reset_parameters = _reset_parameters
 
     def packed_head(self, device) -> PackedHead:
         mods = (self.att_mlp_key_ROT, self.att_mlp_query_ROT, self.mlp_h_mean_ROT)
@@ -389,77 +322,63 @@ class IEGMN(nn.Module):
             self._head_key = key
         return self._head
 
-    def run_engine(self, batch_hetero_graph, check_status=True, record_event=True, dropout='draw'):
+    def run_engine(self, batch_hetero_graph, check_status=True, record_event=True):
         """The whole hot path on the device; returns the engine's raw output dict.  With ``check_status=False`` the
         per-pair status words are left pending (``resolve(out)`` finishes the call).  ``record_event=False`` is for
-        CUDA-graph capture (``graphed.GraphedForward``), which records its own completion event per replay.
-        ``dropout``: 'draw' = draw this forward's dropout in training mode (engine.draw_dropout), else the tuple of a
-        forward being re-run."""
+        CUDA-graph capture (``graphed.GraphedForward``), which records its own completion event per replay.  In
+        training mode this forward's dropout is drawn here (engine.draw_dropout)."""
+        dev = self.residue_emb_layer.weight.device
+        dropout = self.iegmn_layers[0].dropout_now() if self.training else None
+        return retry_sorted(batch_hetero_graph, plan_for(batch_hetero_graph, dev, self.graph_max_neighbor),
+                            lambda plan: self._launch(batch_hetero_graph, plan, check_status, record_event, dropout))
+
+    def _launch(self, batch_hetero_graph, plan, check_status, record_event, dropout):
         emb = self.residue_emb_layer.weight
         dev = emb.device
         eng = IEGMNEngine(dev)
         layers = [lay.packed(dev) for lay in self.iegmn_layers]
-        head = self.packed_head(dev)
         nl, nr = batch_hetero_graph.nodes[LIGAND].data, batch_hetero_graph.nodes[RECEPTOR].data
-        plan = _plan_for(batch_hetero_graph, dev, self.graph_max_neighbor)
-        emb32 = emb.detach().to(torch.float32).contiguous()
-        products = PRECISIONS[self.precision]
-        if isinstance(dropout, str):
-            dropout = self.iegmn_layers[0].dropout_now() if self.training else None
-        call = lambda p, chk: eng.forward(p, emb32, layers, head, nl['res_feat'], nr['res_feat'], nl['mu_r_norm'],
-                                          nr['mu_r_norm'], nl['new_x'], nr['x'], chk, self.log,
-                                          record_event=record_event, mma_products=products, dropout=dropout)
-        try:
-            out = call(plan, check_status)
-        except UnsortedEdges:
-            plan = _sorted_plan(batch_hetero_graph, dev, self.graph_max_neighbor)
-            out = call(plan, True)
+        out = eng.forward(plan, emb.detach().to(torch.float32).contiguous(), layers, self.packed_head(dev), nl['res_feat'],
+                          nr['res_feat'], nl['mu_r_norm'], nr['mu_r_norm'], nl['new_x'], nr['x'], check_status, self.log,
+                          record_event=record_event, mma_products=PRECISIONS[self.precision], dropout=dropout)
         out['plan'], out['engine'], out['graph'], out['dropout'] = plan, eng, batch_hetero_graph, dropout
         return out
 
     def resolve(self, out):
         """Finishes a ``run_engine(..., check_status=False)`` call: waits for its status words and replays the
         reference's host-side control flow for flagged pairs (:570-584).  Unsorted edge lists are re-run sorted."""
-        try:
-            out['engine'].resolve_status(out['plan'], out, out['kabsch'], self.log)
+        def finish(plan):
+            if plan is not out['plan']:     # re-run sorted: the same forward, so the same dropout seed
+                return self._launch(out['graph'], plan, True, True, out['dropout'])
+            out['engine'].resolve_status(plan, out, out['kabsch'], self.log)
             return out
-        except UnsortedEdges:     # re-run sorted: the same forward, so the same dropout seed
-            return self.run_engine(out['graph'], True, dropout=out['dropout'])
+        return retry_sorted(out['graph'], out['plan'], finish)
 
     def forward(self, batch_hetero_graph, epoch):
         """Returns ``[T list, b list, Y_ligand list, Y_receptor list]`` like the reference (:602) and
         writes ``x_iegmn_out`` / ``hv_iegmn_out`` into the graph (:507-510).  Under the condition of
         ``Rigid_Body_Docking_Net.forward`` the whole stack is the same single autograd node (``training._HotPath``)."""
         if _wants_autograd(self, graph_inputs(batch_hetero_graph)):
-            return self._forward_autograd(batch_hetero_graph)
+            from .training import autograd_forward
+            fwd, outs = autograd_forward(self, batch_hetero_graph, self.log)
+            return self.package(fwd, batch_hetero_graph, outs[1:])
         return self.package(self.run_engine(batch_hetero_graph), batch_hetero_graph)
 
-    def _forward_autograd(self, batch_hetero_graph):
-        from .training import autograd_forward
-        fwd, (_, keypts, rot, trans, x_fin, h_fin) = autograd_forward(self, batch_hetero_graph, self.log)
-        plan = fwd['plan']
-        B, N_l = plan.n_pairs, plan.N_l
+    def package(self, out, batch_hetero_graph, tensors=None):
+        """The reference's return value from a forward's raw output dict ``out``; ``tensors`` = (keypoints, rotations,
+        translations, last-layer coordinates, last-layer features) are used in place of the dict's (the differentiable
+        outputs of an autograd node)."""
+        keypts, rot, trans, x_fin, h_fin = tensors if tensors is not None else (
+            out['keypts'], out['rotation'], out['translation'], out['x64'], out['h'])
+        B, N_l = out['plan'].n_pairs, out['plan'].N_l
         nl, nr = batch_hetero_graph.nodes[LIGAND].data, batch_hetero_graph.nodes[RECEPTOR].data
         dt = nl['new_x'].dtype
         x_fin = x_fin.to(dt)
         nl['x_iegmn_out'], nr['x_iegmn_out'] = x_fin[:N_l], x_fin[N_l:]
         nl['hv_iegmn_out'], nr['hv_iegmn_out'] = h_fin[:N_l], h_fin[N_l:]
-        self.last_outputs = fwd
         keyp = keypts.to(dt)
-        return [list(rot.unbind(0)), list(trans.unbind(0)), list(keyp[:B].unbind(0)), list(keyp[B:].unbind(0))]
-
-    def package(self, out, batch_hetero_graph):
-        plan = out['plan']
-        B, N_l = plan.n_pairs, plan.N_l
-        dt = batch_hetero_graph.nodes[LIGAND].data['new_x'].dtype
-        x_fin = out['x64'].to(dt)
-        nl, nr = batch_hetero_graph.nodes[LIGAND].data, batch_hetero_graph.nodes[RECEPTOR].data
-        nl['x_iegmn_out'], nr['x_iegmn_out'] = x_fin[:N_l], x_fin[N_l:]
-        nl['hv_iegmn_out'], nr['hv_iegmn_out'] = out['h'][:N_l], out['h'][N_l:]
-        keyp = out['keypts'].to(dt)
         self.last_outputs = out
-        return [list(out['rotation'].unbind(0)), list(out['translation'].unbind(0)),
-                list(keyp[:B].unbind(0)), list(keyp[B:].unbind(0))]
+        return [list(rot.unbind(0)), list(trans.unbind(0)), list(keyp[:B].unbind(0)), list(keyp[B:].unbind(0))]
 
     def __repr__(self):
         return 'IEGMN (H100 engine) ' + str({k: v for k, v in self.__dict__.items() if not k.startswith('_')})
@@ -486,12 +405,7 @@ class Rigid_Body_Docking_Net(nn.Module):
     def precision(self, value: str):
         self.iegmn_original.precision = value
 
-    def reset_parameters(self):
-        for p in self.parameters():
-            if p.dim() > 1:
-                torch.nn.init.xavier_normal_(p, gain=1.)
-            else:
-                torch.nn.init.zeros_(p)
+    reset_parameters = _reset_parameters
 
     def forward_async(self, batch_hetero_graph, epoch=0):
         """Launches the whole forward without waiting for its status words; ``.result()`` of the returned handle
@@ -516,37 +430,26 @@ class Rigid_Body_Docking_Net(nn.Module):
         return GraphedForward(self, device_batch)
 
     def forward(self, batch_hetero_graph, epoch):
-        if _wants_autograd(self, graph_inputs(batch_hetero_graph)):
-            return self._forward_autograd(batch_hetero_graph)
-        return self._assemble(self.iegmn_original(batch_hetero_graph, epoch))
-
-    def _forward_autograd(self, batch_hetero_graph):
         """Training mode (``model.train()``, src/train.py:64), or any mode when a graph input tensor requires grad: the
         whole hot path is ONE autograd node whose backward is the hand-written CUDA backward (``training.TrainEngine``), so
         ``loss.backward()`` (train.py:154) fills ``param.grad`` of every parameter and ``.grad`` of the graph's ``new_x`` /
         ``x`` / ``mu_r_norm`` / ``he`` exactly like the reference's autograd graph does.  Outputs, and ``x_iegmn_out`` /
         ``hv_iegmn_out`` in the graph, are autograd-connected views of the node's outputs.  Evaluation under
         ``torch.no_grad()``, or in ``model.eval()`` with no input requiring grad, keeps the inference path."""
-        from .training import autograd_forward
-        fwd, (coors, keypts, rot, trans, x_fin, h_fin) = autograd_forward(self, batch_hetero_graph, self.log)
-        plan = fwd['plan']
-        B, N_l = plan.n_pairs, plan.N_l
-        nl, nr = batch_hetero_graph.nodes[LIGAND].data, batch_hetero_graph.nodes[RECEPTOR].data
-        dt = nl['new_x'].dtype
-        x_fin = x_fin.to(dt)
-        nl['x_iegmn_out'], nr['x_iegmn_out'] = x_fin[:N_l], x_fin[N_l:]
-        nl['hv_iegmn_out'], nr['hv_iegmn_out'] = h_fin[:N_l], h_fin[N_l:]
-        self.iegmn_original.last_outputs = fwd
-        keyp = keypts.to(dt)
-        return (list(torch.split(coors, plan.n_lig_list, dim=0)), list(keyp[:B].unbind(0)), list(keyp[B:].unbind(0)),
-                list(rot.unbind(0)), list(trans.unbind(0)))
+        if _wants_autograd(self, graph_inputs(batch_hetero_graph)):
+            from .training import autograd_forward
+            fwd, outs = autograd_forward(self, batch_hetero_graph, self.log)
+            return self._assemble(self.iegmn_original.package(fwd, batch_hetero_graph, outs[1:]), outs[0])
+        return self._assemble(self.iegmn_original(batch_hetero_graph, epoch))
 
-    def _assemble(self, outputs):
+    def _assemble(self, outputs, ligand_coors=None):
+        """The 5-tuple from IEGMN's four lists and the batched ligand coordinates (default: the last forward's)."""
         assert len(outputs) == 4
         raw = self.iegmn_original.last_outputs
-        plan = raw['plan']
+        if ligand_coors is None:
+            ligand_coors = raw['ligand_coors']
         # T new_x + b of every ligand node was applied by the Kabsch kernel (:665)
-        ligand_coors = list(torch.split(raw['ligand_coors'], plan.n_lig_list, dim=0))
+        ligand_coors = list(torch.split(ligand_coors, raw['plan'].n_lig_list, dim=0))
         for b_align in outputs[1]:
             assert b_align.shape[0] == 1 and b_align.shape[1] == 3
         return ligand_coors, outputs[2], outputs[3], outputs[0], outputs[1]

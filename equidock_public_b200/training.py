@@ -21,7 +21,9 @@ import numpy as np
 import torch
 
 from . import _native as nat
-from .engine import GraphPlan, IEGMNEngine, PackedHead, PackedLayer, _StatusLease, _upload_blob, _host_f32, with_dropout
+from .engine import (GraphPlan, IEGMNEngine, PackedLayer, _upload_blob, _host_f32, plan_for, retry_sorted, run_layer,
+                     with_dropout)
+from .hetero_graph import LIGAND, RECEPTOR
 
 _f32 = torch.float32
 
@@ -235,13 +237,12 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
     N, E = plan.N, plan.E
     lp = C.byref(desc if desc is not None else lp_obj.struct)
     dh, dhp, pw = tp.dh, tp.dhp, tp.pw
-    ldh = nat.H0_PAD if dh == nat.H0 else nat.HID
-    ldmu = nat.H0_PAD if dh == nat.H0 else nat.HID
+    ld = nat.H0_PAD if dh == nat.H0 else nat.HID     # row stride of h_in and of mu
     h_in, x_in, aggr, mu, h0 = _vp(h_in), _vp(x_in), _vp(aggr), _vp(mu), _vp(h0)
-    nat.check(lib.eqd_project(g, lp, h_in, ldh, nat.ptr(ws.proj), st), 'eqd_project')
+    nat.check(lib.eqd_project(g, lp, h_in, ld, nat.ptr(ws.proj), st), 'eqd_project')
     nparts = C.c_int32(0)
-    nat.check(lib.eqd_bwd_node_mlp(g, lp, nat.ptr(tp.t['w_node1_lin']), nat.ptr(tp.t['w_node2_lin']), h_in, ldh,
-                                   aggr, mu, ldmu, h0, nat.ptr(dh_out), nat.ptr(dh_in), nat.ptr(ws.daggr),
+    nat.check(lib.eqd_bwd_node_mlp(g, lp, nat.ptr(tp.t['w_node1_lin']), nat.ptr(tp.t['w_node2_lin']), h_in, ld,
+                                   aggr, mu, ld, h0, nat.ptr(dh_out), nat.ptr(dh_in), nat.ptr(ws.daggr),
                                    nat.ptr(ws.dmu), nat.ptr(ws.dh0), nat.ptr(ws.n5), nat.ptr(ws.du),
                                    nat.ptr(ws.vec), C.byref(nparts), st), 'eqd_bwd_node_mlp')
     _reduce(lib, ws.vec, nparts.value, 144, tp.maps['nodevec'], flat, st)
@@ -250,13 +251,13 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
     nch = _tn(lib, ws, ws.n5, dhp, dhp, dh_out, 64, 64, N, sk, True, st)
     _reduce(lib, ws.partial, nch, dhp * 64, tp.maps['node2'], flat, st)
     _reduce(lib, ws.colsum, nch, 64, tp.maps['node2_bias'], flat, st)
-    for name, X, ldx, K, want in (('node_h', h_in, ldh, dhp, True), ('node_aggr', aggr, 64, 64, False),
-                                  ('node_mu', mu, ldmu, dhp, False), ('node_h0', h0, nat.H0_PAD, nat.H0_PAD, False)):
+    for name, X, ldx, K, want in (('node_h', h_in, ld, dhp, True), ('node_aggr', aggr, 64, 64, False),
+                                  ('node_mu', mu, ld, dhp, False), ('node_h0', h0, nat.H0_PAD, nat.H0_PAD, False)):
         nchx = _tn(lib, ws, X, ldx, K, ws.du, dhp, dhp, N, 1.0, want, st)
         _reduce(lib, ws.partial, nchx, K * dhp, tp.maps[name], flat, st)
         if want:
             _reduce(lib, ws.colsum, nchx, dhp, tp.maps['node1_bias'], flat, st)
-    nat.check(lib.eqd_bwd_attention(g, lp, nat.ptr(ws.proj), mu, ldmu, nat.ptr(ws.dmu), nat.ptr(ws.dP),
+    nat.check(lib.eqd_bwd_attention(g, lp, nat.ptr(ws.proj), mu, ld, nat.ptr(ws.dmu), nat.ptr(ws.dP),
                                     nat.ptr(ws.rowstat), st), 'eqd_bwd_attention')
     nat.check(lib.eqd_bwd_edge(g, lp, nat.ptr(tp.t['w2lin']), nat.ptr(tp.t['w3lin']), nat.ptr(ws.proj), x_in,
                                nat.ptr(ws.daggr), nat.ptr(dx_out), nat.ptr(ws.ein), nat.ptr(ws.n1),
@@ -286,7 +287,7 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
               'eqd_bwd_project')
     if capture is not None:
         capture[-1]['dh'] = dh_in.reshape(-1)[:N * dhp].clone().view(N, dhp)
-    nchx = _tn(lib, ws, h_in, ldh, dhp, ws.dP, pw, pw, N, 1.0, True, st)
+    nchx = _tn(lib, ws, h_in, ld, dhp, ws.dP, pw, pw, N, 1.0, True, st)
     _reduce(lib, ws.partial, nchx, dhp * pw, tp.maps['proj'], flat, st)
     _reduce(lib, ws.colsum, nchx, pw, tp.maps['proj_bias'], flat, st)
     return dh_in, dx_in, ws.dh0, dhe, dx_orig
@@ -334,17 +335,12 @@ class TrainEngine:
 
     # ---- forward with stash -----------------------------------------------------------------------------------------
     def forward(self, graph, log=None):
-        from .rigid_docking_model import _plan_for, _sorted_plan, UnsortedEdges
-        iegmn, dev, lib = self.iegmn, self.device, self.lib
-        plan = _plan_for(graph, dev, iegmn.graph_max_neighbor)
+        iegmn = self.iegmn
         dropout = iegmn.iegmn_layers[0].dropout_now(self.rank) if iegmn.training else None
-        try:
-            return self._forward_plan(graph, plan, log, dropout)
-        except UnsortedEdges:
-            return self._forward_plan(graph, _sorted_plan(graph, dev, iegmn.graph_max_neighbor), log, dropout)
+        return retry_sorted(graph, plan_for(graph, self.device, iegmn.graph_max_neighbor),
+                            lambda plan: self._forward_plan(graph, plan, log, dropout))
 
     def _forward_plan(self, graph, plan, log, dropout=None):
-        from .hetero_graph import LIGAND, RECEPTOR
         iegmn, dev, lib = self.iegmn, self.device, self.lib
         layers = [lay.packed(dev) for lay in iegmn.iegmn_layers]
         head = iegmn.packed_head(dev)
@@ -366,12 +362,6 @@ class TrainEngine:
         return out
 
     # ---- backward -------------------------------------------------------------------------------------------------
-    def _tn(self, ws, X, ldx, K, D, ldd, ncols, nrows, alpha, want_colsum, st):
-        return _tn(self.lib, ws, X, ldx, K, D, ldd, ncols, nrows, alpha, want_colsum, st)
-
-    def _reduce(self, src_t, nch, stride, mp, flat, st):
-        _reduce(self.lib, src_t, nch, stride, mp, flat, st)
-
     def backward(self, fwd, d_coors, d_keypts, d_rot=None, d_trans=None, flat: Optional[torch.Tensor] = None,
                  on_bucket_done=None, capture: Optional[list] = None, d_x_out=None, d_h_out=None,
                  inputs_out: Optional[dict] = None) -> torch.Tensor:
@@ -426,9 +416,9 @@ class TrainEngine:
             if capture is not None:
                 capture.append({'head': True, 'dh': dh_cur.reshape(-1)[:N * 64].clone().view(N, 64), 'dx': dx_cur.clone()})
             hm = self.head_maps()
-            nch = self._tn(ws, fwd['h'], 64, 64, ws.dpre, 64, 64, N, 1.0, True, st)
-            self._reduce(ws.partial, nch, 64 * 64, hm['wm'], flat, st)
-            self._reduce(ws.colsum, nch, 64, hm['bm'], flat, st)
+            nch = _tn(lib, ws, fwd['h'], 64, 64, ws.dpre, 64, 64, N, 1.0, True, st)
+            _reduce(lib, ws.partial, nch, 64 * 64, hm['wm'], flat, st)
+            _reduce(lib, ws.colsum, nch, 64, hm['bm'], flat, st)
             buckets = {lab: (lo, hi) for lab, lo, hi in lay_out.buckets}
             if on_bucket_done:
                 on_bucket_done('head', *buckets['head'])
@@ -461,7 +451,6 @@ class TrainEngine:
             if on_bucket_done:
                 on_bucket_done('emb', *buckets['emb'])
             if inputs_out is not None:
-                from .hetero_graph import LIGAND, RECEPTOR
                 dmu = torch.empty(N, 5, dtype=_f32, device=dev)
                 dx_in = torch.empty(N, 3, dtype=torch.float64, device=dev)
                 mu = [fwd['graph'].nodes[nt].data['mu_r_norm'].detach().to(device=dev, dtype=_f32).contiguous()
@@ -469,11 +458,8 @@ class TrainEngine:
                 nat.check(lib.eqd_bwd_inputs(g, nat.ptr(ws.dh0), nat.ptr(dh_cur), nat.ptr(mu[0]), nat.ptr(mu[1]),
                                              nat.ptr(dx_cur), nat.ptr(dx_orig), nat.ptr(fwd['rotation']), nat.ptr(d_coors),
                                              nat.ptr(dmu), nat.ptr(dx_in), st), 'eqd_bwd_inputs')
-                N_l, E_l = plan.N_l, plan.E_l
-                dhe_l, dhe_r = dhe[:E_l], dhe[E_l:E]
-                if plan.edge_perm is not None:     # the plan holds a destination-sorted copy: sorted edge i = perm[i]
-                    dhe_l = torch.empty_like(dhe_l).index_copy_(0, plan.edge_perm[0].to(dev), dhe_l)
-                    dhe_r = torch.empty_like(dhe_r).index_copy_(0, plan.edge_perm[1].to(dev), dhe_r)
+                N_l = plan.N_l
+                dhe_l, dhe_r = plan.caller_edge_order(dhe)
                 inputs_out.update(x_lig=dx_in[:N_l], x_rec=dx_in[N_l:], mu_lig=dmu[:N_l], mu_rec=dmu[N_l:],
                                   he_lig=dhe_l, he_rec=dhe_r)
         return flat
@@ -579,35 +565,13 @@ class _LayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, holder, x_l, h_l, h0_l, he_l, xo_l, x_r, h_r, h0_r, he_r, xo_r, *params):
         module, plan = holder['module'], holder['plan']
-        dev = x_l.device
-        lib = nat.load()
-        lay = module.packed(dev)
-        layout, tp = layer_train_pack(module, lay, dev)
-        N, dhp = plan.N, lay.dhp
-        f32, f64 = dict(dtype=_f32, device=dev), dict(dtype=torch.float64, device=dev)
-        h = torch.zeros(N, dhp, **f32)
-        h[:, :lay.dh] = torch.cat([h_l, h_r])
-        h0 = torch.zeros(N, nat.H0_PAD, **f32)
-        h0[:, :nat.H0] = torch.cat([h0_l, h0_r])
-        x_in = torch.cat([x_l, x_r]).to(**f64).contiguous()
-        x_orig = torch.cat([xo_l, xo_r]).to(**f64).contiguous()
-        proj = torch.empty(N, 128 + 3 * dhp, **f32)
-        aggr, mu, h_out = torch.empty(N, nat.HID, **f32), torch.empty(N, dhp, **f32), torch.empty(N, nat.HID, **f32)
-        x_out = torch.empty(N, 3, **f64)
-        status = torch.zeros(plan.n_pairs + 1, dtype=torch.int32, device=dev)
+        inputs = (x_l, h_l, h0_l, he_l, xo_l, x_r, h_r, h0_r, he_r, xo_r)
+        lay = module.packed(x_l.device)
+        layout, tp = layer_train_pack(module, lay, x_l.device)
         desc = with_dropout([lay.struct], module.dropout_now())[0]   # each call is its own forward: own seed, layer 0
-        with torch.cuda.device(dev):
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            g, lp = C.byref(plan.struct), C.byref(desc)
-            nat.check(lib.eqd_project(g, lp, nat.ptr(h), dhp, nat.ptr(proj), st), 'eqd_project')
-            nat.check(lib.eqd_iegmn_layer_forward(g, lp, None, nat.ptr(h), dhp, nat.ptr(h0), nat.ptr(x_in),
-                                                  nat.ptr(x_orig), nat.ptr(proj), None, nat.ptr(aggr), nat.ptr(mu),
-                                                  nat.ptr(h_out), nat.ptr(x_out), nat.ptr(status), st),
-                      'eqd_iegmn_layer_forward')
-        if int(status[plan.n_pairs].item()) & nat.STATUS_DEGREE_OVERFLOW:
-            raise nat.NativeLibraryError(f'IEGMN_Layer.forward: in-degree above {plan.struct.max_in_degree}')
+        h, h0, x_in, aggr, mu, h_out, x_out = run_layer(plan, lay, desc, inputs, keep_mu=True)
         ctx.saved = (plan, lay, layout, tp, h, h0, x_in, aggr, mu, desc)
-        ctx.input_meta = [(t.dtype, t.device) for t in (x_l, h_l, h0_l, he_l, xo_l, x_r, h_r, h0_r, he_r, xo_r)]
+        ctx.input_meta = [(t.dtype, t.device) for t in inputs]
         ctx.set_materialize_grads(False)    # a loss on only one of the two outputs launches nothing for the other
         return x_out, h_out
 
@@ -618,7 +582,7 @@ class _LayerFn(torch.autograd.Function):
         if d_x is None and d_h is None:
             return (None,) * (1 + n_in + len(layout.params))
         dev, lib = h.device, nat.load()
-        N, E, N_l, E_l = plan.N, plan.E, plan.N_l, plan.E_l
+        N, E, N_l = plan.N, plan.E, plan.N_l
         need = ctx.needs_input_grad[1:1 + n_in]
         with torch.cuda.device(dev):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
@@ -644,10 +608,7 @@ class _LayerFn(torch.autograd.Function):
                            dx_orig, desc=desc)
             dh0 = ws.dh0[:, :nat.H0].clone() if need[2] or need[7] else None
             if dhe is not None:
-                dhe_l, dhe_r = dhe[:E_l], dhe[E_l:E]
-                if plan.edge_perm is not None:     # the plan holds a destination-sorted copy: sorted edge i = perm[i]
-                    dhe_l = torch.empty_like(dhe_l).index_copy_(0, plan.edge_perm[0].to(dev), dhe_l)
-                    dhe_r = torch.empty_like(dhe_r).index_copy_(0, plan.edge_perm[1].to(dev), dhe_r)
+                dhe_l, dhe_r = plan.caller_edge_order(dhe)
         dh_in = dh_in[:, :lay.dh]
         per_side = {0: dx_in, 1: dh_in, 2: dh0, 4: dx_orig}
         grads = []
