@@ -15,6 +15,8 @@ earlier layers are still being differentiated); ``param.grad`` tensors are views
 from __future__ import annotations
 
 import ctypes as C
+import functools
+from collections import namedtuple
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
@@ -26,6 +28,12 @@ from .engine import (GraphPlan, IEGMNEngine, PackedLayer, _upload_blob, _host_f3
 from .hetero_graph import LIGAND, RECEPTOR
 
 _f32 = torch.float32
+
+
+def _padded(numel: int) -> int:
+    """Floats one parameter takes in a flat buffer: every parameter starts on a 64-float (256-byte) boundary, because
+    the kernels read weights 16 bytes at a time straight from the flat buffer (the index maps are built against it)."""
+    return (numel + 63) & ~63
 
 
 class ParamLayout:
@@ -48,8 +56,7 @@ class ParamLayout:
                 seen.add(id(p))
                 self.entries.append((f'{prefix}{n}', p))
                 self._offs.append(self.total)
-                self.total += (p.numel() + 63) & ~63       # every parameter starts on a 256-byte boundary: the kernels
-                                                           # read weights 16 bytes at a time straight from the flat buffer
+                self.total += _padded(p.numel())
             if self.total > lo:
                 self.buckets.append((label, lo, self.total))
                 self.module_bucket[id(module)] = label
@@ -78,10 +85,77 @@ def _i32(a, device):
     return torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(device)
 
 
+# A weight block: partial [k][c0 + n] -> param [n][k0 + k] (an nn.Linear weight [out][width]), k < rows, n < cols.
+Block = namedtuple('Block', 'param width k0 c0 rows cols')
+# One weight-gradient reduction, launched right after the kernel of its ``stage`` ('node': eqd_bwd_node_mlp, 'edge':
+# eqd_bwd_edge, 'proj': eqd_bwd_project, 'head': eqd_bwd_head_dropout): ws.partial / colsum / vec are reused between
+# stages.  With X, eqd_tn_gemm computes alpha * X^T D over ``rows`` ('N' nodes or 'E' edges) into the row-chunk
+# partials ws.partial [K][ncols] and, when there are ``sums``, the column sums of D into ws.colsum; alpha is the layer's
+# skip_weight_h if ``skip``, else 1.  X and D name a stage operand or a BackwardWorkspace tensor.  Without X, the stage
+# kernel left per-CTA sums in ws.vec, ``ncols`` floats per CTA.  eqd_grad_reduce adds the partials' ``blocks`` and the
+# ``sums`` ((parameter, first column), each covering the whole parameter) into the flat gradient.
+Reduction = namedtuple('Reduction', 'name stage X ldx K D ldd ncols rows blocks sums skip', defaults=((), (), False))
+
+
+@functools.lru_cache(maxsize=None)
+def layer_reductions(dh: int, dhp: int) -> tuple:
+    """The weight-gradient reductions of one IEGMN_Layer of width dh whose node rows are padded to dhp, in launch order
+    (see Reduction).  h_in and mu have row stride dhp, h0 has H0_PAD."""
+    pw = 128 + 3 * dhp                                # projection width: [Psrc | Pdst | Q | K | V]
+    ein, w1n = 2 * dh + 42, 2 * dh + 64 + nat.H0      # input widths of edge_mlp.0 and node_mlp.0
+    R, B, w5 = Reduction, Block, 'node_mlp.0.weight'
+    return (
+        # R(name, stage, X, ldx, K, D, ldd, ncols, rows, blocks, sums): B(param, width, k0, c0, rows, cols), (param, c0)
+        R('nodevec', 'node', None, 0, 0, None, 0, 144, None, (), (('node_mlp.3.weight', 0), ('node_mlp.3.bias', 72))),
+        R('node2', 'node', 'n5', dhp, dhp, 'dh_out', 64, 64, 'N', (B('node_mlp.4.weight', dh, 0, 0, dh, 64),),
+          (('node_mlp.4.bias', 0),), skip=dh == nat.HID),
+        R('node_h', 'node', 'h_in', dhp, dhp, 'du', dhp, dhp, 'N', (B(w5, w1n, 0, 0, dh, dh),),
+          (('node_mlp.0.bias', 0),)),
+        R('node_aggr', 'node', 'aggr', 64, 64, 'du', dhp, dhp, 'N', (B(w5, w1n, dh, 0, 64, dh),)),
+        R('node_mu', 'node', 'mu', dhp, dhp, 'du', dhp, dhp, 'N', (B(w5, w1n, dh + 64, 0, dh, dh),)),
+        R('node_h0', 'node', 'h0', nat.H0_PAD, nat.H0_PAD, 'du', dhp, dhp, 'N',
+          (B(w5, w1n, 2 * dh + 64, 0, nat.H0, dh),)),
+        R('edgevec', 'edge', None, 0, 0, None, 0, 256, None, (),
+          (('edge_mlp.3.weight', 0), ('edge_mlp.3.bias', 64), ('coors_mlp.4.weight', 128), ('coors_mlp.4.bias', 192))),
+        R('edge1', 'edge', 'ein', 44, 44, 'dz1', 64, 64, 'E', (B('edge_mlp.0.weight', ein, 2 * dh, 0, 42, 64),)),
+        R('edge2', 'edge', 'n1', 64, 64, 'dmsg', 64, 64, 'E', (B('edge_mlp.4.weight', 64, 0, 0, 64, 64),),
+          (('edge_mlp.4.bias', 0),)),
+        R('edge3', 'edge', 'msg', 64, 64, 'dz3', 64, 64, 'E', (B('coors_mlp.0.weight', 64, 0, 0, 64, 64),),
+          (('coors_mlp.0.bias', 0),)),
+        R('proj', 'proj', 'h_in', dhp, dhp, 'dP', pw, pw, 'N',
+          (B('edge_mlp.0.weight', ein, 0, 0, dh, 64), B('edge_mlp.0.weight', ein, dh, 64, dh, 64),
+           B('att_mlp_Q.0.weight', dh, 0, 128, dh, dh), B('att_mlp_K.0.weight', dh, 0, 128 + dhp, dh, dh),
+           B('att_mlp_V.0.weight', dh, 0, 128 + 2 * dhp, dh, dh)),
+          (('edge_mlp.0.bias', 64),)),
+    )
+
+
+HEAD_REDUCTION = Reduction('head', 'head', 'h', 64, 64, 'dpre', 64, 64, 'N',
+                           (Block('iegmn_original.mlp_h_mean_ROT.0.weight', 64, 0, 0, 64, 64),),
+                           (('iegmn_original.mlp_h_mean_ROT.0.bias', 0),))
+
+
+def _block_map(off: int, b: Block, ncols: int):
+    k, n = np.meshgrid(np.arange(b.rows), np.arange(b.cols), indexing='ij')     # k = input feature, n = output unit
+    return (k * ncols + b.c0 + n).reshape(-1), (off + n * b.width + b.k0 + k).reshape(-1)
+
+
+def reduction_maps(table, named_params, layout, device) -> Dict[str, tuple]:
+    """{reduction name: (blocks map, sums map)} of the reductions in ``table``: each map is the (source index,
+    destination index) int32 pair eqd_grad_reduce reads (partial, colsum or vec -> flat gradient at ``layout.offset``),
+    or None.  ``named_params`` yields the (name, parameter) pairs the table's names refer to."""
+    params = dict(named_params)
+    off = lambda name: layout.offset[id(params[name])]
+    span = lambda name: np.arange(params[name].numel())
+    join = lambda pieces: tuple(_i32(np.concatenate(a), device) for a in zip(*pieces)) if pieces else None
+    return {r.name: (join([_block_map(off(b.param), b, r.ncols) for b in r.blocks]),
+                     join([(c0 + span(p), off(p) + span(p)) for p, c0 in r.sums])) for r in table}
+
+
 class LayerTrainPack:
     """Backward-side tensors of one IEGMN_Layer module: the nn.Linear-layout weight panels the data-gradient GEMMs
     read, and the (source index, destination index) maps of every weight-gradient reduction (packed k-major partial ->
-    flat state_dict-layout gradient)."""
+    flat state_dict-layout gradient).  The maps depend on the layout only: ``maps`` passes those of an earlier pack."""
 
     def __init__(self, layer_module, packed: PackedLayer, layout: ParamLayout, device, maps=None):
         dh, dhp = packed.dh, packed.dhp
@@ -101,65 +175,15 @@ class LayerTrainPack:
                                'w2lin': sd['edge_mlp.4.weight'].contiguous(),
                                'w3lin': sd['coors_mlp.0.weight'].contiguous()}, device)
         self.dh, self.dhp, self.pw = dh, dhp, pw
-        if maps is not None:           # the index maps depend on the layout only: built once per module
-            self.maps = maps
-            return
-        off = {n: layout.offset[id(p)] for n, p in layer_module.named_parameters()}
-        ein = 2 * dh + 42
-        w1n = 2 * dh + 64 + nat.H0            # node_mlp.0 input width
-        kk, nn = np.meshgrid(np.arange(dh), np.arange(64), indexing='ij')     # k = input feature, n = output unit
-
-        def m(src, dst):
-            return _i32(np.asarray(src).reshape(-1), device), _i32(np.asarray(dst).reshape(-1), device)
-
-        maps = {}
-        # (a) projections: partial [dhp][pw], colsum [pw]
-        src, dst = [], []
-        src.append(kk * pw + nn); dst.append(off['edge_mlp.0.weight'] + nn * ein + kk)                  # Psrc block
-        src.append(kk * pw + 64 + nn); dst.append(off['edge_mlp.0.weight'] + nn * ein + dh + kk)        # Pdst block
-        k2, c2 = np.meshgrid(np.arange(dh), np.arange(dh), indexing='ij')
-        for gi, name in enumerate(('att_mlp_Q.0.weight', 'att_mlp_K.0.weight', 'att_mlp_V.0.weight')):
-            src.append(k2 * pw + 128 + gi * dhp + c2); dst.append(off[name] + c2 * dh + k2)
-        maps['proj'] = m(np.concatenate([a.reshape(-1) for a in src]), np.concatenate([a.reshape(-1) for a in dst]))
-        maps['proj_bias'] = m(64 + np.arange(64), off['edge_mlp.0.bias'] + np.arange(64))
-        # (b) edge GEMM1: partial [44][64]
-        k42, n64 = np.meshgrid(np.arange(42), np.arange(64), indexing='ij')
-        maps['edge1'] = m(k42 * 64 + n64, off['edge_mlp.0.weight'] + n64 * ein + 2 * dh + k42)
-        k64, n64b = np.meshgrid(np.arange(64), np.arange(64), indexing='ij')
-        maps['edge2'] = m(k64 * 64 + n64b, off['edge_mlp.4.weight'] + n64b * 64 + k64)
-        maps['edge2_bias'] = m(np.arange(64), off['edge_mlp.4.bias'] + np.arange(64))
-        maps['edge3'] = m(k64 * 64 + n64b, off['coors_mlp.0.weight'] + n64b * 64 + k64)
-        maps['edge3_bias'] = m(np.arange(64), off['coors_mlp.0.bias'] + np.arange(64))
-        maps['edgevec'] = m(np.concatenate([np.arange(64), 64 + np.arange(64), 128 + np.arange(64), [192]]),
-                            np.concatenate([off['edge_mlp.3.weight'] + np.arange(64), off['edge_mlp.3.bias'] + np.arange(64),
-                                            off['coors_mlp.4.weight'] + np.arange(64), [off['coors_mlp.4.bias']]]))
-        # node MLP layer 1: four TN products against du [N][dhp] -> partial [K][dhp]
-        kh, nh = np.meshgrid(np.arange(dh), np.arange(dh), indexing='ij')
-        maps['node_h'] = m(kh * dhp + nh, off['node_mlp.0.weight'] + nh * w1n + kh)
-        ka, na = np.meshgrid(np.arange(64), np.arange(dh), indexing='ij')
-        maps['node_aggr'] = m(ka * dhp + na, off['node_mlp.0.weight'] + na * w1n + dh + ka)
-        maps['node_mu'] = m(kh * dhp + nh, off['node_mlp.0.weight'] + nh * w1n + dh + 64 + kh)
-        k0, n0 = np.meshgrid(np.arange(nat.H0), np.arange(dh), indexing='ij')
-        maps['node_h0'] = m(k0 * dhp + n0, off['node_mlp.0.weight'] + n0 * w1n + 2 * dh + 64 + k0)
-        maps['node1_bias'] = m(np.arange(dh), off['node_mlp.0.bias'] + np.arange(dh))
-        kn, nn2 = np.meshgrid(np.arange(dh), np.arange(64), indexing='ij')
-        maps['node2'] = m(kn * 64 + nn2, off['node_mlp.4.weight'] + nn2 * dh + kn)
-        maps['node2_bias'] = m(np.arange(64), off['node_mlp.4.bias'] + np.arange(64))
-        maps['nodevec'] = m(np.concatenate([np.arange(dh), 72 + np.arange(dh)]),
-                            np.concatenate([off['node_mlp.3.weight'] + np.arange(dh), off['node_mlp.3.bias'] + np.arange(dh)]))
-        self.maps = maps
+        self.reductions = layer_reductions(dh, dhp)
+        self.maps = maps or reduction_maps(self.reductions, layer_module.named_parameters(), layout, device)
 
 
 def tn_gemm_shapes(N: int, E: int, dhps: Sequence[int] = (nat.H0_PAD, nat.HID)) -> List[tuple]:
     """Every (rows, K, ncols) that TrainEngine.backward passes to eqd_tn_gemm, for a batch of N nodes and E edges whose
     layers have the padded widths ``dhps`` (72 for the 69-wide layer 0, 64 for the others)."""
-    shapes = [(N, 64, 64)]                                   # head: mlp_h_mean_ROT.0 (h, dpre)
-    for dhp in dhps:
-        shapes += [(N, dhp, 64),                             # node_mlp.4 (n5, dh')
-                   (N, dhp, dhp), (N, 64, dhp), (N, nat.H0_PAD, dhp),   # node_mlp.0: h and mu | aggr | h0 blocks (du)
-                   (N, dhp, 128 + 3 * dhp),                  # projections: edge_mlp.0 node blocks, att_mlp_Q/K/V (h, dP)
-                   (E, 44, 64), (E, 64, 64)]                 # edge_mlp.0 [he | rbf] block, edge_mlp.4, coors_mlp.0
-    return sorted(set(shapes))
+    table = [HEAD_REDUCTION] + [r for dhp in dhps for r in layer_reductions(nat.HID if dhp == nat.HID else nat.H0, dhp)]
+    return sorted({(N if r.rows == 'N' else E, r.K, r.ncols) for r in table if r.X is not None})
 
 
 def tn_workspace_floats(N: int, E: int, dhps: Sequence[int] = (nat.H0_PAD, nat.HID)) -> tuple:
@@ -207,23 +231,31 @@ def _vp(t):
     return t if t is None or isinstance(t, C.c_void_p) else nat.ptr(t)
 
 
-def _tn(lib, ws, X, ldx, K, D, ldd, ncols, nrows, alpha, want_colsum, st):
-    nch = C.c_int32(0)
-    nat.check(lib.eqd_tn_gemm(_vp(X), ldx, K, _vp(D), ldd, ncols, nrows, alpha, nat.ptr(ws.partial),
-                              nat.ptr(ws.colsum) if want_colsum else None, C.byref(nch), st), 'eqd_tn_gemm')
-    return nch.value
-
-
-def _reduce(lib, src_t, nch, stride, mp, flat, st):
-    nat.check(lib.eqd_grad_reduce(nat.ptr(src_t), nch, stride, nat.ptr(mp[0]), nat.ptr(mp[1]), int(mp[0].numel()),
-                                  nat.ptr(flat), st), 'eqd_grad_reduce')
+def _weight_grads(lib, ws, table, maps, stage, operands, N, E, flat, st, nparts=0, skip_weight_h=1.0):
+    """Launches the reductions of ``table`` that follow ``stage``, in table order (see Reduction).  ``operands`` holds
+    the stage's named operands that are not BackwardWorkspace tensors; ``nparts`` is the number of per-CTA sums in
+    ws.vec."""
+    opd = lambda name: _vp(operands[name] if name in operands else getattr(ws, name))
+    partial, colsum, vec, grad = nat.ptr(ws.partial), nat.ptr(ws.colsum), nat.ptr(ws.vec), nat.ptr(flat)
+    for r in table:
+        if r.stage != stage:
+            continue
+        nch = C.c_int32(nparts)          # partial sums per element: eqd_tn_gemm sets its row-chunk count
+        if r.X is not None:
+            nat.check(lib.eqd_tn_gemm(opd(r.X), r.ldx, r.K, opd(r.D), r.ldd, r.ncols, N if r.rows == 'N' else E,
+                                      skip_weight_h if r.skip else 1.0, partial, colsum if r.sums else None,
+                                      C.byref(nch), st), 'eqd_tn_gemm')
+        for src, stride, mp in zip((partial, colsum if r.X else vec), (r.K * r.ncols, r.ncols), maps[r.name]):
+            if mp is not None:
+                nat.check(lib.eqd_grad_reduce(src, nch.value, stride, nat.ptr(mp[0]), nat.ptr(mp[1]),
+                                              int(mp[0].numel()), grad, st), 'eqd_grad_reduce')
 
 
 def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack, ws: BackwardWorkspace, h_in, x_in, aggr,
                    mu, h0, dh_out, dx_out, dh_in, dx_in, flat, st, dhe=None, dx_orig=None, capture=None, li=None, desc=None):
     """Backward of ONE IEGMN_Layer, the fixed kernel sequence eqd_project (recompute) -> eqd_bwd_node_mlp ->
     eqd_bwd_attention -> eqd_bwd_edge -> (eqd_bwd_layer_inputs) -> eqd_bwd_edge_gather -> eqd_bwd_project, with the weight
-    gradients of each stage through eqd_tn_gemm + eqd_grad_reduce.
+    gradients of each stage through eqd_tn_gemm + eqd_grad_reduce (``tp.reductions``, see layer_reductions).
 
     The layer's stashed inputs (tensors or device pointers): h_in [N][dhp] f32 (row stride 72 for the 69-wide layer 0,
     else 64), x_in [N][3] f64, aggr [N][64] f32, mu [N][dhp] f32, h0 [N][72] f32.  Upstream gradients: dh_out [N][64] f32
@@ -239,24 +271,15 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
     dh, dhp, pw = tp.dh, tp.dhp, tp.pw
     ld = nat.H0_PAD if dh == nat.H0 else nat.HID     # row stride of h_in and of mu
     h_in, x_in, aggr, mu, h0 = _vp(h_in), _vp(x_in), _vp(aggr), _vp(mu), _vp(h0)
+    ops = {'h_in': h_in, 'aggr': aggr, 'mu': mu, 'h0': h0, 'dh_out': dh_out}
     nat.check(lib.eqd_project(g, lp, h_in, ld, nat.ptr(ws.proj), st), 'eqd_project')
     nparts = C.c_int32(0)
     nat.check(lib.eqd_bwd_node_mlp(g, lp, nat.ptr(tp.t['w_node1_lin']), nat.ptr(tp.t['w_node2_lin']), h_in, ld,
                                    aggr, mu, ld, h0, nat.ptr(dh_out), nat.ptr(dh_in), nat.ptr(ws.daggr),
                                    nat.ptr(ws.dmu), nat.ptr(ws.dh0), nat.ptr(ws.n5), nat.ptr(ws.du),
                                    nat.ptr(ws.vec), C.byref(nparts), st), 'eqd_bwd_node_mlp')
-    _reduce(lib, ws.vec, nparts.value, 144, tp.maps['nodevec'], flat, st)
-    # node MLP weight gradients
-    sk = float(lp_obj.struct.dev.skip_weight_h) if dh == nat.HID else 1.0
-    nch = _tn(lib, ws, ws.n5, dhp, dhp, dh_out, 64, 64, N, sk, True, st)
-    _reduce(lib, ws.partial, nch, dhp * 64, tp.maps['node2'], flat, st)
-    _reduce(lib, ws.colsum, nch, 64, tp.maps['node2_bias'], flat, st)
-    for name, X, ldx, K, want in (('node_h', h_in, ld, dhp, True), ('node_aggr', aggr, 64, 64, False),
-                                  ('node_mu', mu, ld, dhp, False), ('node_h0', h0, nat.H0_PAD, nat.H0_PAD, False)):
-        nchx = _tn(lib, ws, X, ldx, K, ws.du, dhp, dhp, N, 1.0, want, st)
-        _reduce(lib, ws.partial, nchx, K * dhp, tp.maps[name], flat, st)
-        if want:
-            _reduce(lib, ws.colsum, nchx, dhp, tp.maps['node1_bias'], flat, st)
+    _weight_grads(lib, ws, tp.reductions, tp.maps, 'node', ops, N, E, flat, st, nparts.value,
+                  float(lp_obj.struct.dev.skip_weight_h))
     nat.check(lib.eqd_bwd_attention(g, lp, nat.ptr(ws.proj), mu, ld, nat.ptr(ws.dmu), nat.ptr(ws.dP),
                                     nat.ptr(ws.rowstat), st), 'eqd_bwd_attention')
     nat.check(lib.eqd_bwd_edge(g, lp, nat.ptr(tp.t['w2lin']), nat.ptr(tp.t['w3lin']), nat.ptr(ws.proj), x_in,
@@ -266,15 +289,7 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
     if dhe is not None:
         nat.check(lib.eqd_bwd_layer_inputs(g, lp, nat.ptr(ws.dz1), nat.ptr(dx_out), nat.ptr(dhe),
                                            nat.ptr(dx_orig), st), 'eqd_bwd_layer_inputs')
-    _reduce(lib, ws.vec, nparts.value, 256, tp.maps['edgevec'], flat, st)
-    nch = _tn(lib, ws, ws.ein, 44, 44, ws.dz1, 64, 64, E, 1.0, False, st)
-    _reduce(lib, ws.partial, nch, 44 * 64, tp.maps['edge1'], flat, st)
-    nch = _tn(lib, ws, ws.n1, 64, 64, ws.dmsg, 64, 64, E, 1.0, True, st)
-    _reduce(lib, ws.partial, nch, 64 * 64, tp.maps['edge2'], flat, st)
-    _reduce(lib, ws.colsum, nch, 64, tp.maps['edge2_bias'], flat, st)
-    nch = _tn(lib, ws, ws.msg, 64, 64, ws.dz3, 64, 64, E, 1.0, True, st)
-    _reduce(lib, ws.partial, nch, 64 * 64, tp.maps['edge3'], flat, st)
-    _reduce(lib, ws.colsum, nch, 64, tp.maps['edge3_bias'], flat, st)
+    _weight_grads(lib, ws, tp.reductions, tp.maps, 'edge', ops, N, E, flat, st, nparts.value)
     nat.check(lib.eqd_bwd_edge_gather(g, nat.ptr(ws.out_ptr), nat.ptr(ws.out_edge), nat.ptr(ws.dz1),
                                       nat.ptr(ws.dxrel), nat.ptr(dx_out), float(lp_obj.struct.dev.x_connection_init),
                                       nat.ptr(ws.dP), pw, nat.ptr(dx_in), st), 'eqd_bwd_edge_gather')
@@ -287,9 +302,7 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
               'eqd_bwd_project')
     if capture is not None:
         capture[-1]['dh'] = dh_in.reshape(-1)[:N * dhp].clone().view(N, dhp)
-    nchx = _tn(lib, ws, h_in, ld, dhp, ws.dP, pw, pw, N, 1.0, True, st)
-    _reduce(lib, ws.partial, nchx, dhp * pw, tp.maps['proj'], flat, st)
-    _reduce(lib, ws.colsum, nchx, pw, tp.maps['proj_bias'], flat, st)
+    _weight_grads(lib, ws, tp.reductions, tp.maps, 'proj', ops, N, E, flat, st)
     return dh_in, dx_in, ws.dh0, dhe, dx_orig
 
 
@@ -307,7 +320,7 @@ class TrainEngine:
         self._packs: Dict[int, tuple] = {}
         self._maps: Dict[int, dict] = {}
         self._ws: Optional[BackwardWorkspace] = None
-        self._head_maps = None
+        self._head_maps = reduction_maps((HEAD_REDUCTION,), self.layout.entries, self.layout, self.device)
         self.rank = 0        # data-parallel rank: an input of the dropout masks (DataParallelTrainer sets it)
 
     # ---- packs ----------------------------------------------------------------------------------------------------
@@ -321,17 +334,6 @@ class TrainEngine:
             hit = (packed, tp)
             self._packs[id(lay_module)] = hit
         return hit[1]
-
-    def head_maps(self):
-        if self._head_maps is None:
-            off = self.layout.name_offset
-            k, n = np.meshgrid(np.arange(64), np.arange(64), indexing='ij')
-            self._head_maps = {
-                'wm': (_i32((k * 64 + n).reshape(-1), self.device),
-                       _i32((off['iegmn_original.mlp_h_mean_ROT.0.weight'] + n * 64 + k).reshape(-1), self.device)),
-                'bm': (_i32(np.arange(64), self.device),
-                       _i32(off['iegmn_original.mlp_h_mean_ROT.0.bias'] + np.arange(64), self.device))}
-        return self._head_maps
 
     # ---- forward with stash -----------------------------------------------------------------------------------------
     def forward(self, graph, log=None):
@@ -415,10 +417,7 @@ class TrainEngine:
                 dx_orig = torch.zeros(N, 3, dtype=torch.float64, device=dev)
             if capture is not None:
                 capture.append({'head': True, 'dh': dh_cur.reshape(-1)[:N * 64].clone().view(N, 64), 'dx': dx_cur.clone()})
-            hm = self.head_maps()
-            nch = _tn(lib, ws, fwd['h'], 64, 64, ws.dpre, 64, 64, N, 1.0, True, st)
-            _reduce(lib, ws.partial, nch, 64 * 64, hm['wm'], flat, st)
-            _reduce(lib, ws.colsum, nch, 64, hm['bm'], flat, st)
+            _weight_grads(lib, ws, (HEAD_REDUCTION,), self._head_maps, 'head', {'h': fwd['h']}, N, E, flat, st)
             buckets = {lab: (lo, hi) for lab, lo, hi in lay_out.buckets}
             if on_bucket_done:
                 on_bucket_done('head', *buckets['head'])
@@ -536,7 +535,7 @@ class LayerLayout:
         for p in layer_module.parameters():
             self.offset[id(p)] = self.total
             self.params.append(p)
-            self.total += (p.numel() + 63) & ~63
+            self.total += _padded(p.numel())
 
     views = ParamLayout.views
 
@@ -547,7 +546,7 @@ def layer_train_pack(layer_module, packed: PackedLayer, device):
     hit = getattr(layer_module, '_eqd_layer_train', None)
     if hit is not None and hit[0] is packed:
         return hit[1], hit[2]
-    if hit is not None and hit[2].maps['proj'][0].device == torch.device(device):
+    if hit is not None and hit[2].maps['proj'][0][0].device == torch.device(device):
         layout, maps = hit[1], hit[2].maps
     else:
         layout, maps = LayerLayout(layer_module), None
