@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # EQD_LIB_PATH: load another build of the same ABI instead (A/B runs of kernel variants, scripts/forward_ab.py)
 LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.so')
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
@@ -58,10 +58,15 @@ def dropout_descriptor(p: float, seed: int, layer: int, rank: int = 0) -> EqdDro
     return d
 
 
+class EqdLayerNorms(C.Structure):
+    """eqd_layer_norms: device pointers of the optional LayerNorms of a layer (NULL = off)."""
+    _fields_ = [('coors_ln_g', _vp), ('coors_ln_b', _vp), ('final_ln_g', _vp), ('final_ln_b', _vp)]
+
+
 class EqdLayer(C.Structure):
     """eqd_layer: what the entry points take -- `dev` (device pointers + scalars, passed to kernels by value) + `consts`,
-    and `dropout` (training-mode dropout; zero = off)."""
-    _fields_ = [('dev', EqdLayerParams), ('consts', EqdLayerConsts), ('dropout', EqdDropout)]
+    `dropout` (training-mode dropout; zero = off) and `norms` (optional LayerNorms; NULL = off)."""
+    _fields_ = [('dev', EqdLayerParams), ('consts', EqdLayerConsts), ('dropout', EqdDropout), ('norms', EqdLayerNorms)]
 
 
 class EqdForwardIO(C.Structure):

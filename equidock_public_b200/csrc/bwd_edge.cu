@@ -36,17 +36,22 @@ struct EdgeBwdSmem {
   double dxm[EQD_TM * 3];
   float phi[EQD_TM], dphi[EQD_TM], rstd[EQD_TM], invdeg[EQD_TM];
   int src[EQD_TM], dst[EQD_TM];
+  float cln_g[64], cln_b[64];   // coors_mlp.3 (CLN only)
 };
 
 // DROP: the forward applied dropout sites 0 / 1 of `dr` to z1 / z3; the same masks and scale enter the chain rule
 // (dz = d(dropout output) * mask * scale).
-template <bool DROP>
+// CLN: the forward ran the coordinate LayerNorm coors_mlp.3 of `nm` on c3 = lrelu(z3): n3 and its statistics are recomputed,
+// phi = w4 . n3 + b4, dw4 += n3 dphi, dn3 = dphi w4, dgamma_c += dn3 n-hat_c, dbeta_c += dn3, LayerNorm backward -> dc3,
+// dz3 = dc3 lrelu'(z3).  Its per-CTA partials take 384 floats instead of 256.
+template <bool DROP, bool CLN>
 __global__ void __launch_bounds__(EQD_THREADS)
 bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin, const float* __restrict__ w3lin,
                 const float* __restrict__ proj, const double* __restrict__ x_in, const float* __restrict__ daggr,
                 const double* __restrict__ dx_out, float* __restrict__ ein_out, float* __restrict__ n1_out,
                 float* __restrict__ msg_out, float* __restrict__ dz3_out, float* __restrict__ dmsg_out,
-                float* __restrict__ dz1_out, double* __restrict__ dxrel_out, float* __restrict__ vec_partial, eqd_dropout dr) {
+                float* __restrict__ dz1_out, double* __restrict__ dxrel_out, float* __restrict__ vec_partial, eqd_dropout dr,
+                eqd_layer_norms nm) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   EdgeBwdSmem& s = *reinterpret_cast<EdgeBwdSmem*>(smem_raw);
   const int tid = threadIdx.x, ty = tid >> 3, tx = tid & 7;
@@ -67,10 +72,15 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
     s.b3[tid] = p.b_coor1[tid];
     s.w4[tid] = p.w_coor2[tid];
   }
+  if (CLN && tid < 64) {
+    s.cln_g[tid] = nm.coors_ln_g[tid];
+    s.cln_b[tid] = nm.coors_ln_b[tid];
+  }
   __syncthreads();
   float gsum[8], bsum[8], w4sum[8], b4sum = 0.f;
+  float cgsum[8], cbsum[8];   // CLN: d coors_mlp.3.weight / .bias
 #pragma unroll
-  for (int j = 0; j < 8; ++j) gsum[j] = bsum[j] = w4sum[j] = 0.f;
+  for (int j = 0; j < 8; ++j) gsum[j] = bsum[j] = w4sum[j] = cgsum[j] = cbsum[j] = 0.f;
 
   const int E = g.n_edges;
   const int ntiles = (E + EQD_TM - 1) / EQD_TM;
@@ -215,13 +225,51 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
         const int r = ty * 8 + i;
         const float dph = s.dphi[r];
         float v = 0.f;
+        if (CLN) {   // LayerNorm statistics in the order of the forward's lrelu_layernorm
+          float c3[8], sum = 0.f;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float c3 = lrelu(acc[i][j], slope);
-          v = fmaf(c3, w4r[j], v);
-          w4sum[j] = fmaf(c3, dph, w4sum[j]);
-          acc[i][j] = dph * w4r[j] * lrelu_grad_from_post(c3, slope);     // dz3
-          if (DROP) acc[i][j] *= keep[i][j];
+          for (int j = 0; j < 8; ++j) {
+            c3[j] = lrelu(acc[i][j], slope);
+            sum += c3[j];
+          }
+          const float mean = row_sum8(sum) * (1.f / 64.f);
+          float q = 0.f;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float d = c3[j] - mean;
+            q = fmaf(d, d, q);
+          }
+          const float rstd = 1.f / sqrtf(row_sum8(q) * (1.f / 64.f) + 1e-5f);
+          float nhat[8], dnh[8], s1 = 0.f, s2 = 0.f;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int c = col_nn(tx, j);
+            nhat[j] = (c3[j] - mean) * rstd;
+            const float n3 = nhat[j] * s.cln_g[c] + s.cln_b[c];
+            v = fmaf(n3, w4r[j], v);
+            w4sum[j] = fmaf(n3, dph, w4sum[j]);
+            const float dn3 = dph * w4r[j];
+            cgsum[j] = fmaf(dn3, nhat[j], cgsum[j]);
+            cbsum[j] += dn3;
+            dnh[j] = dn3 * s.cln_g[c];
+            s1 += dnh[j];
+            s2 = fmaf(dnh[j], nhat[j], s2);
+          }
+          const float m1 = row_sum8(s1) * (1.f / 64.f), m2 = row_sum8(s2) * (1.f / 64.f);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            acc[i][j] = rstd * (dnh[j] - m1 - nhat[j] * m2) * lrelu_grad_from_post(c3[j], slope);   // dz3
+            if (DROP) acc[i][j] *= keep[i][j];
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float c3 = lrelu(acc[i][j], slope);
+            v = fmaf(c3, w4r[j], v);
+            w4sum[j] = fmaf(c3, dph, w4sum[j]);
+            acc[i][j] = dph * w4r[j] * lrelu_grad_from_post(c3, slope);     // dz3
+            if (DROP) acc[i][j] *= keep[i][j];
+          }
         }
         v = row_sum8(v);
         if (tx == 0) s.phi[r] = v + p.b_coor2;
@@ -315,11 +363,15 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
     }
     __syncthreads();
   }
-  // per-CTA partials: [0:64) dgamma, [64:128) dbeta, [128:192) dw4, [192] db4
-  float* vp = vec_partial + (long)blockIdx.x * 256;
+  // per-CTA partials: [0:64) dgamma, [64:128) dbeta, [128:192) dw4, [192] db4; CLN: [256:320) dgamma_c, [320:384) dbeta_c
+  float* vp = vec_partial + (long)blockIdx.x * (CLN ? 384 : 256);
   colacc8_flush(gsum, s.scratch, vp, tid);
   colacc8_flush(bsum, s.scratch, vp + 64, tid);
   colacc8_flush(w4sum, s.scratch, vp + 128, tid);
+  if (CLN) {
+    colacc8_flush(cgsum, s.scratch, vp + 256, tid);
+    colacc8_flush(cbsum, s.scratch, vp + 320, tid);
+  }
   s.scratch[tid] = b4sum;
   __syncthreads();
   if (tid == 0) {
@@ -327,6 +379,20 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
     for (int q = 0; q < EQD_THREADS; ++q) t += s.scratch[q];
     vp[192] = t;
   }
+}
+
+template <bool DROP, bool CLN>
+static int launch_bwd_edge(const eqd_graph* g, const eqd_layer* p_l, const float* w2lin, const float* w3lin,
+                           const float* proj, const double* x_in, const float* daggr, const double* dx_out, float* ein_out,
+                           float* n1_out, float* msg_out, float* dz3_out, float* dmsg_out, float* dz1_out, double* dxrel_out,
+                           float* vec_partial, int grid, void* stream) {
+  const size_t smem = sizeof(EdgeBwdSmem);
+  EQD_SET_SMEM((bwd_edge_kernel<DROP, CLN>), smem);
+  bwd_edge_kernel<DROP, CLN><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(
+      *g, p_l->dev, w2lin, w3lin, proj, x_in, daggr, dx_out, ein_out, n1_out, msg_out, dz3_out, dmsg_out, dz1_out, dxrel_out,
+      vec_partial, p_l->dropout, p_l->norms);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
 }
 
 // One warp per node; lane l owns channels 2l, 2l+1 of dPsrc / dPdst and (lanes 0..2) one coordinate.
@@ -367,25 +433,19 @@ extern "C" int eqd_bwd_edge(const eqd_graph* g, const eqd_layer* p_l, const floa
   if (!g || !p || !w2lin || !w3lin || !proj || !x_in || !daggr || !dx_out || !ein_out || !n1_out || !msg_out || !dz3_out ||
       !dmsg_out || !dz1_out || !dxrel_out || !vec_partial)
     return EQD_ERR_BAD_ARG;
+  const int cln = eqd_coors_ln(p_l);
+  if (cln < 0) return EQD_ERR_BAD_ARG;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;
   const int ntiles = (g->n_edges + EQD_TM - 1) / EQD_TM;
   int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   if (n_partials_out) *n_partials_out = grid > 0 ? grid : 0;
   if (g->n_edges <= 0) return EQD_OK;
-  size_t smem = sizeof(eqd::EdgeBwdSmem);
-  if (p_l->dropout.p > 0.f) {
-    EQD_SET_SMEM((eqd::bwd_edge_kernel<true>), smem);
-    eqd::bwd_edge_kernel<true><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(
-        *g, *p, w2lin, w3lin, proj, x_in, daggr, dx_out, ein_out, n1_out, msg_out, dz3_out, dmsg_out, dz1_out, dxrel_out,
-        vec_partial, p_l->dropout);
-  } else {
-    EQD_SET_SMEM((eqd::bwd_edge_kernel<false>), smem);
-    eqd::bwd_edge_kernel<false><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(
-        *g, *p, w2lin, w3lin, proj, x_in, daggr, dx_out, ein_out, n1_out, msg_out, dz3_out, dmsg_out, dz1_out, dxrel_out,
-        vec_partial, p_l->dropout);
-  }
-  EQD_CUDA_LAUNCH_CHECK();
-  return EQD_OK;
+  const bool drop = p_l->dropout.p > 0.f;
+#define EQD_BWD_EDGE_ARGS g, p_l, w2lin, w3lin, proj, x_in, daggr, dx_out, ein_out, n1_out, msg_out, dz3_out, dmsg_out, \
+                          dz1_out, dxrel_out, vec_partial, grid, stream
+  if (cln) return drop ? eqd::launch_bwd_edge<true, true>(EQD_BWD_EDGE_ARGS) : eqd::launch_bwd_edge<false, true>(EQD_BWD_EDGE_ARGS);
+  return drop ? eqd::launch_bwd_edge<true, false>(EQD_BWD_EDGE_ARGS) : eqd::launch_bwd_edge<false, false>(EQD_BWD_EDGE_ARGS);
+#undef EQD_BWD_EDGE_ARGS
 }
 
 extern "C" int eqd_bwd_edge_gather(const eqd_graph* g, const int32_t* out_ptr, const int32_t* out_edge, const float* dz1,

@@ -22,7 +22,11 @@ struct NodeBwdCfg {
 };
 
 // DROP: the forward applied dropout site 2 of `dr` to u5; du = d(dropout output) * mask * scale.
-template <bool EXTRA, bool DROP>
+// HLN: the forward applied the final feature LayerNorm (eqd_layer_norms `nm`) to y = skip(node_mlp.4(n5)).  y is recomputed
+// from n5 (one 64 x 64 product per tile), dh_out (the gradient w.r.t. LN_f(y)) goes through the LayerNorm backward into dy,
+// which replaces dh_out in place (dy_io, the same rows) for the rest of the tile and for the node_mlp.4 reductions; the
+// per-CTA partials grow from 144 to 272 floats ([144:208) d final_h_layernorm_layer.weight, [208:272) .bias).
+template <bool EXTRA, bool DROP, bool HLN>
 __global__ void __launch_bounds__(EQD_THREADS)
 bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w_node1_lin /*[dhp][2dhp+136]*/,
                     const float* __restrict__ w_node2_lin /*[64][dhp]*/, const float* __restrict__ h_in, int ldh,
@@ -30,7 +34,7 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
                     const float* __restrict__ h0, const float* __restrict__ dh_out, float* __restrict__ dh_in,
                     float* __restrict__ daggr, float* __restrict__ dmu, float* __restrict__ dh0_acc,
                     float* __restrict__ n5_out, float* __restrict__ du_out, float* __restrict__ vec_partial,
-                    eqd_dropout dr) {
+                    eqd_dropout dr, eqd_layer_norms nm, float* dy_io) {
   using C = NodeBwdCfg<EXTRA>;
   constexpr int DHP = C::DHP, LD = C::LD;
   extern __shared__ __align__(16) float smem[];
@@ -47,8 +51,10 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
   const float sk = skip ? p.skip_weight_h : 1.f;
   const bool xvalid = EXTRA && (64 + tx < p.dh);
   float gsum[8], bsum[8], gsumx = 0.f, bsumx = 0.f;
+  float fgsum[8], fbsum[8];   // HLN: d final_h_layernorm_layer.weight / .bias
 #pragma unroll
-  for (int j = 0; j < 8; ++j) gsum[j] = bsum[j] = 0.f;
+  for (int j = 0; j < 8; ++j) gsum[j] = bsum[j] = fgsum[j] = fbsum[j] = 0.f;
+  const float* dsrc = HLN ? dy_io : dh_out;   // the gradient w.r.t. y once the final LayerNorm is undone
 
   const int ntiles = (n_nodes + EQD_TM - 1) / EQD_TM;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -120,6 +126,19 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
       if (EXTRA) accx[i] = xvalid ? (accx[i] - mean) * rstd : 0.f;
     }
     store_tile_smem<EXTRA>(bufH, LD, acc, accx, ty, tx);
+    if (HLN) {   // n5 of every row -> bufB: A operand of the recomputed node_mlp.4 product
+      float n5t[8][8], n5x[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = col_nn(tx, j);
+          n5t[i][j] = acc[i][j] * p.node_ln_g[c] + p.node_ln_b[c];
+        }
+        n5x[i] = xvalid ? accx[i] * p.node_ln_g[64 + tx] + p.node_ln_b[64 + tx] : 0.f;
+      }
+      store_tile_smem<EXTRA>(bufB, LD, n5t, n5x, ty, tx);
+    }
     // n5 = nhat * gamma + beta -> global (X operand of dW6 = n5^T . do)
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -137,8 +156,65 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
         if (EXTRA) n5_out[(long)(node0 + r) * DHP + 64 + tx] = xvalid ? accx[i] * p.node_ln_g[64 + tx] + p.node_ln_b[64 + tx] : 0.f;
       }
     }
+    if (HLN) {   // y = skip(n5 . W6 + b6), its LayerNorm statistics, dy = LN_f backward of dh_out -> dy_io
+      __syncthreads();
+      float y[8][8], yx[8];
+      acc_set_bias(y, p.b_node2, tx);
+      gemm_nn_stream<false>(y, yx, bufB + ty * 8 * LD, LD, DHP, p.w_node2, 64, 64, wbuf, tid);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int r = ty * 8 + i;
+        if (skip && r < nvalid) {
+          const float* hr = h_in + (long)(node0 + r) * ldh + tx * 4;
+          const float4 a = *reinterpret_cast<const float4*>(hr), b = *reinterpret_cast<const float4*>(hr + 32);
+          const float s1 = 1.f - p.skip_weight_h, s0 = p.skip_weight_h;
+          y[i][0] = s0 * y[i][0] + s1 * a.x; y[i][1] = s0 * y[i][1] + s1 * a.y;
+          y[i][2] = s0 * y[i][2] + s1 * a.z; y[i][3] = s0 * y[i][3] + s1 * a.w;
+          y[i][4] = s0 * y[i][4] + s1 * b.x; y[i][5] = s0 * y[i][5] + s1 * b.y;
+          y[i][6] = s0 * y[i][6] + s1 * b.z; y[i][7] = s0 * y[i][7] + s1 * b.w;
+        }
+        float s = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s += y[i][j];
+        const float mean = row_sum8(s) * (1.f / 64.f);
+        float q = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float dv = y[i][j] - mean;
+          q = fmaf(dv, dv, q);
+        }
+        const float rstd = 1.f / sqrtf(row_sum8(q) * (1.f / 64.f) + 1e-5f);
+        float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (r < nvalid) {
+          const float* gr = dy_io + (long)(node0 + r) * 64 + tx * 4;
+          const float4 a = *reinterpret_cast<const float4*>(gr), b = *reinterpret_cast<const float4*>(gr + 32);
+          g[0] = a.x; g[1] = a.y; g[2] = a.z; g[3] = a.w; g[4] = b.x; g[5] = b.y; g[6] = b.z; g[7] = b.w;
+        }
+        float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int c = col_nn(tx, j);
+          y[i][j] = (y[i][j] - mean) * rstd;                   // y-hat
+          fgsum[j] = fmaf(g[j], y[i][j], fgsum[j]);
+          fbsum[j] += g[j];
+          g[j] *= nm.final_ln_g[c];
+          s1 += g[j];
+          s2 = fmaf(g[j], y[i][j], s2);
+        }
+        const float m1 = row_sum8(s1) * (1.f / 64.f), m2 = row_sum8(s2) * (1.f / 64.f);
+        if (r < nvalid) {
+          float dy[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) dy[j] = rstd * (g[j] - m1 - y[i][j] * m2);
+          float* o = dy_io + (long)(node0 + r) * 64 + tx * 4;
+          *reinterpret_cast<float4*>(o) = make_float4(dy[0], dy[1], dy[2], dy[3]);
+          *reinterpret_cast<float4*>(o + 32) = make_float4(dy[4], dy[5], dy[6], dy[7]);
+        }
+      }
+      __syncthreads();   // dy of the tile is in dy_io for the loads below
+    }
     // ---------------- dn = (skH dh') . W6 ----------------
-    tile_load_async(bufA, LD, dh_out + (long)node0 * 64, 64, EQD_TM, nvalid, 64, tid);
+    tile_load_async(bufA, LD, dsrc + (long)node0 * 64, 64, EQD_TM, nvalid, 64, tid);
     cp_async_commit();
     cp_async_wait<0>();
     __syncthreads();
@@ -230,7 +306,7 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
         if (blk == 0) {          // dh = (1 - skH) dh' + h block
           float add[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
           if (skip) {
-            const float* d = dh_out + n * 64 + tx * 4;
+            const float* d = dsrc + n * 64 + tx * 4;
             float4 a = *reinterpret_cast<const float4*>(d), b = *reinterpret_cast<const float4*>(d + 32);
             const float s1 = 1.f - p.skip_weight_h;
             add[0] = s1 * a.x; add[1] = s1 * a.y; add[2] = s1 * a.z; add[3] = s1 * a.w;
@@ -260,8 +336,13 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
     }
     __syncthreads();
   }
-  // per-CTA partials of the LayerNorm affine gradients: vec_partial[cta][0:72] = dgamma, [72:144] = dbeta
-  float* vp = vec_partial + (long)blockIdx.x * 144;
+  // per-CTA partials of the LayerNorm affine gradients: vec_partial[cta][0:72] = dgamma, [72:144] = dbeta; HLN:
+  // [144:208) / [208:272) those of final_h_layernorm_layer
+  float* vp = vec_partial + (long)blockIdx.x * (HLN ? 272 : 144);
+  if (HLN) {
+    colacc8_flush(fgsum, scratch, vp + 144, tid);
+    colacc8_flush(fbsum, scratch, vp + 208, tid);
+  }
   colacc8_flush(gsum, scratch, vp, tid);
   colacc8_flush(bsum, scratch, vp + 72, tid);
   {   // channels 64..71 (layer 0 only): reduce over the 16 row groups in fixed order
@@ -282,7 +363,7 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
 
 extern "C" int eqd_bwd_node_mlp(const eqd_graph* g, const eqd_layer* p_l, const float* w_node1_lin,
                                 const float* w_node2_lin, const float* h_in, int32_t ldh, const float* aggr,
-                                const float* mu, int32_t ldmu, const float* h0, const float* dh_out, float* dh_in,
+                                const float* mu, int32_t ldmu, const float* h0, float* dh_out, float* dh_in,
                                 float* daggr, float* dmu, float* dh0_acc, float* n5_out, float* du_out,
                                 float* vec_partial, int32_t* n_partials_out, void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
@@ -293,27 +374,36 @@ extern "C" int eqd_bwd_node_mlp(const eqd_graph* g, const eqd_layer* p_l, const 
   if (!extra && !(p->dh == 64 && p->dhp == 64)) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;
   if ((ldh & 3) || (ldmu & 3) || ldh < p->dhp || ldmu < p->dhp) return EQD_ERR_BAD_ARG;
+  const int hln = eqd_final_ln(p_l);
+  if (hln < 0) return EQD_ERR_BAD_ARG;
   const int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
   int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
   if (n_partials_out) *n_partials_out = grid > 0 ? grid : 0;
   if (g->n_nodes <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const eqd_dropout& dr = p_l->dropout;
-#define EQD_BWD_NODE_LAUNCH(EXTRA, DROP)                                                                                 \
+  // HLN: dh_out is only read and written through dy_io (the kernel's dh_out parameter is never dereferenced)
+#define EQD_BWD_NODE_LAUNCH(EXTRA, DROP, HLN)                                                                            \
   do {                                                                                                                \
     size_t smem = eqd::NodeBwdCfg<EXTRA>::SMEM;                                                                       \
-    EQD_SET_SMEM((eqd::bwd_node_mlp_kernel<EXTRA, DROP>), smem);                                                      \
-    eqd::bwd_node_mlp_kernel<EXTRA, DROP><<<grid, EQD_THREADS, smem, st>>>(g->n_nodes, *p, w_node1_lin, w_node2_lin, h_in, \
-                                                                           ldh, aggr, mu, ldmu, h0, dh_out, dh_in, daggr, \
-                                                                           dmu, dh0_acc, n5_out, du_out, vec_partial, dr); \
+    EQD_SET_SMEM((eqd::bwd_node_mlp_kernel<EXTRA, DROP, HLN>), smem);                                                 \
+    eqd::bwd_node_mlp_kernel<EXTRA, DROP, HLN><<<grid, EQD_THREADS, smem, st>>>(                                      \
+        g->n_nodes, *p, w_node1_lin, w_node2_lin, h_in, ldh, aggr, mu, ldmu, h0, HLN ? nullptr : dh_out, dh_in, daggr, \
+        dmu, dh0_acc, n5_out, du_out, vec_partial, dr, p_l->norms, HLN ? dh_out : nullptr);                            \
+  } while (0)
+#define EQD_BWD_NODE_HLN(EXTRA, DROP)              \
+  do {                                             \
+    if (hln) EQD_BWD_NODE_LAUNCH(EXTRA, DROP, true); \
+    else EQD_BWD_NODE_LAUNCH(EXTRA, DROP, false);  \
   } while (0)
   if (dr.p > 0.f) {
-    if (extra) EQD_BWD_NODE_LAUNCH(true, true);
-    else EQD_BWD_NODE_LAUNCH(false, true);
+    if (extra) EQD_BWD_NODE_HLN(true, true);
+    else EQD_BWD_NODE_HLN(false, true);
   } else {
-    if (extra) EQD_BWD_NODE_LAUNCH(true, false);
-    else EQD_BWD_NODE_LAUNCH(false, false);
+    if (extra) EQD_BWD_NODE_HLN(true, false);
+    else EQD_BWD_NODE_HLN(false, false);
   }
+#undef EQD_BWD_NODE_HLN
 #undef EQD_BWD_NODE_LAUNCH
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;

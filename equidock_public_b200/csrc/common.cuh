@@ -48,6 +48,12 @@ inline int eqd_mma_products(const eqd_layer_params* p) {
   return p->mma_products == 3 && p->dh == EQD_HID ? 3 : 0;
 }
 
+// The optional LayerNorms of a layer (eqd_layer_norms): 1 on, 0 off, -1 for only one of the two vectors set
+// (EQD_ERR_BAD_ARG).
+inline int eqd_norm_on(const float* g, const float* b) { return (g != nullptr) == (b != nullptr) ? (int)(g != nullptr) : -1; }
+inline int eqd_coors_ln(const eqd_layer* l) { return eqd_norm_on(l->norms.coors_ln_g, l->norms.coors_ln_b); }
+inline int eqd_final_ln(const eqd_layer* l) { return eqd_norm_on(l->norms.final_ln_g, l->norms.final_ln_b); }
+
 namespace eqd {
 
 // LeakyReLU for 0 <= slope <= 1 (checked by the launchers): max(v, slope*v) is bit-identical to the select form
@@ -237,6 +243,31 @@ __device__ __forceinline__ void lrelu_layernorm(float (&acc)[8][8], float (&accx
       acc[i][j] = (acc[i][j] - mean) * rstd * gamma[c] + beta[c];
     }
     if (EXTRA) accx[i] = xvalid ? (accx[i] - mean) * rstd * gamma[64 + tx] + beta[64 + tx] : 0.f;
+  }
+}
+
+// nn.LayerNorm(64) (biased variance, eps 1e-5) of each row of a 64-wide micro-tile, with the statistics code of
+// lrelu_layernorm.  gamma/beta indexed by channel.
+__device__ __forceinline__ void layernorm64(float (&acc)[8][8], const float* __restrict__ gamma,
+                                            const float* __restrict__ beta, int tx) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s += acc[i][j];
+    const float mean = row_sum8(s) * (1.f / 64.f);
+    float q = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float d = acc[i][j] - mean;
+      q = fmaf(d, d, q);
+    }
+    const float rstd = 1.f / sqrtf(row_sum8(q) * (1.f / 64.f) + 1e-5f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = col_nn(tx, j);
+      acc[i][j] = (acc[i][j] - mean) * rstd * gamma[c] + beta[c];
+    }
   }
 }
 

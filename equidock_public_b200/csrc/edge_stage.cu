@@ -25,14 +25,17 @@ struct EdgeSmem {
   int src[EQD_TM];
   int dst[EQD_TM];
   int rp[EQD_TM + 1];
+  float cln_g[64], cln_b[64];   // coors_mlp.3 (CLN only)
 };
 
 // DROP: training-mode dropout sites 0 (z1) and 1 (z3) of eqd_dropout `dr`, applied before their LeakyReLU.
-template <bool DROP>
+// CLN: the coordinate LayerNorm coors_mlp.3 of eqd_layer_norms `nm` after coors_mlp.2 (the same statistics code as
+// edge_mlp.3), so phi = w4 . LN(LeakyReLU(z3)) + b4.
+template <bool DROP, bool CLN>
 __global__ void __launch_bounds__(EQD_THREADS, 2)
 edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ proj, const double* __restrict__ x_in,
                   const double* __restrict__ x_orig, float* __restrict__ aggr, double* __restrict__ x_out,
-                  int* __restrict__ status, int tn /* destination nodes per tile */, eqd_dropout dr) {
+                  int* __restrict__ status, int tn /* destination nodes per tile */, eqd_dropout dr, eqd_layer_norms nm) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   EdgeSmem& s = *reinterpret_cast<EdgeSmem*>(smem_raw);
   const int tid = threadIdx.x, ty = tid >> 3, tx = tid & 7;
@@ -51,6 +54,10 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
     s.b2[tid] = p.b_edge2[tid];
     s.b3[tid] = p.b_coor1[tid];
     s.w4[tid] = p.w_coor2[tid];
+  }
+  if (CLN && tid < 64) {
+    s.cln_g[tid] = nm.coors_ln_g[tid];
+    s.cln_b[tid] = nm.coors_ln_b[tid];
   }
   __syncthreads();
 
@@ -143,10 +150,11 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
     store_tile_smem<false>(s.buf, EDGE_LD, acc, accx, ty, tx);  // msg tile (A of coors_mlp, source of aggr)
     __syncthreads();
 
-    // ---- coors_mlp: Linear, LeakyReLU, Linear(64->1) -> phi ------------------------------------
+    // ---- coors_mlp: Linear, LeakyReLU, (LayerNorm,) Linear(64->1) -> phi ------------------------
     acc_set_bias(acc, s.b3, tx);
     gemm_nn<false>(acc, accx, s.buf + ty * 8 * EDGE_LD, EDGE_LD, s.w3, 64, 64, tx);
     if (DROP) dropout_tile<false>(acc, accx, dr, 1, e0 + ty * 8, tx);
+    if (CLN) lrelu_layernorm<false>(acc, accx, s.cln_g, s.cln_b, 64, p.leaky_slope, tx);  // coors_mlp.2-3
     {
       float w4r[8];
 #pragma unroll
@@ -155,7 +163,7 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
       for (int i = 0; i < 8; ++i) {
         float v = 0.f;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) v = fmaf(lrelu(acc[i][j], p.leaky_slope), w4r[j], v);
+        for (int j = 0; j < 8; ++j) v = fmaf(CLN ? acc[i][j] : lrelu(acc[i][j], p.leaky_slope), w4r[j], v);
         v = row_sum8(v);
         if (tx == 0) s.phi[ty * 8 + i] = v + p.b_coor2;
       }
@@ -186,29 +194,37 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
   }
 }
 
+template <bool DROP, bool CLN>
+static int launch_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const float* proj, const double* x_in,
+                             const double* x_orig, float* aggr, double* x_out, int32_t* status, int tn, int grid,
+                             void* stream) {
+  const size_t smem = sizeof(EdgeSmem);
+  EQD_SET_SMEM((edge_stage_kernel<DROP, CLN>), smem);
+  edge_stage_kernel<DROP, CLN><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, p_l->dev, proj, x_in, x_orig, aggr,
+                                                                                  x_out, status, tn, p_l->dropout, p_l->norms);
+  EQD_CUDA_LAUNCH_CHECK();
+  return EQD_OK;
+}
+
 }  // namespace eqd
 
 extern "C" int eqd_edge_stage_ffma(const eqd_graph* g, const eqd_layer* p_l, const float* proj, const double* x_in,
                               const double* x_orig, float* aggr, double* x_out, int32_t* status, void* stream) {
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !proj || !x_in || !x_orig || !aggr || !x_out || !status) return EQD_ERR_BAD_ARG;
+  const int cln = eqd_coors_ln(p_l);
+  if (cln < 0) return EQD_ERR_BAD_ARG;
   if (g->max_in_degree < 1 || g->max_in_degree > EQD_TM) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
   if (g->n_nodes <= 0) return EQD_OK;
   int tn = EQD_TM / g->max_in_degree;
   if (tn > EQD_TM) tn = EQD_TM;
   int ntiles = (g->n_nodes + tn - 1) / tn;
-  size_t smem = sizeof(eqd::EdgeSmem);
   int grid = ntiles < EQD_SMS * 2 ? ntiles : EQD_SMS * 2;
-  if (p_l->dropout.p > 0.f) {
-    EQD_SET_SMEM((eqd::edge_stage_kernel<true>), smem);
-    eqd::edge_stage_kernel<true><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, proj, x_in, x_orig, aggr,
-                                                                                  x_out, status, tn, p_l->dropout);
-  } else {
-    EQD_SET_SMEM((eqd::edge_stage_kernel<false>), smem);
-    eqd::edge_stage_kernel<false><<<grid, EQD_THREADS, smem, (cudaStream_t)stream>>>(*g, *p, proj, x_in, x_orig, aggr,
-                                                                                   x_out, status, tn, p_l->dropout);
-  }
-  EQD_CUDA_LAUNCH_CHECK();
-  return EQD_OK;
+  const bool drop = p_l->dropout.p > 0.f;
+  if (cln)
+    return drop ? eqd::launch_edge_stage<true, true>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, grid, stream)
+                : eqd::launch_edge_stage<false, true>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, grid, stream);
+  return drop ? eqd::launch_edge_stage<true, false>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, grid, stream)
+              : eqd::launch_edge_stage<false, false>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, grid, stream);
 }

@@ -13,7 +13,7 @@
 //        the 4 lanes of a quad: lane shuffles) -> bf16x3 A fragments in registers
 //   GEMM2 and GEMM3 as RS wgmma on those fragments (2 x 24, N=64 halves of the stacked panel [W2 ; W3 W2])
 //     -> msg (+b2) -> fp32 tile in smem (mean aggregation at the destination nodes)
-//     -> coordinate MLP hidden layer -> LeakyReLU, dot w4 -> phi (lane shuffles);
+//     -> coordinate MLP hidden layer -> LeakyReLU, (coordinate LayerNorm,) dot w4 -> phi (lane shuffles);
 //        x' = eta x0 + (1-eta) x + mean(x_rel phi) in fp64.
 // Per-edge activations never leave the SM; weights are read from HBM/L2 once per CTA.  A tile whose nodes all have 10
 // in-edges (a k-NN graph) needs no row_ptr lookups in the aggregation.
@@ -61,13 +61,21 @@ struct TcSmem {
   unsigned long long w_bar;
 };
 
-template <int P>
+// Bytes of dynamic shared memory past TcSmem: the coordinate LayerNorm's gamma | beta (CLN only)
+#define TC_CLN_BYTES 512
+static_assert(sizeof(TcSmem) + 128 + TC_CLN_BYTES <= 232448, "edge stage shared memory exceeds the sm_90 limit");
+
+// CLN: the coordinate LayerNorm coors_mlp.3 (eqd_layer_norms `nm`) on LeakyReLU(hidden + b3), with the statistics and
+// order of edge_mlp.3, before the dot product with w4.
+template <int P, bool CLN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ EdgeConsts cst_p,
                      const float* __restrict__ proj, const double* __restrict__ x_in, const double* __restrict__ x_orig,
-                     float* __restrict__ aggr, double* __restrict__ x_out, int* __restrict__ status, int tn) {
+                     float* __restrict__ aggr, double* __restrict__ x_out, int* __restrict__ status, int tn,
+                     eqd_layer_norms nm) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   TcSmem& S = *reinterpret_cast<TcSmem*>(smem_raw);
+  float* cln = reinterpret_cast<float*>(smem_raw + sizeof(TcSmem));   // [gamma 64 | beta 64]
   const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, r = t & 63, half = t >> 6;
   const int warp = t >> 5, lane = t & 31;
   TcWgSmem& W = S.wg[wgi];
@@ -86,6 +94,7 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
     bulk_g2s(S.w, p.w_edge_tc, TC_W_BYTES, &S.w_bar);
   }
   for (int i = tid; i < 5 * 64; i += TC_THREADS) (&S.cst.ln_g[0])[i] = (&cst_p.ln_g[0])[i];
+  if (CLN && tid < 128) cln[tid] = tid < 64 ? nm.coors_ln_g[tid] : nm.coors_ln_b[tid - 64];
   __syncthreads();
   mbar_wait(&S.w_bar, 0);
   unsigned he_phase = 0;
@@ -355,6 +364,11 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
           u[4 * j + 2 * h + 1] = fmaxf(x1, __fmul_rn(x1, slope));
         }
       }
+      if (CLN) {   // coors_mlp.3
+        float mean[2], rstd[2];
+        quad_ln_stats(u, mean, rstd);
+        quad_ln_apply(u, mean, rstd, cln, cln + 64, fc);
+      }
       // phi = w4 . u + b_coor2 in the chain order of the row-per-thread formulation: four fp32 chains per 32-column half,
       // combined in fp64
       float pu[32];
@@ -437,18 +451,18 @@ edge_stage_tc_kernel(eqd_graph g, eqd_layer_params p, const __grid_constant__ Ed
   __syncthreads();
 }
 
-template <int P>
+template <int P, bool CLN>
 static int launch_edge_stage_tc(const eqd_graph* g, const eqd_layer* p_l, const float* proj, const double* x_in,
                                 const double* x_orig, float* aggr, double* x_out, int32_t* status, int tn, void* stream) {
   const int ntiles = (g->n_nodes + tn - 1) / tn;
   EdgeConsts cst;
   memcpy(&cst, p_l->consts.edge, sizeof(cst));
-  size_t smem = sizeof(TcSmem) + 128;
-  EQD_SET_SMEM((edge_stage_tc_kernel<P>), smem);
+  size_t smem = sizeof(TcSmem) + 128 + (CLN ? TC_CLN_BYTES : 0);
+  EQD_SET_SMEM((edge_stage_tc_kernel<P, CLN>), smem);
   int grid = (ntiles + TC_WGS - 1) / TC_WGS;
   if (grid > EQD_SMS) grid = EQD_SMS;
-  edge_stage_tc_kernel<P><<<grid, TC_THREADS, smem, (cudaStream_t)stream>>>(*g, p_l->dev, cst, proj, x_in, x_orig, aggr,
-                                                                           x_out, status, tn);
+  edge_stage_tc_kernel<P, CLN><<<grid, TC_THREADS, smem, (cudaStream_t)stream>>>(*g, p_l->dev, cst, proj, x_in, x_orig,
+                                                                                aggr, x_out, status, tn, p_l->norms);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }
@@ -460,6 +474,8 @@ extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const fl
   const eqd_layer_params* p = p_l ? &p_l->dev : nullptr;
   if (!g || !p || !proj || !x_in || !x_orig || !aggr || !x_out || !status) return EQD_ERR_BAD_ARG;
   if (!p->w_edge_tc) return EQD_ERR_BAD_ARG;
+  const int cln = eqd_coors_ln(p_l);
+  if (cln < 0) return EQD_ERR_BAD_ARG;
   const int products = eqd_mma_products(p);
   if (!products) return EQD_ERR_UNSUPPORTED;
   if (g->max_in_degree < 1 || g->max_in_degree > EQD_TM) return EQD_ERR_UNSUPPORTED;
@@ -472,6 +488,9 @@ extern "C" int eqd_edge_stage(const eqd_graph* g, const eqd_layer* p_l, const fl
   if (g->n_nodes <= 0) return EQD_OK;
   int tn = TC_ROWS / g->max_in_degree;
   if (tn > TC_MAX_TN) tn = TC_MAX_TN;
-  return products == 3 ? eqd::launch_edge_stage_tc<3>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream)
-                       : eqd::launch_edge_stage_tc<6>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream);
+  if (cln)
+    return products == 3 ? eqd::launch_edge_stage_tc<3, true>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream)
+                         : eqd::launch_edge_stage_tc<6, true>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream);
+  return products == 3 ? eqd::launch_edge_stage_tc<3, false>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream)
+                       : eqd::launch_edge_stage_tc<6, false>(g, p_l, proj, x_in, x_orig, aggr, x_out, status, tn, stream);
 }

@@ -36,13 +36,20 @@ struct NmSmem {
   unsigned long long w_bar;
 };
 
-template <int P>
+// Bytes of dynamic shared memory past NmSmem: the final LayerNorm's gamma | beta (HLN only)
+#define NM_HLN_BYTES 512
+static_assert(sizeof(NmSmem) + 128 + NM_HLN_BYTES <= 232448, "node MLP shared memory exceeds the sm_90 limit");
+
+// HLN: the final feature LayerNorm (final_h_layernorm_layer of eqd_layer_norms `nm`) on the row after the skip combination,
+// statistics over the quad as for node_mlp.3 (quad_ln_stats), the last step before h' is stored.
+template <int P, bool HLN>
 __global__ void __launch_bounds__(NM_CHAINS * 128, 1)
 node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmConsts cst, const float* __restrict__ h_in,
                    const float* __restrict__ aggr, const float* __restrict__ mu, const float* __restrict__ h0,
-                   float* __restrict__ h_out) {
+                   float* __restrict__ h_out, eqd_layer_norms nm) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   NmSmem& S = *reinterpret_cast<NmSmem*>(smem_raw);
+  float* hln = reinterpret_cast<float*>(smem_raw + sizeof(NmSmem));   // [gamma 64 | beta 64]
   const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, lane = t & 31;
   float (&ring)[NM_SLOTS][64 * 64] = S.stage[wgi];
   const int bar = 1 + wgi;   // this chain's named barrier
@@ -54,6 +61,7 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
     bulk_g2s(S.w, p.w_node_tc, NM_W_BYTES, &S.w_bar);
   }
   for (int i = tid; i < 256; i += NM_CHAINS * 128) S.c[i] = reinterpret_cast<const float*>(&cst)[i];
+  if (HLN && tid < 128) hln[tid] = tid < 64 ? nm.final_ln_g[tid] : nm.final_ln_b[tid - 64];
   __syncthreads();
   const unsigned w_saddr = smem_u32(S.w);
   const float slope = p.leaky_slope, sk = p.skip_weight_h, sk1 = 1.f - p.skip_weight_h;
@@ -189,6 +197,31 @@ node_mlp_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ NmCo
       wg_gemm6_rs_issue<64, 4, 0, false, P>(d, af, [&](int sp, int kb) {
         return b_desc_ex(w_saddr + NM_W6_BASE + sp * NM_W6_SPLIT + kb * 2048, 1024, 128); }, false);
       wg_mma_wait(d);
+      if (HLN) {   // y = skip(...) for every fragment row (the quad reductions need all of them), then LN_f, store
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float2 bj = *reinterpret_cast<const float2*>(&S.c[192 + 8 * j + fc]);
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int i = 4 * j + 2 * hh;
+            d[i] = __fmaf_rn(__fadd_rn(d[i], bj.x), sk, __fmul_rn(hs[i], sk1));
+            d[i + 1] = __fmaf_rn(__fadd_rn(d[i + 1], bj.y), sk, __fmul_rn(hs[i + 1], sk1));
+          }
+        }
+        float mean[2], rstd[2];
+        quad_ln_stats(d, mean, rstd);
+        quad_ln_apply(d, mean, rstd, hln, hln + 64, fc);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = fr0 + 8 * hh;
+          if (row < nvalid) {
+            float* o = h_out + (long)(node0 + row) * EQD_HID + fc;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+              *reinterpret_cast<float2*>(o + 8 * j) = make_float2(d[4 * j + 2 * hh], d[4 * j + 2 * hh + 1]);
+          }
+        }
+      } else
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         const int row = fr0 + 8 * hh;
@@ -230,9 +263,13 @@ struct Nm0Smem {
   unsigned long long w_bar;
 };
 
+// HLN: the final feature LayerNorm (eqd_layer_norms `nm`) on node_mlp's output (layer 0 has no skip), its row statistics
+// over the two halves of a row through `red`, the last step before h' is stored.
+template <bool HLN>
 __global__ void __launch_bounds__(NM_THREADS, 1)
 node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0Consts cst, const float* __restrict__ h0,
-                    const float* __restrict__ aggr, const float* __restrict__ mu /*[n][72]*/, float* __restrict__ h_out) {
+                    const float* __restrict__ aggr, const float* __restrict__ mu /*[n][72]*/, float* __restrict__ h_out,
+                    eqd_layer_norms nm) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Nm0Smem& S = *reinterpret_cast<Nm0Smem*>(smem_raw);
   const int tid = threadIdx.x, q = tid, half = q >> 7, r = q & 127, wgi = tid >> 7;
@@ -376,6 +413,25 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
       tile_ld32f(dtile, NM0_LD, r, half * 32, v);
 #pragma unroll
       for (int c = 0; c < 32; ++c) v[c] += cst.b6[half * 32 + c];
+      if (HLN) {   // final_h_layernorm_layer: two-pass row statistics of the 64 outputs, half rows combined in red
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < 32; ++c) s += v[c];
+        red[(r * 2 + half) * 2] = s;
+        __syncthreads();
+        const float mean = (red[r * 4] + red[r * 4 + 2]) * (1.f / 64.f);
+        float q = 0.f;
+#pragma unroll
+        for (int c = 0; c < 32; ++c) {
+          const float dv = v[c] - mean;
+          q = fmaf(dv, dv, q);
+        }
+        red[(r * 2 + half) * 2 + 1] = q;
+        __syncthreads();
+        const float rstd = 1.f / sqrtf((red[r * 4 + 1] + red[r * 4 + 3]) * (1.f / 64.f) + 1e-5f);
+#pragma unroll
+        for (int c = 0; c < 32; ++c) v[c] = (v[c] - mean) * rstd * nm.final_ln_g[half * 32 + c] + nm.final_ln_b[half * 32 + c];
+      }
       if (valid) {
         float4* o = reinterpret_cast<float4*>(h_out + (long)node * EQD_HID + half * 32);
 #pragma unroll
@@ -386,18 +442,18 @@ node_mlp0_tc_kernel(int n_nodes, eqd_layer_params p, const __grid_constant__ Nm0
   }
 }
 
-template <int P>
+template <int P, bool HLN>
 static int launch_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const float* h_in, const float* aggr,
                               const float* mu, const float* h0, float* h_out, void* stream) {
   NmConsts cst;
   memcpy(&cst, p_l->consts.node, sizeof(cst));
   const int ntiles = (g->n_nodes + 63) / 64;
-  const size_t smem = sizeof(NmSmem) + 128;
-  EQD_SET_SMEM(node_mlp_tc_kernel<P>, smem);
+  const size_t smem = sizeof(NmSmem) + 128 + (HLN ? NM_HLN_BYTES : 0);
+  EQD_SET_SMEM((node_mlp_tc_kernel<P, HLN>), smem);
   int grid = (ntiles + NM_CHAINS - 1) / NM_CHAINS;
   if (grid > EQD_SMS) grid = EQD_SMS;
-  node_mlp_tc_kernel<P><<<grid, NM_CHAINS * 128, smem, (cudaStream_t)stream>>>(g->n_nodes, p_l->dev, cst, h_in, aggr, mu,
-                                                                             h0, h_out);
+  node_mlp_tc_kernel<P, HLN><<<grid, NM_CHAINS * 128, smem, (cudaStream_t)stream>>>(g->n_nodes, p_l->dev, cst, h_in, aggr,
+                                                                                   mu, h0, h_out, p_l->norms);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }
@@ -414,9 +470,14 @@ extern "C" int eqd_node_mlp_tc(const eqd_graph* g, const eqd_layer* p_l, const f
   const int products = eqd_mma_products(p);
   if (!products) return EQD_ERR_UNSUPPORTED;
   if (!p->w_node_tc || (reinterpret_cast<uintptr_t>(p->w_node_tc) & 15)) return EQD_ERR_BAD_ARG;
+  const int hln = eqd_final_ln(p_l);
+  if (hln < 0) return EQD_ERR_BAD_ARG;
   if (g->n_nodes <= 0) return EQD_OK;
-  return products == 3 ? eqd::launch_node_mlp_tc<3>(g, p_l, h_in, aggr, mu, h0, h_out, stream)
-                       : eqd::launch_node_mlp_tc<6>(g, p_l, h_in, aggr, mu, h0, h_out, stream);
+  if (hln)
+    return products == 3 ? eqd::launch_node_mlp_tc<3, true>(g, p_l, h_in, aggr, mu, h0, h_out, stream)
+                         : eqd::launch_node_mlp_tc<6, true>(g, p_l, h_in, aggr, mu, h0, h_out, stream);
+  return products == 3 ? eqd::launch_node_mlp_tc<3, false>(g, p_l, h_in, aggr, mu, h0, h_out, stream)
+                       : eqd::launch_node_mlp_tc<6, false>(g, p_l, h_in, aggr, mu, h0, h_out, stream);
 }
 
 extern "C" int eqd_node_mlp_tc0(const eqd_graph* g, const eqd_layer* p_l, const float* h0, const float* aggr,
@@ -427,14 +488,23 @@ extern "C" int eqd_node_mlp_tc0(const eqd_graph* g, const eqd_layer* p_l, const 
   if (p->dh != 69 || p->dhp != 72 || !eqd_mma_products(p)) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
   if (!p->w_node_tc || (reinterpret_cast<uintptr_t>(p->w_node_tc) & 15)) return EQD_ERR_BAD_ARG;
+  const int hln = eqd_final_ln(p_l);
+  if (hln < 0) return EQD_ERR_BAD_ARG;
   if (g->n_nodes <= 0) return EQD_OK;
   eqd::Nm0Consts cst;
   memcpy(&cst, p_l->consts.node, sizeof(cst));
   int ntiles = (g->n_nodes + EQD_TM - 1) / EQD_TM;
   size_t smem = sizeof(eqd::Nm0Smem) + 128;
-  EQD_SET_SMEM((eqd::node_mlp0_tc_kernel), smem);
   int grid = ntiles < EQD_SMS ? ntiles : EQD_SMS;
-  eqd::node_mlp0_tc_kernel<<<grid, NM_THREADS, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h0, aggr, mu, h_out);
+  if (hln) {
+    EQD_SET_SMEM((eqd::node_mlp0_tc_kernel<true>), smem);
+    eqd::node_mlp0_tc_kernel<true><<<grid, NM_THREADS, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h0, aggr, mu, h_out,
+                                                                                    p_l->norms);
+  } else {
+    EQD_SET_SMEM((eqd::node_mlp0_tc_kernel<false>), smem);
+    eqd::node_mlp0_tc_kernel<false><<<grid, NM_THREADS, smem, (cudaStream_t)stream>>>(g->n_nodes, *p, cst, h0, aggr, mu,
+                                                                                     h_out, p_l->norms);
+  }
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }

@@ -26,12 +26,14 @@ struct NodeCfg {
 };
 
 // DROP: training-mode dropout site 2 (u5) of eqd_dropout `dr`, applied before the LeakyReLU.
-template <bool EXTRA, bool DROP>
+// HLN: the final feature LayerNorm (final_h_layernorm_layer, eqd_layer_norms `nm`) on the row after the skip combination:
+// h' = LN_f(y), the last step before h' is stored and projected.
+template <bool EXTRA, bool DROP, bool HLN>
 __global__ void __launch_bounds__(EQD_THREADS, 2)
 node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_next, const float* __restrict__ h_in,
                   int ldh, const float* __restrict__ h0, const float* __restrict__ proj,
                   const float* __restrict__ aggr, float* __restrict__ h_out, float* __restrict__ proj_next,
-                  float* __restrict__ mu_out, eqd_dropout dr) {
+                  float* __restrict__ mu_out, eqd_dropout dr, eqd_layer_norms nm) {
   using C = NodeCfg<EXTRA>;
   constexpr int DHP = C::DHP, LD = C::LD, KC = C::KC;
   extern __shared__ __align__(16) float smem[];
@@ -164,6 +166,31 @@ node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_
 
     // skip connection (only when in/out widths match, :332-334), write h'
     const bool skip = (p.dh == EQD_HID);
+    if constexpr (HLN) {   // every row takes part in the row reductions; rows past nvalid are not stored
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int r = ty * 8 + i;
+        if (skip && r < nvalid) {
+          const float* hr = h_in + (long)(node0 + r) * ldh + tx * 4;
+          float4 a = *reinterpret_cast<const float4*>(hr), b = *reinterpret_cast<const float4*>(hr + 32);
+          const float sk = p.skip_weight_h, sk1 = 1.f - p.skip_weight_h;
+          acc[i][0] = sk * acc[i][0] + sk1 * a.x; acc[i][1] = sk * acc[i][1] + sk1 * a.y;
+          acc[i][2] = sk * acc[i][2] + sk1 * a.z; acc[i][3] = sk * acc[i][3] + sk1 * a.w;
+          acc[i][4] = sk * acc[i][4] + sk1 * b.x; acc[i][5] = sk * acc[i][5] + sk1 * b.y;
+          acc[i][6] = sk * acc[i][6] + sk1 * b.z; acc[i][7] = sk * acc[i][7] + sk1 * b.w;
+        }
+      }
+      layernorm64(acc, nm.final_ln_g, nm.final_ln_b, tx);   // final_h_layernorm_layer
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int r = ty * 8 + i;
+        if (r < nvalid) {
+          float* orow = h_out + (long)(node0 + r) * EQD_HID + tx * 4;
+          *reinterpret_cast<float4*>(orow) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
+          *reinterpret_cast<float4*>(orow + 32) = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
+        }
+      }
+    } else {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       int r = ty * 8 + i;
@@ -181,6 +208,7 @@ node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_
         *reinterpret_cast<float4*>(orow) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
         *reinterpret_cast<float4*>(orow + 32) = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
       }
+    }
     }
     if (has_next) {  // fused projections of h' for the next layer
       store_tile_smem<false>(bufB, LD, acc, accx, ty, tx);
@@ -200,6 +228,8 @@ extern "C" int eqd_node_stage(const eqd_graph* g, const eqd_layer* p_l, const eq
   if (!g || !p || !h_in || !h0 || !proj || !aggr || !h_out) return EQD_ERR_BAD_ARG;
   if (reinterpret_cast<uintptr_t>(mu) & 15) return EQD_ERR_BAD_ARG;   // rows are written 16 bytes at a time
   if (p_next && (!proj_next || p_next->dh != 64 || p_next->dhp != 64)) return EQD_ERR_BAD_ARG;
+  const int hln = eqd_final_ln(p_l);
+  if (hln < 0) return EQD_ERR_BAD_ARG;
   const bool extra = (p->dh == 69 && p->dhp == 72);
   if (!extra && !(p->dh == 64 && p->dhp == 64)) return EQD_ERR_UNSUPPORTED;
   if (!(p->leaky_slope >= 0.f && p->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;  // lrelu() = max(v, slope*v)
@@ -209,20 +239,26 @@ extern "C" int eqd_node_stage(const eqd_graph* g, const eqd_layer* p_l, const eq
   cudaStream_t st = (cudaStream_t)stream;
   const eqd_dropout& dr = p_l->dropout;
   const int grid = g->n_node_tiles < EQD_SMS * 2 ? g->n_node_tiles : EQD_SMS * 2;
-#define EQD_NODE_STAGE_LAUNCH(EXTRA, DROP)                                                                              \
+#define EQD_NODE_STAGE_LAUNCH(EXTRA, DROP, HLN)                                                                         \
   do {                                                                                                                \
     size_t smem = eqd::NodeCfg<EXTRA>::SMEM;                                                                          \
-    EQD_SET_SMEM((eqd::node_stage_kernel<EXTRA, DROP>), smem);                                                        \
-    eqd::node_stage_kernel<EXTRA, DROP><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, aggr, \
-                                                                         h_out, proj_next, mu, dr);                   \
+    EQD_SET_SMEM((eqd::node_stage_kernel<EXTRA, DROP, HLN>), smem);                                                   \
+    eqd::node_stage_kernel<EXTRA, DROP, HLN><<<grid, EQD_THREADS, smem, st>>>(*g, *p, pn, has_next, h_in, ldh, h0, proj, \
+                                                                              aggr, h_out, proj_next, mu, dr, p_l->norms); \
+  } while (0)
+#define EQD_NODE_STAGE_HLN(EXTRA, DROP)             \
+  do {                                              \
+    if (hln) EQD_NODE_STAGE_LAUNCH(EXTRA, DROP, true); \
+    else EQD_NODE_STAGE_LAUNCH(EXTRA, DROP, false);  \
   } while (0)
   if (dr.p > 0.f) {
-    if (extra) EQD_NODE_STAGE_LAUNCH(true, true);
-    else EQD_NODE_STAGE_LAUNCH(false, true);
+    if (extra) EQD_NODE_STAGE_HLN(true, true);
+    else EQD_NODE_STAGE_HLN(false, true);
   } else {
-    if (extra) EQD_NODE_STAGE_LAUNCH(true, false);
-    else EQD_NODE_STAGE_LAUNCH(false, false);
+    if (extra) EQD_NODE_STAGE_HLN(true, false);
+    else EQD_NODE_STAGE_HLN(false, false);
   }
+#undef EQD_NODE_STAGE_HLN
 #undef EQD_NODE_STAGE_LAUNCH
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;

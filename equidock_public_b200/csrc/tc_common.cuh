@@ -308,4 +308,62 @@ __device__ __forceinline__ void tile_ld32f(const float* tile, int ld, int row, i
   }
 }
 
+// LayerNorm statistics of the optional LayerNorms (coordinate, final feature): the edge_mlp.3 block of
+// edge_stage_tc_kernel restated as a function (that block stays inline, as it compiles to the same instructions as before
+// this function existed).  Rows of an accumulator
+// fragment v (a row's 64 columns sit on the 4 lanes of a quad) in the chain order of the row-per-thread formulation: per
+// 32-column half, two-pass (mean_h, M2_h) over four chains, then mean = (m0+m1)/2, M2 = M2_0 + M2_1 + (m0-m1)^2 * 16.
+__device__ __forceinline__ void quad_ln_stats(const float (&v)[32], float (&mean)[2], float (&rstd)[2]) {
+  float pv[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) pv[i] = __shfl_xor_sync(0xffffffffu, v[i], 2);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mh[2], qh[2];
+#pragma unroll
+    for (int ch = 0; ch < 2; ++ch) {
+      float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+      for (int c4 = 0; c4 < 8; ++c4) {
+        s0 = __fadd_rn(s0, chain_val(v, pv, h, ch, c4, 0));
+        s1 = __fadd_rn(s1, chain_val(v, pv, h, ch, c4, 1));
+      }
+      const float sp = s0 + s1;
+      mh[ch] = (sp + __shfl_xor_sync(0xffffffffu, sp, 1)) * (1.f / 32.f);
+      float q0 = 0.f, q1 = 0.f;
+#pragma unroll
+      for (int c4 = 0; c4 < 8; ++c4) {
+        const float d0 = __fadd_rn(chain_val(v, pv, h, ch, c4, 0), -mh[ch]);
+        const float d1 = __fadd_rn(chain_val(v, pv, h, ch, c4, 1), -mh[ch]);
+        q0 = fmaf(d0, d0, q0);
+        q1 = fmaf(d1, d1, q1);
+      }
+      const float qp = q0 + q1;
+      qh[ch] = qp + __shfl_xor_sync(0xffffffffu, qp, 1);
+    }
+    const float m0 = mh[0], m1 = mh[1];
+    mean[h] = 0.5f * (m0 + m1);
+    const float dm = m0 - m1;
+    const float var = (qh[0] + qh[1] + dm * dm * 16.f) * (1.f / 64.f);
+    rstd[h] = 1.f / sqrtf(var + 1e-5f);
+  }
+}
+
+// v <- (v - mean) * rstd * gamma + beta on an accumulator fragment (columns 8 j + fc + {0, 1})
+__device__ __forceinline__ void quad_ln_apply(float (&v)[32], const float (&mean)[2], const float (&rstd)[2],
+                                              const float* ln_g, const float* ln_b, int fc) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float2 gj = *reinterpret_cast<const float2*>(&ln_g[8 * j + fc]);
+    const float2 bj = *reinterpret_cast<const float2*>(&ln_b[8 * j + fc]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float& x0 = v[4 * j + 2 * h];
+      float& x1 = v[4 * j + 2 * h + 1];
+      x0 = fmaf(__fmul_rn(__fadd_rn(x0, -mean[h]), rstd[h]), gj.x, bj.x);
+      x1 = fmaf(__fmul_rn(__fadd_rn(x1, -mean[h]), rstd[h]), gj.y, bj.y);
+    }
+  }
+}
+
 }  // namespace eqd

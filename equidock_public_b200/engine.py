@@ -109,7 +109,14 @@ class PackedLayer:
     """One IEGMN_Layer's parameters repacked k-major for the kernels (see eqd_layer_params)."""
 
     def __init__(self, sd: Dict[str, torch.Tensor], device, skip_weight_h: float, x_connection_init: float,
-                 leaky_slope: float):
+                 leaky_slope: float, *, layer_norm_coors: str = '0', final_h_layer_norm: str = '0'):
+        """``layer_norm_coors`` / ``final_h_layer_norm`` = the module's args: 'LN' uploads coors_mlp.3.* /
+        final_h_layernorm_layer.* and sets them in the descriptor's ``norms``; '0' (the shipped checkpoints) packs exactly
+        what it packed without the options."""
+        for name, v in (('layer_norm_coors', layer_norm_coors), ('final_h_layer_norm', final_h_layer_norm)):
+            if v not in ('0', 'LN'):
+                raise ValueError(f"{name}={v!r}: the CUDA engine implements '0' and 'LN'")
+        self.layer_norm_coors, self.final_h_layer_norm = layer_norm_coors, final_h_layer_norm
         f = lambda k: _host_f32(sd[k])      # everything below is host arithmetic; ONE upload at the end
         w1, b1 = f('edge_mlp.0.weight'), f('edge_mlp.0.bias')
         wq, wk, wv = f('att_mlp_Q.0.weight'), f('att_mlp_K.0.weight'), f('att_mlp_V.0.weight')
@@ -190,6 +197,10 @@ class PackedLayer:
             'w_node1': w_node1, 'b_node1': pad(b5),
             'node_ln_g': pad(f('node_mlp.3.weight')), 'node_ln_b': pad(f('node_mlp.3.bias')),
             'w_node2': w_node2, 'b_node2': b6, 'w_edge_tc': w_edge_tc,
+            **({'_coors_ln_g': f('coors_mlp.3.weight'), '_coors_ln_b': f('coors_mlp.3.bias')}
+               if layer_norm_coors == 'LN' else {}),
+            **({'_final_ln_g': f('final_h_layernorm_layer.weight'), '_final_ln_b': f('final_h_layernorm_layer.bias')}
+               if final_h_layer_norm == 'LN' else {}),
         }, device)
         lay = nat.EqdLayer()
         s = lay.dev
@@ -203,6 +214,10 @@ class PackedLayer:
                 C.memmove(C.addressof(getattr(lay.consts, name)), flat.ctypes.data, flat.nbytes)
         s.b_coor2 = float(sd['coors_mlp.4.bias'].detach().reshape(-1)[0].item())
         s.skip_weight_h, s.x_connection_init, s.leaky_slope = skip_weight_h, x_connection_init, leaky_slope
+        if layer_norm_coors == 'LN':
+            lay.norms.coors_ln_g, lay.norms.coors_ln_b = self.t['_coors_ln_g'].data_ptr(), self.t['_coors_ln_b'].data_ptr()
+        if final_h_layer_norm == 'LN':
+            lay.norms.final_ln_g, lay.norms.final_ln_b = self.t['_final_ln_g'].data_ptr(), self.t['_final_ln_b'].data_ptr()
         self.struct = lay
         self._descriptors = {}
 

@@ -17,7 +17,9 @@ checkpoints load with ``strict=True``.  The graph argument may be a batched DGL 
 
 Scope of this engine: forward AND backward of the configuration the shipped checkpoints use
 (``nonlin='lkyrelu'``, ``layer_norm='LN'``, ``layer_norm_coors='0'``, ``final_h_layer_norm='0'``,
-``cross_msgs``, ``use_dist_in_layers``, ``rot_model='kb_att'``, ``fine_tune=False``).  ``dropout > 0`` is applied in
+``cross_msgs``, ``use_dist_in_layers``, ``rot_model='kb_att'``, ``fine_tune=False``), and ``layer_norm_coors='LN'`` (the
+coordinate MLP's ``coors_mlp.3`` LayerNorm) and ``final_h_layer_norm='LN'`` (``final_h_layernorm_layer`` on each layer's
+node output), both in the CUDA forward and backward.  ``dropout > 0`` is applied in
 training mode, as ``nn.Dropout`` does, with masks from a counter-based generator seeded per forward from torch's default
 CPU generator (``engine.draw_dropout``): same distribution as torch's, a different random stream.
 Anything else raises ``NotImplementedError``; a missing CUDA library raises -- there is no CPU path.
@@ -106,15 +108,15 @@ def compute_cross_attention(queries, keys, values, mask, cross_msgs):
 
 # ---- shared host-side plumbing -------------------------------------------------------------------
 
-_SUPPORTED = {'nonlin': 'lkyrelu', 'layer_norm': 'LN', 'layer_norm_coors': '0', 'final_h_layer_norm': '0',
-              'cross_msgs': True, 'use_dist_in_layers': True}
+# args values the CUDA engine implements (the first is the shipped checkpoints' configuration)
+_SUPPORTED = {'nonlin': ('lkyrelu',), 'layer_norm': ('LN',), 'layer_norm_coors': ('0', 'LN'), 'final_h_layer_norm': ('0', 'LN'),
+              'cross_msgs': (True,), 'use_dist_in_layers': (True,)}
 
 
 def _check_layer_args(args):
-    for k, v in _SUPPORTED.items():
-        if args[k] != v:
-            raise NotImplementedError(f"args[{k!r}]={args[k]!r}: the CUDA engine implements {v!r} only "
-                                      '(the configuration of both shipped checkpoints)')
+    for k, vs in _SUPPORTED.items():
+        if args[k] not in vs:
+            raise NotImplementedError(f"args[{k!r}]={args[k]!r}: the CUDA engine implements {' / '.join(map(repr, vs))} only")
 
 
 def _layer_plan(graph, device, max_in_degree, he_l, he_r):
@@ -173,6 +175,7 @@ class IEGMN_Layer(nn.Module):
         act = lambda: get_non_lin(args['nonlin'], slope)
         self.cross_msgs = args['cross_msgs']
         self.final_h_layer_norm = args['final_h_layer_norm']
+        self.layer_norm_coors = args['layer_norm_coors']
         self.use_dist_in_layers = args['use_dist_in_layers']
         self.skip_weight_h = args['skip_weight_h']
         self.x_connection_init = args['x_connection_init']
@@ -210,7 +213,9 @@ class IEGMN_Layer(nn.Module):
         key = (_version_key(self), str(device))
         if self._packed is None or self._packed_key != key:
             self._packed = PackedLayer(_module_state(self), device, float(self.skip_weight_h),
-                                       float(self.x_connection_init), float(self.leakyrelu_neg_slope))
+                                       float(self.x_connection_init), float(self.leakyrelu_neg_slope),
+                                       layer_norm_coors=self.layer_norm_coors,
+                                       final_h_layer_norm=self.final_h_layer_norm)
             self._packed_key = key
         return self._packed
 

@@ -98,15 +98,23 @@ Reduction = namedtuple('Reduction', 'name stage X ldx K D ldd ncols rows blocks 
 
 
 @functools.lru_cache(maxsize=None)
-def layer_reductions(dh: int, dhp: int) -> tuple:
+def layer_reductions(dh: int, dhp: int, coors_ln: bool = False, final_ln: bool = False) -> tuple:
     """The weight-gradient reductions of one IEGMN_Layer of width dh whose node rows are padded to dhp, in launch order
-    (see Reduction).  h_in and mu have row stride dhp, h0 has H0_PAD."""
+    (see Reduction); ``coors_ln`` / ``final_ln``: the layer has the coordinate LayerNorm coors_mlp.3
+    (layer_norm_coors='LN') / the final feature LayerNorm final_h_layernorm_layer (final_h_layer_norm='LN').  h_in and
+    mu have row stride dhp, h0 has H0_PAD."""
     pw = 128 + 3 * dhp                                # projection width: [Psrc | Pdst | Q | K | V]
+    edgevec = (('edge_mlp.3.weight', 0), ('edge_mlp.3.bias', 64), ('coors_mlp.4.weight', 128), ('coors_mlp.4.bias', 192))
+    if coors_ln:
+        edgevec += (('coors_mlp.3.weight', 256), ('coors_mlp.3.bias', 320))
+    nodevec = (('node_mlp.3.weight', 0), ('node_mlp.3.bias', 72))
+    if final_ln:
+        nodevec += (('final_h_layernorm_layer.weight', 144), ('final_h_layernorm_layer.bias', 208))
     ein, w1n = 2 * dh + 42, 2 * dh + 64 + nat.H0      # input widths of edge_mlp.0 and node_mlp.0
     R, B, w5 = Reduction, Block, 'node_mlp.0.weight'
     return (
         # R(name, stage, X, ldx, K, D, ldd, ncols, rows, blocks, sums): B(param, width, k0, c0, rows, cols), (param, c0)
-        R('nodevec', 'node', None, 0, 0, None, 0, 144, None, (), (('node_mlp.3.weight', 0), ('node_mlp.3.bias', 72))),
+        R('nodevec', 'node', None, 0, 0, None, 0, 272 if final_ln else 144, None, (), nodevec),
         R('node2', 'node', 'n5', dhp, dhp, 'dh_out', 64, 64, 'N', (B('node_mlp.4.weight', dh, 0, 0, dh, 64),),
           (('node_mlp.4.bias', 0),), skip=dh == nat.HID),
         R('node_h', 'node', 'h_in', dhp, dhp, 'du', dhp, dhp, 'N', (B(w5, w1n, 0, 0, dh, dh),),
@@ -115,8 +123,7 @@ def layer_reductions(dh: int, dhp: int) -> tuple:
         R('node_mu', 'node', 'mu', dhp, dhp, 'du', dhp, dhp, 'N', (B(w5, w1n, dh + 64, 0, dh, dh),)),
         R('node_h0', 'node', 'h0', nat.H0_PAD, nat.H0_PAD, 'du', dhp, dhp, 'N',
           (B(w5, w1n, 2 * dh + 64, 0, nat.H0, dh),)),
-        R('edgevec', 'edge', None, 0, 0, None, 0, 256, None, (),
-          (('edge_mlp.3.weight', 0), ('edge_mlp.3.bias', 64), ('coors_mlp.4.weight', 128), ('coors_mlp.4.bias', 192))),
+        R('edgevec', 'edge', None, 0, 0, None, 0, 384 if coors_ln else 256, None, (), edgevec),
         R('edge1', 'edge', 'ein', 44, 44, 'dz1', 64, 64, 'E', (B('edge_mlp.0.weight', ein, 2 * dh, 0, 42, 64),)),
         R('edge2', 'edge', 'n1', 64, 64, 'dmsg', 64, 64, 'E', (B('edge_mlp.4.weight', 64, 0, 0, 64, 64),),
           (('edge_mlp.4.bias', 0),)),
@@ -129,6 +136,9 @@ def layer_reductions(dh: int, dhp: int) -> tuple:
           (('edge_mlp.0.bias', 64),)),
     )
 
+
+# Floats per CTA of the widest per-CTA partial sums a stage kernel leaves in BackwardWorkspace.vec
+VEC_FLOATS = max(r.ncols for r in layer_reductions(nat.H0, nat.H0_PAD, True, True) if r.X is None)
 
 HEAD_REDUCTION = Reduction('head', 'head', 'h', 64, 64, 'dpre', 64, 64, 'N',
                            (Block('iegmn_original.mlp_h_mean_ROT.0.weight', 64, 0, 0, 64, 64),),
@@ -175,7 +185,7 @@ class LayerTrainPack:
                                'w2lin': sd['edge_mlp.4.weight'].contiguous(),
                                'w3lin': sd['coors_mlp.0.weight'].contiguous()}, device)
         self.dh, self.dhp, self.pw = dh, dhp, pw
-        self.reductions = layer_reductions(dh, dhp)
+        self.reductions = layer_reductions(dh, dhp, packed.layer_norm_coors == 'LN', packed.final_h_layer_norm == 'LN')
         self.maps = maps or reduction_maps(self.reductions, layer_module.named_parameters(), layout, device)
 
 
@@ -216,7 +226,7 @@ class BackwardWorkspace:
         lib = nat.load()
         n_partial, n_colsum = tn_workspace_floats(N, E)
         self.partial, self.colsum = f(n_partial), f(n_colsum)
-        self.vec = f(132 * 256)   # per-CTA partial sums of bwd_node / bwd_edge (grid <= EQD_SMS)
+        self.vec = f(132 * VEC_FLOATS)   # per-CTA partial sums of bwd_node / bwd_edge (grid <= EQD_SMS)
         self.head_ws_bytes = int(lib.eqd_bwd_head_workspace_bytes(N, plan.n_node_tiles, B))
         self.head_ws = torch.empty(self.head_ws_bytes, dtype=torch.uint8, device=device)
         # edges grouped by SOURCE node (ascending edge id inside a group): the transpose index of the CSR-by-destination
@@ -259,7 +269,8 @@ def layer_backward(lib, plan: GraphPlan, lp_obj: PackedLayer, tp: LayerTrainPack
 
     The layer's stashed inputs (tensors or device pointers): h_in [N][dhp] f32 (row stride 72 for the 69-wide layer 0,
     else 64), x_in [N][3] f64, aggr [N][64] f32, mu [N][dhp] f32, h0 [N][72] f32.  Upstream gradients: dh_out [N][64] f32
-    and dx_out [N][3] f64 of the layer's output features and coordinates.  Writes dh_in [N][dhp] and dx_in [N][3] f64
+    and dx_out [N][3] f64 of the layer's output features and coordinates (with the final LayerNorm on, eqd_bwd_node_mlp
+    overwrites dh_out with the gradient w.r.t. the pre-norm row, which the node_mlp.4 reductions read).  Writes dh_in [N][dhp] and dx_in [N][3] f64
     (overwritten), adds the gradient w.r.t. h0 into ws.dh0 and the parameter gradients into `flat` (through the index maps
     of `tp`).  With dhe [E][27] f32 / dx_orig [N][3] f64 given, it also adds the gradients w.r.t. the edge features and the
     original coordinates there (eqd_bwd_layer_inputs); without them that kernel is not launched.  ``desc`` is the eqd_layer

@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define EQD_ABI_VERSION 14
+#define EQD_ABI_VERSION 15
 
 #define EQD_EDGE_FEATS 27     /* input_edge_feats_dim, protein_utils.py:71-86 + :373-389 */
 #define EQD_N_RBF 15          /* all_sigmas_dist = 1.5**s, rigid_docking_model.py:116 */
@@ -167,16 +167,37 @@ typedef struct eqd_dropout {
   int32_t reserved;           /* 0 */
 } eqd_dropout;
 
+/* Optional LayerNorms of the reference's IEGMN_Layer, device pointers (all NULL = off, which is what a layer of the shipped
+ * checkpoints holds; such a layer runs exactly the kernels it ran before this descriptor existed).
+ *   coors_ln_g, coors_ln_b : [64] coors_mlp.3.weight / .bias, args['layer_norm_coors'] = 'LN': the coordinate MLP becomes
+ *                            phi = coors_mlp.4(LayerNorm(LeakyReLU(coors_mlp.0(msg)))) (nn.LayerNorm(64): eps 1e-5, biased
+ *                            variance).  Both or neither.  Read by eqd_edge_stage, eqd_edge_stage_ffma (and so
+ *                            eqd_iegmn_layer_forward, eqd_iegmn_forward) and eqd_bwd_edge.
+ *   final_ln_g, final_ln_b : [64] final_h_layernorm_layer.weight / .bias, args['final_h_layer_norm'] = 'LN': the layer's
+ *                            node output becomes h' = LayerNorm_f(skip_weight_h node_mlp(.) + (1 - skip_weight_h) h) (layer
+ *                            0: LayerNorm_f(node_mlp(.))), the last step before h' is stored; the fused next-layer
+ *                            projections read the normalised h'.  Both or neither.  Read by eqd_node_stage,
+ *                            eqd_node_mlp_tc, eqd_node_mlp_tc0 (and the node-stage, layer and whole-forward entry points
+ *                            built on them) and eqd_bwd_node_mlp.                                                      */
+typedef struct eqd_layer_norms {
+  const float* coors_ln_g;
+  const float* coors_ln_b;
+  const float* final_ln_g;
+  const float* final_ln_b;
+} eqd_layer_norms;
+
 /* One IEGMN layer as the entry points take it: a HOST-resident descriptor.  `dev` holds device pointers and scalars only
  * and is what kernels receive by value (a binding may keep or upload it wholesale); `consts` holds host VALUES.  Entry
- * points of the fp32 FFMA path and of the backward read `dev` only, plus `dropout` (sites 0-2) where it is on.
+ * points of the fp32 FFMA path and of the backward read `dev` only, plus `dropout` (sites 0-2) where it is on, plus
+ * `norms` where a LayerNorm is on.
  * Dropout runs on the fp32 CUDA-core kernels: eqd_edge_stage routes a layer with dropout on to eqd_edge_stage_ffma,
  * eqd_iegmn_forward runs its node stage with eqd_node_stage, and the tensor-core node-stage entry points refuse it
- * (EQD_ERR_UNSUPPORTED).                                                                                            */
+ * (EQD_ERR_UNSUPPORTED).  A layer with only one vector of a LayerNorm set is refused (EQD_ERR_BAD_ARG).         */
 typedef struct eqd_layer {
   eqd_layer_params dev;
   eqd_layer_consts consts;
   eqd_dropout dropout;
+  eqd_layer_norms norms;
 } eqd_layer;
 
 /* ---- keypoint read-out parameters (IEGMN.__init__ :427-438), reference layouts ------------- */
@@ -399,10 +420,14 @@ int eqd_grad_reduce(const float* partial, int32_t nchunks, int64_t stride, const
  * = the padded input blocks h | aggr | mu | h0(72)), w_node2_lin = node_mlp.4.weight as [64][dhp].  mu has row stride
  * ldmu.  Outputs: dh_in [n][dhp] (overwritten: skip path + h block), daggr [n][64], dmu [n][dhp], dh0_acc [n][72]
  * (accumulated), n5_out / du_out [n][dhp] (operands of the weight-gradient reductions), vec_partial
- * [n_partials][144] = per-CTA partials of {d node_mlp.3.weight [72], d node_mlp.3.bias [72]}.                          */
+ * [n_partials][144] = per-CTA partials of {d node_mlp.3.weight [72], d node_mlp.3.bias [72]}.
+ * With the final LayerNorm on (eqd_layer_norms.final_ln_g): the kernel recomputes the pre-norm row y from the stash, and
+ * dh_out, the gradient w.r.t. the normalised h', is OVERWRITTEN with the gradient w.r.t. y (the D operand of the
+ * node_mlp.4 weight-gradient reductions); vec_partial rows are [272], [144:208) / [208:272) = d final_h_layernorm_layer
+ * .weight / .bias.                                                                                                    */
 int eqd_bwd_node_mlp(const eqd_graph* g, const eqd_layer* p, const float* w_node1_lin, const float* w_node2_lin,
                      const float* h_in, int32_t ldh, const float* aggr, const float* mu, int32_t ldmu, const float* h0,
-                     const float* dh_out, float* dh_in, float* daggr, float* dmu, float* dh0_acc, float* n5_out,
+                     float* dh_out, float* dh_in, float* daggr, float* dmu, float* dh0_acc, float* n5_out,
                      float* du_out, float* vec_partial /* [132][144] */, int32_t* n_partials_out, void* stream);
 /* Cross attention backward (:46-64, 247-256): dmu [n][dhp] -> dP[:, 128:] = [dQpre | dKpre | dV] of the combined
  * projection-gradient matrix dP [n][128 + 3 dhp].  proj = this layer's fp32 projections (eqd_project), mu the stashed
@@ -412,11 +437,14 @@ int eqd_bwd_attention(const eqd_graph* g, const eqd_layer* p, const float* proj,
 /* Edge stage backward (:204-237, 263-292).  w2lin / w3lin = edge_mlp.4.weight / coors_mlp.0.weight [64][64] as in the
  * state_dict.  Outputs per edge: ein [E][44] = [he | rbf | 0 0], n1, msg, dz3, dmsg, dz1 [E][64], dxrel [E][3] (fp64);
  * vec_partial [n_partials][256] = per-CTA partials {d edge_mlp.3.weight [64], d edge_mlp.3.bias [64],
- * d coors_mlp.4.weight [64], d coors_mlp.4.bias [1]}.                                                                */
+ * d coors_mlp.4.weight [64], d coors_mlp.4.bias [1]}.  With the coordinate LayerNorm on (eqd_layer_norms) the rows are
+ * [n_partials][384] and [256:320) / [320:384) hold d coors_mlp.3.weight / d coors_mlp.3.bias; msg_out and dz3_out keep
+ * their meaning (dz3 = the gradient w.r.t. the coors_mlp.0 output).                                                  */
 int eqd_bwd_edge(const eqd_graph* g, const eqd_layer* p, const float* w2lin, const float* w3lin, const float* proj,
                  const double* x_in, const float* daggr, const double* dx_out, float* ein_out, float* n1_out,
                  float* msg_out, float* dz3_out, float* dmsg_out, float* dz1_out, double* dxrel_out,
-                 float* vec_partial /* [132][256] */, int32_t* n_partials_out, void* stream);
+                 float* vec_partial /* [132][256], [132][384] with the coordinate LayerNorm */, int32_t* n_partials_out,
+                 void* stream);
 /* Per node: dP[:, 0:64] = sum over OUT-edges of dz1, dP[:, 64:128] = sum over IN-edges, dx_in = (1 - eta) dx_out +
  * sum_out dxrel - sum_in dxrel.  out_ptr [n+1] / out_edge [E]: edges grouped by SOURCE node (ascending edge id).      */
 int eqd_bwd_edge_gather(const eqd_graph* g, const int32_t* out_ptr, const int32_t* out_edge, const float* dz1,
