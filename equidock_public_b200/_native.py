@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get('EQD_LIB_PATH') or os.path.join(_HERE, 'libeqd_iegmn.s
 
 ABI_VERSION = 15
 EDGE_FEATS, N_RBF, HID, H0, H0_PAD, N_RES_TYPES, HEADS, TILE_ROWS = 27, 15, 64, 69, 72, 21, 50, 128
+MAX_HEADS = 64   # EQD_MAX_HEADS: num_att_heads K may be 1..MAX_HEADS (HEADS = 50 is the shipped checkpoints' K)
 STATUS_SVD_DEGENERATE, STATUS_NAN, STATUS_DEGREE_OVERFLOW, STATUS_BAD_RESIDUE = 1, 2, 4, 8
 
 _vp, _i32, _f32 = C.c_void_p, C.c_int32, C.c_float
@@ -77,7 +78,8 @@ class EqdForwardIO(C.Structure):
 
 
 class EqdHeadParams(C.Structure):
-    _fields_ = [('w_mean', _vp), ('b_mean', _vp), ('w_key', _vp), ('w_query', _vp), ('m_qk', _vp), ('leaky_slope', _f32)]
+    _fields_ = [('w_mean', _vp), ('b_mean', _vp), ('w_key', _vp), ('w_query', _vp), ('m_qk', _vp), ('leaky_slope', _f32),
+                ('n_heads', _i32)]
 
 
 class EqdPairArchive(C.Structure):
@@ -101,6 +103,7 @@ _G, _L, _H = C.POINTER(EqdGraph), C.POINTER(EqdLayer), C.POINTER(EqdHeadParams)
 PROTOTYPES = {
     'eqd_abi_version': (C.c_int, []),
     'eqd_workspace_bytes': (C.c_size_t, [_i32, _i32, _i32]),
+    'eqd_workspace_bytes_k': (C.c_size_t, [_i32, _i32, _i32, _i32]),
     'eqd_embed': (C.c_int, [_G, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_embed_checked': (C.c_int, [_G, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_project': (C.c_int, [_G, _L, _vp, _i32, _vp, _vp]),
@@ -121,6 +124,7 @@ PROTOTYPES = {
                                           _vp]),
     'eqd_head_fold': (C.c_int, [_H, _vp, _vp]),
     'eqd_forward_workspace_bytes': (C.c_size_t, [_G]),
+    'eqd_forward_workspace_bytes_k': (C.c_size_t, [_G, _i32]),
     'eqd_iegmn_forward': (C.c_int, [_G, C.POINTER(_L), _i32, _H, C.POINTER(EqdForwardIO), _vp, C.c_size_t, _vp]),
     'eqd_forward_stash_bytes': (C.c_size_t, [_G, _i32]),
     'eqd_forward_stash_offsets': (C.c_int, [_G, _i32, C.POINTER(C.c_size_t)]),
@@ -134,12 +138,16 @@ PROTOTYPES = {
     'eqd_bwd_project': (C.c_int, [_G, _L, _vp, _vp, _vp, _vp]),
     'eqd_bwd_embed': (C.c_int, [_G, _vp, _vp, _vp, _vp, _vp, _vp]),
     'eqd_bwd_head_workspace_bytes': (C.c_size_t, [_i32, _i32, _i32]),
+    'eqd_bwd_head_workspace_bytes_k': (C.c_size_t, [_i32, _i32, _i32, _i32]),
     'eqd_bwd_head': (C.c_int, [_G, _H] + [_vp] * 9 + [C.c_size_t] + [_vp] * 6),
     'eqd_bwd_head_dropout': (C.c_int, [_G, _H, C.POINTER(EqdDropout)] + [_vp] * 9 + [C.c_size_t] + [_vp] * 6),
     'eqd_bwd_layer_inputs': (C.c_int, [_G, _L] + [_vp] * 5),
     'eqd_bwd_inputs': (C.c_int, [_G] + [_vp] * 11),
     'eqd_losses_workspace_bytes': (C.c_size_t, [_i32, _i32]),
     'eqd_losses': (C.c_int, [_G] + [_vp] * 7 + [_i32, _i32, _f32, _f32, _f32, _f32, _vp, C.c_size_t] + [_vp] * 6),
+    'eqd_losses_workspace_bytes_k': (C.c_size_t, [_i32, _i32, _i32]),
+    'eqd_losses_k': (C.c_int, [_G] + [_vp] * 4 + [_i32] + [_vp] * 3 + [_i32, _i32, _f32, _f32, _f32, _f32, _vp, C.c_size_t] +
+                     [_vp] * 6),
     'eqd_graph_build_workspace_bytes': (C.c_size_t, [_i32]),
     'eqd_graph_build_knn': (C.c_int, [_i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _f32, _i32, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     'eqd_graph_build_edges': (C.c_int, [_i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -54,6 +54,11 @@ inline int eqd_norm_on(const float* g, const float* b) { return (g != nullptr) =
 inline int eqd_coors_ln(const eqd_layer* l) { return eqd_norm_on(l->norms.coors_ln_g, l->norms.coors_ln_b); }
 inline int eqd_final_ln(const eqd_layer* l) { return eqd_norm_on(l->norms.final_ln_g, l->norms.final_ln_b); }
 
+// Keypoint count K of a head (eqd_head_params.n_heads, 0 = EQD_HEADS); 0 for a value outside [1, EQD_MAX_HEADS], which the
+// head entry points refuse with EQD_ERR_UNSUPPORTED and the sizing functions answer with 0 bytes.
+inline int eqd_valid_heads(int32_t k) { return k >= 1 && k <= EQD_MAX_HEADS ? k : 0; }
+inline int eqd_n_heads(const eqd_head_params* hp) { return eqd_valid_heads(hp->n_heads ? hp->n_heads : EQD_HEADS); }
+
 namespace eqd {
 
 // LeakyReLU for 0 <= slope <= 1 (checked by the launchers): max(v, slope*v) is bit-identical to the select form

@@ -15,7 +15,8 @@ struct Carve {
   size_t kv_bytes, x5_rows, head_bytes;
 };
 
-Carve carve(const eqd_graph* g) {
+// K = the head's keypoint count, 1..EQD_MAX_HEADS
+Carve carve(const eqd_graph* g, int K) {
   Carve c;
   const size_t N = (size_t)(g->n_nodes > 0 ? g->n_nodes : 0), B = (size_t)(g->n_pairs > 0 ? g->n_pairs : 0);
   size_t o = 0;
@@ -34,9 +35,9 @@ Carve carve(const eqd_graph* g) {
   c.kv = take(c.kv_bytes);
   c.x5_rows = ((N + 7) / 8 + 8) * 8;
   c.x5 = take(c.x5_rows * 16 * 4);
-  c.head_bytes = eqd_workspace_bytes(g->n_nodes, g->n_node_tiles, g->n_pairs);
+  c.head_bytes = eqd_workspace_bytes_k(g->n_nodes, g->n_node_tiles, g->n_pairs, K);
   c.head = take(c.head_bytes);
-  c.keypts = take(2 * B * EQD_HEADS * 3 * 8);
+  c.keypts = take(2 * B * K * 3 * 8);
   c.ymean = take(2 * B * 3 * 8);
   c.cov = take(B * 9 * 8);
   c.total = o;
@@ -45,7 +46,11 @@ Carve carve(const eqd_graph* g) {
 
 }  // namespace
 
-extern "C" size_t eqd_forward_workspace_bytes(const eqd_graph* g) { return g ? carve(g).total : 0; }
+extern "C" size_t eqd_forward_workspace_bytes_k(const eqd_graph* g, int32_t n_heads) {
+  const int K = eqd_valid_heads(n_heads);
+  return g && K ? carve(g, K).total : 0;
+}
+extern "C" size_t eqd_forward_workspace_bytes(const eqd_graph* g) { return eqd_forward_workspace_bytes_k(g, EQD_HEADS); }
 
 // ---- training stash: the per-layer inputs the backward kernels recompute from -----------------------------------------
 namespace {
@@ -90,7 +95,9 @@ extern "C" int eqd_iegmn_forward(const eqd_graph* g, const eqd_layer* const* lay
     return EQD_ERR_BAD_ARG;   // rows are written 16 bytes at a time
   for (int li = 0; li < n_layers; ++li)
     if (!layers[li]) return EQD_ERR_BAD_ARG;
-  const Carve c = carve(g);
+  const int K = eqd_n_heads(hp);
+  if (!K) return EQD_ERR_UNSUPPORTED;
+  const Carve c = carve(g, K);
   if (workspace_bytes < c.total) return EQD_ERR_WORKSPACE;
   if (reinterpret_cast<uintptr_t>(workspace) & 255) return EQD_ERR_BAD_ARG;
   if (g->n_pairs <= 0 || g->n_nodes <= 0) return EQD_OK;

@@ -1,11 +1,11 @@
 // Keypoint read-out + Kabsch (IEGMN.forward, rigid_docking_model.py:521-600) and the final rigid
 // transform of the ligand (Rigid_Body_Docking_Net.forward :657-665).  All arithmetic after the
-// mean-pooling GEMM is fp64: the 50-head softmax weights multiply last-layer coordinates that
+// mean-pooling GEMM is fp64: the K-head softmax weights multiply last-layer coordinates that
 // reach O(10^3) A, so this is where fp32 rounding would cost 1e-4 A.
 //
 // Algebra: the reference materialises keys (n x 3200) and compares them with the 3200-d query;
 //   logits[k][j] = <W_K,k h_j , W_Q,k qbar> / sqrt(64) = h_j . u_k,   u_k = (W_K,k^T W_Q,k / 8) qbar = m_qk[k]^T qbar
-// so only u (50 x 64) is formed per protein, from 50 64x64 matrices folded once per model (eqd_head_fold; SURVEY 8a
+// so only u (K x 64, K = num_att_heads) is formed per protein, from K 64x64 matrices folded once per model (eqd_head_fold; SURVEY 8a
 // row a9) -- 40x fewer FLOPs, same value up to rounding.
 #include <cstdlib>
 
@@ -16,7 +16,7 @@
 namespace eqd {
 
 #define HEAD_THREADS 256
-#define HEAD_ULD 66   // padded row stride (doubles) of u[50][64]; even: rows are read as double2
+#define HEAD_ULD 66   // padded row stride (doubles) of u[K][64]; even: rows are read as double2
 #define HEAD_HLD 66   // padded row stride (doubles) of the staged h chunk
 #define HEAD_JC 64    // nodes per staged chunk
 
@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(256) head_fold_kernel(eqd_head_params hp, doub
 // u[s][k][d] = sum_d' m_qk[k][d'][d] * qbar[partner(s)][d'].  CTA = one head k (its 32 KB fold in smem) x a stripe of
 // segments; a thread owns channels (lane, lane + 32) of 8 segments at a time (the qbar loads are warp-uniform
 // broadcasts): 4 shared + 8 global 16-byte loads feed 32 DFMAs.
-__global__ void __launch_bounds__(256) head_u_kernel(int n_pairs, const double* __restrict__ m_qk,
+__global__ void __launch_bounds__(256) head_u_kernel(int n_pairs, int K, const double* __restrict__ m_qk,
                                                      const double* __restrict__ qbar, double* __restrict__ u) {
   __shared__ double m[64][64];
   const int k = blockIdx.x, tid = threadIdx.x, nseg = 2 * n_pairs;
@@ -126,13 +126,13 @@ __global__ void __launch_bounds__(256) head_u_kernel(int n_pairs, const double* 
 #pragma unroll
     for (int j = 0; j < 8; ++j)
       if (s0 + j < nseg) {
-        u[((long)(s0 + j) * EQD_HEADS + k) * 64 + lane] = acc[j][0];
-        u[((long)(s0 + j) * EQD_HEADS + k) * 64 + lane + 32] = acc[j][1];
+        u[((long)(s0 + j) * K + k) * 64 + lane] = acc[j][0];
+        u[((long)(s0 + j) * K + k) * 64 + lane + 32] = acc[j][1];
       }
   }
 }
 
-// ---- keypoints: grid (segment, head half); 5 warps x 5 heads per CTA ------------------------------------------------
+// ---- keypoints: grid (segment, group of 25 heads); 5 warps x 5 heads per CTA -----------------------------------------
 #define KP_HEADS_PER_CTA 25
 #define KP_NH 5            // heads per warp
 #define KP_THREADS 160
@@ -142,20 +142,22 @@ struct KeypSmem {
   double xc[HEAD_JC * 3];
 };
 
-// One CTA per (protein s, 25 of the 50 heads): keypoints Y_s[k][3] (:542-560).  Warp w owns heads 25 y + 5 w + j; every
+// One CTA per (protein s, 25 of the K heads): keypoints Y_s[k][3] (:542-560).  Warp w owns heads 25 y + 5 w + j; the last
+// group holds the K - 25 y < 25 heads that are left (its other head slots compute on zero u and are not stored).  Every
 // lane keeps its OWN online-softmax state (max, sum, sum p x) per head over the rows it sees (rows lane, lane + 32 of each
 // 64-row chunk), so the chunk loop has no cross-lane traffic at all; the 32 partial states are merged once at the end.
 __global__ void __launch_bounds__(KP_THREADS, 4)
-keypoints_kernel(eqd_graph g, const float* __restrict__ h, const double* __restrict__ x,
-                 const double* __restrict__ u_all /* [2B][50][64] */, double* __restrict__ keypts) {
+keypoints_kernel(eqd_graph g, int K, const float* __restrict__ h, const double* __restrict__ x,
+                 const double* __restrict__ u_all /* [2B][K][64] */, double* __restrict__ keypts) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   KeypSmem& s = *reinterpret_cast<KeypSmem*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int seg = blockIdx.x, head0 = blockIdx.y * KP_HEADS_PER_CTA;
   const int i0 = g.seg_ptr[seg], i1 = g.seg_ptr[seg + 1];
+  const int nh = min(KP_HEADS_PER_CTA, K - head0);   // heads of this group
 
   for (int o = tid; o < KP_HEADS_PER_CTA * 64; o += KP_THREADS)
-    s.u[(o >> 6) * HEAD_ULD + (o & 63)] = u_all[((long)seg * EQD_HEADS + head0) * 64 + o];
+    s.u[(o >> 6) * HEAD_ULD + (o & 63)] = o < nh * 64 ? u_all[((long)seg * K + head0) * 64 + o] : 0.0;
 
   double m[KP_NH], l[KP_NH], sx[KP_NH], sy[KP_NH], sz[KP_NH];
 #pragma unroll
@@ -231,9 +233,9 @@ keypoints_kernel(eqd_graph g, const float* __restrict__ h, const double* __restr
     const double mm = warp_max_d(m[j]);
     const double sc = m[j] == -INFINITY ? 0.0 : exp(m[j] - mm);
     const double lt = warp_sum_d(l[j] * sc), ax = warp_sum_d(sx[j] * sc), ay = warp_sum_d(sy[j] * sc), az = warp_sum_d(sz[j] * sc);
-    if (lane == 0) {
+    if (lane == 0 && warp * KP_NH + j < nh) {
       const double inv = 1.0 / lt;
-      double* y = keypts + ((long)seg * EQD_HEADS + head0 + warp * KP_NH + j) * 3;
+      double* y = keypts + ((long)seg * K + head0 + warp * KP_NH + j) * 3;
       y[0] = ax * inv;
       y[1] = ay * inv;
       y[2] = az * inv;
@@ -242,28 +244,28 @@ keypoints_kernel(eqd_graph g, const float* __restrict__ h, const double* __restr
 }
 
 // One warp per pair: keypoint means and A = (Y_rec - mean)^T (Y_lig - mean)  (:563-567).
-__global__ void keypoint_cov_kernel(int n_pairs, const double* __restrict__ keypts, double* __restrict__ ymean,
+__global__ void keypoint_cov_kernel(int n_pairs, int K, const double* __restrict__ keypts, double* __restrict__ ymean,
                                     double* __restrict__ cov) {
   const int lane = threadIdx.x & 31;
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (b >= n_pairs) return;
-  const double* yl = keypts + (long)b * EQD_HEADS * 3;
-  const double* yr = keypts + (long)(n_pairs + b) * EQD_HEADS * 3;
+  const double* yl = keypts + (long)b * K * 3;
+  const double* yr = keypts + (long)(n_pairs + b) * K * 3;
   double ml[3], mr[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     double a = 0.0, r = 0.0;
-    for (int k = lane; k < EQD_HEADS; k += 32) {
+    for (int k = lane; k < K; k += 32) {
       a += yl[k * 3 + c];
       r += yr[k * 3 + c];
     }
-    ml[c] = warp_sum_d(a) / (double)EQD_HEADS;
-    mr[c] = warp_sum_d(r) / (double)EQD_HEADS;
+    ml[c] = warp_sum_d(a) / (double)K;
+    mr[c] = warp_sum_d(r) / (double)K;
   }
   double A[9];
 #pragma unroll
   for (int q = 0; q < 9; ++q) A[q] = 0.0;
-  for (int k = lane; k < EQD_HEADS; k += 32) {
+  for (int k = lane; k < K; k += 32) {
 #pragma unroll
     for (int r = 0; r < 3; ++r)
 #pragma unroll
@@ -369,17 +371,25 @@ extern "C" int eqd_abi_version(void) { return EQD_ABI_VERSION; }
 static inline size_t ws_part_bytes(int32_t n_node_tiles) { return eqd_align256((size_t)(n_node_tiles > 0 ? n_node_tiles : 1) * 64 * sizeof(float)); }
 static inline size_t ws_tile_ptr_bytes(int32_t n_pairs) { return eqd_align256((size_t)(2 * (n_pairs > 0 ? n_pairs : 0) + 1) * sizeof(int)); }
 static inline size_t ws_qbar_bytes(int32_t n_pairs) { return eqd_align256((size_t)2 * (n_pairs > 0 ? n_pairs : 1) * 64 * sizeof(double)); }
-static inline size_t ws_u_bytes(int32_t n_pairs) { return eqd_align256((size_t)2 * (n_pairs > 0 ? n_pairs : 1) * EQD_HEADS * 64 * sizeof(double)); }
+static inline size_t ws_u_bytes(int32_t n_pairs, int K) { return eqd_align256((size_t)2 * (n_pairs > 0 ? n_pairs : 1) * K * 64 * sizeof(double)); }
+
+extern "C" size_t eqd_workspace_bytes_k(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs, int32_t n_heads) {
+  (void)n_nodes;
+  const int K = eqd_valid_heads(n_heads);
+  if (!K) return 0;
+  // per-tile partial sums | first tile of each segment | qbar[2B][64] | u[2B][K][64]   (fp64 from qbar on)
+  return ws_part_bytes(n_node_tiles) + ws_tile_ptr_bytes(n_pairs) + ws_qbar_bytes(n_pairs) + ws_u_bytes(n_pairs, K);
+}
 
 extern "C" size_t eqd_workspace_bytes(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs) {
-  (void)n_nodes;
-  // per-tile partial sums | first tile of each segment | qbar[2B][64] | u[2B][50][64]   (fp64 from qbar on)
-  return ws_part_bytes(n_node_tiles) + ws_tile_ptr_bytes(n_pairs) + ws_qbar_bytes(n_pairs) + ws_u_bytes(n_pairs);
+  return eqd_workspace_bytes_k(n_nodes, n_node_tiles, n_pairs, EQD_HEADS);
 }
 
 extern "C" int eqd_head_fold(const eqd_head_params* hp, double* m_qk, void* stream) {
   if (!hp || !hp->w_key || !hp->w_query || !m_qk) return EQD_ERR_BAD_ARG;
-  eqd::head_fold_kernel<<<EQD_HEADS, 256, 0, (cudaStream_t)stream>>>(*hp, m_qk);
+  const int K = eqd_n_heads(hp);
+  if (!K) return EQD_ERR_UNSUPPORTED;
+  eqd::head_fold_kernel<<<K, 256, 0, (cudaStream_t)stream>>>(*hp, m_qk);
   EQD_CUDA_LAUNCH_CHECK();
   return EQD_OK;
 }
@@ -395,7 +405,9 @@ extern "C" int eqd_keypoints_dropout(const eqd_graph* g, const eqd_head_params* 
                                      double* keypts, double* ymean, double* cov, void* stream) {
   if (!g || !hp || !h || !x || !workspace || !keypts || !ymean || !cov) return EQD_ERR_BAD_ARG;
   if (!hp->m_qk || (reinterpret_cast<uintptr_t>(hp->m_qk) & 15)) return EQD_ERR_BAD_ARG;   // eqd_head_fold() output
-  if (workspace_bytes < eqd_workspace_bytes(g->n_nodes, g->n_node_tiles, g->n_pairs)) return EQD_ERR_WORKSPACE;
+  const int K = eqd_n_heads(hp);
+  if (!K) return EQD_ERR_UNSUPPORTED;
+  if (workspace_bytes < eqd_workspace_bytes_k(g->n_nodes, g->n_node_tiles, g->n_pairs, K)) return EQD_ERR_WORKSPACE;
   if (!(hp->leaky_slope >= 0.f && hp->leaky_slope <= 1.f)) return EQD_ERR_UNSUPPORTED;
   if (g->n_pairs <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;
@@ -425,19 +437,20 @@ extern "C" int eqd_keypoints_dropout(const eqd_graph* g, const eqd_head_params* 
     EQD_CUDA_LAUNCH_CHECK();
     int gy = (nseg + 63) / 64;
     if (gy > 8) gy = 8;
-    eqd::head_u_kernel<<<dim3(EQD_HEADS, gy), 256, 0, st>>>(g->n_pairs, hp->m_qk, qbar, u);
+    eqd::head_u_kernel<<<dim3(K, gy), 256, 0, st>>>(g->n_pairs, K, hp->m_qk, qbar, u);
     EQD_CUDA_LAUNCH_CHECK();
   }
   {
     size_t smem = sizeof(eqd::KeypSmem);
     EQD_SET_SMEM((eqd::keypoints_kernel), smem);
-    eqd::keypoints_kernel<<<dim3(2 * g->n_pairs, EQD_HEADS / KP_HEADS_PER_CTA), KP_THREADS, smem, st>>>(*g, h, x, u, keypts);
+    const int groups = (K + KP_HEADS_PER_CTA - 1) / KP_HEADS_PER_CTA;
+    eqd::keypoints_kernel<<<dim3(2 * g->n_pairs, groups), KP_THREADS, smem, st>>>(*g, K, h, x, u, keypts);
     EQD_CUDA_LAUNCH_CHECK();
   }
   {
     int warps_per_block = 4;
     int grid = (g->n_pairs + warps_per_block - 1) / warps_per_block;
-    eqd::keypoint_cov_kernel<<<grid, warps_per_block * 32, 0, st>>>(g->n_pairs, keypts, ymean, cov);
+    eqd::keypoint_cov_kernel<<<grid, warps_per_block * 32, 0, st>>>(g->n_pairs, K, keypts, ymean, cov);
     EQD_CUDA_LAUNCH_CHECK();
   }
   return EQD_OK;
@@ -465,7 +478,7 @@ namespace eqd {
 // constant (:586-587), A = (Y_r - ym_r)^T (Y_l - ym_l) (:567).  gA = U [ (skew(U^T gU)/E) S + S (skew(V^T gV)/E) ] V^T with
 // gU = gT V D, gV = gT^T U D, E_jk = S_k^2 - S_j^2 (torch's svd_backward; |E| >= 1e-2 is what the guard :574 enforces).
 __global__ void __launch_bounds__(128)
-kabsch_bwd_kernel(eqd_graph g, const double* __restrict__ cov, const double* __restrict__ ymean,
+kabsch_bwd_kernel(eqd_graph g, int K, const double* __restrict__ cov, const double* __restrict__ ymean,
                   const double* __restrict__ keypts, const float* __restrict__ x_lig_in, const float* __restrict__ dcoors,
                   const double* __restrict__ dY_direct, const float* __restrict__ drot, const float* __restrict__ dtrans,
                   double* __restrict__ dY) {
@@ -563,12 +576,12 @@ kabsch_bwd_kernel(eqd_graph g, const double* __restrict__ cov, const double* __r
   }
   __syncthreads();
   // dYc_r = Yc_l dA^T, dYc_l = Yc_r dA; un-centre: dY = dYc - mean_k(dYc) + dym / K
-  __shared__ double dyc[2][EQD_HEADS][3];
+  __shared__ double dyc[2][EQD_MAX_HEADS][3];
   const double* ml = ymean + (long)b * 3;
   const double* mr = ymean + (long)(B + b) * 3;
-  const double* yl = keypts + (long)b * EQD_HEADS * 3;
-  const double* yr = keypts + (long)(B + b) * EQD_HEADS * 3;
-  if (tid < EQD_HEADS) {
+  const double* yl = keypts + (long)b * K * 3;
+  const double* yr = keypts + (long)(B + b) * K * 3;
+  if (tid < K) {
     const int k = tid;
     const double cl[3] = {yl[k * 3] - ml[0], yl[k * 3 + 1] - ml[1], yl[k * 3 + 2] - ml[2]};
     const double cr[3] = {yr[k * 3] - mr[0], yr[k * 3 + 1] - mr[1], yr[k * 3 + 2] - mr[2]};
@@ -583,48 +596,48 @@ kabsch_bwd_kernel(eqd_graph g, const double* __restrict__ cov, const double* __r
   if (tid < 6) {
     const int side = tid / 3, c = tid % 3;
     double t = 0.0;
-    for (int k = 0; k < EQD_HEADS; ++k) t += dyc[side][k][c];
-    mean_d[side][c] = t / (double)EQD_HEADS;
+    for (int k = 0; k < K; ++k) t += dyc[side][k][c];
+    mean_d[side][c] = t / (double)K;
   }
   __syncthreads();
-  for (int o = tid; o < 2 * EQD_HEADS * 3; o += 128) {
-    const int side = o / (EQD_HEADS * 3), rem = o - side * EQD_HEADS * 3, k = rem / 3, c = rem - k * 3;
-    const long gi = ((long)(side == 0 ? b : B + b) * EQD_HEADS + k) * 3 + c;
-    double v = dyc[side][k][c] - mean_d[side][c] + (side == 0 ? dyml[c] : dymr[c]) / (double)EQD_HEADS;
+  for (int o = tid; o < 2 * K * 3; o += 128) {
+    const int side = o / (K * 3), rem = o - side * K * 3, k = rem / 3, c = rem - k * 3;
+    const long gi = ((long)(side == 0 ? b : B + b) * K + k) * 3 + c;
+    double v = dyc[side][k][c] - mean_d[side][c] + (side == 0 ? dyml[c] : dymr[c]) / (double)K;
     if (dY_direct) v += dY_direct[gi];
     dY[gi] = v;
   }
 }
 
 // logits[n][k] = h_n . u[seg(n)][k]   (warp per node, lanes over heads)
-__global__ void kp_logits_kernel(eqd_graph g, const int* __restrict__ node_seg, const float* __restrict__ h,
+__global__ void kp_logits_kernel(eqd_graph g, int K, const int* __restrict__ node_seg, const float* __restrict__ h,
                                  const double* __restrict__ u, double* __restrict__ logits) {
   const int n = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (n >= g.n_nodes) return;
   const int s = node_seg[n];
   const float* hr = h + (long)n * EQD_HID;
-  for (int k = lane; k < EQD_HEADS; k += 32) {
-    const double* uk = u + ((long)s * EQD_HEADS + k) * 64;
+  for (int k = lane; k < K; k += 32) {
+    const double* uk = u + ((long)s * K + k) * 64;
     double t = 0.0;
 #pragma unroll 8
     for (int d = 0; d < 64; ++d) t = fma((double)hr[d], uk[d], t);
-    logits[(long)n * EQD_HEADS + k] = t;
+    logits[(long)n * K + k] = t;
   }
 }
 
 // per (segment, head): softmax statistics over the segment's nodes and c_k = dY_k . Y_k.  stats[s][k] = {m, 1/l, c}
-__global__ void kp_stats_kernel(eqd_graph g, const double* __restrict__ logits, const double* __restrict__ keypts,
+__global__ void kp_stats_kernel(eqd_graph g, int K, const double* __restrict__ logits, const double* __restrict__ keypts,
                                 const double* __restrict__ dY, double* __restrict__ stats) {
-  const int s = blockIdx.x, k = threadIdx.x;
-  if (k >= EQD_HEADS) return;
+  const int s = blockIdx.x, k = threadIdx.x;   // 64 threads: K <= EQD_MAX_HEADS
+  if (k >= K) return;
   const int i0 = g.seg_ptr[s], i1 = g.seg_ptr[s + 1];
   double m = -INFINITY;
-  for (int i = i0; i < i1; ++i) m = fmax(m, logits[(long)i * EQD_HEADS + k]);
+  for (int i = i0; i < i1; ++i) m = fmax(m, logits[(long)i * K + k]);
   double l = 0.0;
-  for (int i = i0; i < i1; ++i) l += exp(logits[(long)i * EQD_HEADS + k] - m);
-  const double* y = keypts + ((long)s * EQD_HEADS + k) * 3;
-  const double* d = dY + ((long)s * EQD_HEADS + k) * 3;
-  double* o = stats + ((long)s * EQD_HEADS + k) * 3;
+  for (int i = i0; i < i1; ++i) l += exp(logits[(long)i * K + k] - m);
+  const double* y = keypts + ((long)s * K + k) * 3;
+  const double* d = dY + ((long)s * K + k) * 3;
+  double* o = stats + ((long)s * K + k) * 3;
   o[0] = m;
   o[1] = l > 0.0 ? 1.0 / l : 0.0;
   o[2] = d[0] * y[0] + d[1] * y[1] + d[2] * y[2];
@@ -632,23 +645,23 @@ __global__ void kp_stats_kernel(eqd_graph g, const double* __restrict__ logits, 
 
 // warp per node n: att_k = exp(logit - m_k) / l_k; dlog_k = att_k (dY_k . z_n - c_k) (overwrites logits[n][k]);
 // dz_n = sum_k att_k dY_k -> dx[n];  dh[n][d] = sum_k dlog_k u_k[d]
-__global__ void kp_node_bwd_kernel(eqd_graph g, const int* __restrict__ node_seg, const double* __restrict__ x,
+__global__ void kp_node_bwd_kernel(eqd_graph g, int K, const int* __restrict__ node_seg, const double* __restrict__ x,
                                    const double* __restrict__ u, const double* __restrict__ dY,
                                    const double* __restrict__ stats, double* __restrict__ logits,
                                    double* __restrict__ dx, float* __restrict__ dh) {
-  __shared__ double dl[8][EQD_HEADS + 2];
+  __shared__ double dl[8][EQD_MAX_HEADS + 2];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n = blockIdx.x * 8 + w;
   if (n < g.n_nodes) {
     const int s = node_seg[n];
     const double zx = x[(long)n * 3], zy = x[(long)n * 3 + 1], zz = x[(long)n * 3 + 2];
     double ax = 0.0, ay = 0.0, az = 0.0;
-    for (int k = lane; k < EQD_HEADS; k += 32) {
-      const double* st = stats + ((long)s * EQD_HEADS + k) * 3;
-      const double* d = dY + ((long)s * EQD_HEADS + k) * 3;
-      const double att = exp(logits[(long)n * EQD_HEADS + k] - st[0]) * st[1];
+    for (int k = lane; k < K; k += 32) {
+      const double* st = stats + ((long)s * K + k) * 3;
+      const double* d = dY + ((long)s * K + k) * 3;
+      const double att = exp(logits[(long)n * K + k] - st[0]) * st[1];
       const double dlog = att * (d[0] * zx + d[1] * zy + d[2] * zz - st[2]);
-      logits[(long)n * EQD_HEADS + k] = dlog;
+      logits[(long)n * K + k] = dlog;
       dl[w][k] = dlog;
       ax += att * d[0]; ay += att * d[1]; az += att * d[2];
     }
@@ -656,8 +669,8 @@ __global__ void kp_node_bwd_kernel(eqd_graph g, const int* __restrict__ node_seg
     if (lane == 0) { dx[(long)n * 3] = ax; dx[(long)n * 3 + 1] = ay; dx[(long)n * 3 + 2] = az; }
     __syncwarp();
     double a0 = 0.0, a1 = 0.0;
-    for (int k = 0; k < EQD_HEADS; ++k) {
-      const double* uk = u + ((long)s * EQD_HEADS + k) * 64;
+    for (int k = 0; k < K; ++k) {
+      const double* uk = u + ((long)s * K + k) * 64;
       a0 = fma(dl[w][k], uk[lane], a0);
       a1 = fma(dl[w][k], uk[lane + 32], a1);
     }
@@ -667,22 +680,22 @@ __global__ void kp_node_bwd_kernel(eqd_graph g, const int* __restrict__ node_seg
 }
 
 // du[s][k][d] = sum_{n in seg s} dlog[n][k] h[n][d]   (CTA per segment, fixed order over n)
-__global__ void __launch_bounds__(256) kp_du_kernel(eqd_graph g, const double* __restrict__ dlog, const float* __restrict__ h,
-                                                    double* __restrict__ du) {
+__global__ void __launch_bounds__(256) kp_du_kernel(eqd_graph g, int K, const double* __restrict__ dlog,
+                                                    const float* __restrict__ h, double* __restrict__ du) {
   const int s = blockIdx.x, i0 = g.seg_ptr[s], i1 = g.seg_ptr[s + 1];
-  for (int o = threadIdx.x; o < EQD_HEADS * 64; o += 256) {
+  for (int o = threadIdx.x; o < K * 64; o += 256) {
     const int k = o >> 6, d = o & 63;
     double t = 0.0;
-    for (int i = i0; i < i1; ++i) t = fma(dlog[(long)i * EQD_HEADS + k], (double)h[(long)i * EQD_HID + d], t);
-    du[(long)s * EQD_HEADS * 64 + o] = t;
+    for (int i = i0; i < i1; ++i) t = fma(dlog[(long)i * K + k], (double)h[(long)i * EQD_HID + d], t);
+    du[(long)s * K * 64 + o] = t;
   }
 }
 
 // CTA per head k: over all segments s (fixed order): r = W_Q,k qbar_partner(s), a = W_K,k du_{s,k} / 8,
 // dW_K,k[e][d] += r[e] du[d] / 8, dW_Q,k[e][d'] += a[e] qbar_partner[d'].  a is kept for the dqbar pass.
 __global__ void __launch_bounds__(256)
-head_weight_bwd_kernel(int n_pairs, eqd_head_params hp, const double* __restrict__ qbar, const double* __restrict__ du,
-                       double* __restrict__ a_out /*[2B][50][64]*/, float* __restrict__ g_wkey, float* __restrict__ g_wquery) {
+head_weight_bwd_kernel(int n_pairs, int K, eqd_head_params hp, const double* __restrict__ qbar, const double* __restrict__ du,
+                       double* __restrict__ a_out /*[2B][K][64]*/, float* __restrict__ g_wkey, float* __restrict__ g_wquery) {
   __shared__ float wq[64][65], wk[64][65];
   __shared__ double r[64], a[64], qb[64], dv[64];
   const int k = blockIdx.x, tid = threadIdx.x, nseg = 2 * n_pairs;
@@ -699,7 +712,7 @@ head_weight_bwd_kernel(int n_pairs, eqd_head_params hp, const double* __restrict
     __syncthreads();
     if (tid < 64) {
       qb[tid] = qbar[(long)ps * 64 + tid];
-      dv[tid] = du[((long)s * EQD_HEADS + k) * 64 + tid];
+      dv[tid] = du[((long)s * K + k) * 64 + tid];
     }
     __syncthreads();
     if (tid < 64) {
@@ -711,7 +724,7 @@ head_weight_bwd_kernel(int n_pairs, eqd_head_params hp, const double* __restrict
       double t = 0.0;
       for (int dd = 0; dd < 64; ++dd) t = fma((double)wk[e][dd], dv[dd], t);
       a[e] = t * 0.125;
-      a_out[((long)s * EQD_HEADS + k) * 64 + e] = t * 0.125;
+      a_out[((long)s * K + k) * 64 + e] = t * 0.125;
     }
     __syncthreads();
 #pragma unroll
@@ -728,12 +741,12 @@ head_weight_bwd_kernel(int n_pairs, eqd_head_params hp, const double* __restrict
 }
 
 // dqbar[p][d'] = sum_k sum_e W_Q,k[e][d'] a[partner(p)][k][e]      (CTA per segment p, 64 threads)
-__global__ void head_dqbar_kernel(int n_pairs, eqd_head_params hp, const double* __restrict__ a, double* __restrict__ dqbar) {
+__global__ void head_dqbar_kernel(int n_pairs, int K, eqd_head_params hp, const double* __restrict__ a, double* __restrict__ dqbar) {
   const int p = blockIdx.x, dq = threadIdx.x;
   const int s = p < n_pairs ? p + n_pairs : p - n_pairs;     // the segment whose keypoints used qbar_p
   double t = 0.0;
-  for (int k = 0; k < EQD_HEADS; ++k) {
-    const double* ak = a + ((long)s * EQD_HEADS + k) * 64;
+  for (int k = 0; k < K; ++k) {
+    const double* ak = a + ((long)s * K + k) * 64;
     const float* w = hp.w_query + (long)k * 4096;
     for (int e = 0; e < 64; ++e) t = fma((double)w[e * 64 + dq], ak[e], t);
   }
@@ -797,19 +810,24 @@ __global__ void node_seg_kernel(eqd_graph g, int* __restrict__ node_seg) {
 
 }  // namespace eqd
 
+extern "C" size_t eqd_bwd_head_workspace_bytes_k(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs, int32_t n_heads) {
+  const size_t N = n_nodes > 0 ? n_nodes : 1, B = n_pairs > 0 ? n_pairs : 1, K = eqd_valid_heads(n_heads);
+  if (!K) return 0;
+  return eqd_workspace_bytes_k(n_nodes, n_node_tiles, n_pairs, n_heads)      // forward intermediates (qbar, u) are recomputed
+         + eqd_align256(2 * B * K * 3 * 8) * 2 + eqd_align256(B * 9 * 8) + eqd_align256(2 * B * 3 * 8)   // keypts, dY, cov, ymean
+         + eqd_align256(N * 4) + eqd_align256(N * K * 8) + eqd_align256(2 * B * K * 3 * 8)               // node_seg, logits, stats
+         + eqd_align256(2 * B * K * 64 * 8) * 2 + eqd_align256(2 * B * 64 * 8);                           // du, a, dqbar
+}
+
 extern "C" size_t eqd_bwd_head_workspace_bytes(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs) {
-  const size_t N = n_nodes > 0 ? n_nodes : 1, B = n_pairs > 0 ? n_pairs : 1;
-  return eqd_workspace_bytes(n_nodes, n_node_tiles, n_pairs)      // forward intermediates (qbar, u) are recomputed
-         + eqd_align256(2 * B * EQD_HEADS * 3 * 8) * 2 + eqd_align256(B * 9 * 8) + eqd_align256(2 * B * 3 * 8)   // keypts, dY, cov, ymean
-         + eqd_align256(N * 4) + eqd_align256(N * EQD_HEADS * 8) + eqd_align256(2 * B * EQD_HEADS * 3 * 8)       // node_seg, logits, stats
-         + eqd_align256(2 * B * EQD_HEADS * 64 * 8) * 2 + eqd_align256(2 * B * 64 * 8);                           // du, a, dqbar
+  return eqd_bwd_head_workspace_bytes_k(n_nodes, n_node_tiles, n_pairs, EQD_HEADS);
 }
 
 // Backward of eqd_keypoints + eqd_kabsch_apply.  Inputs: last-layer h (fp32) / x (fp64), `cov` as left by the forward
-// (incl. any guard perturbation), the upstream gradients dcoors [N_l][3] (fp32, may be NULL), dkeypts [2B][50][3] (fp64,
+// (incl. any guard perturbation), the upstream gradients dcoors [N_l][3] (fp32, may be NULL), dkeypts [2B][K][3] (fp64,
 // may be NULL), drot [B][9], dtrans [B][3] (fp32, may be NULL).  Outputs: dh [n][64] (fp32, overwritten), dx [n][3]
 // (fp64, overwritten), dpre [n][64] (the D operand of d mlp_h_mean_ROT.0.weight = dpre^T h, reduced by the caller with
-// eqd_tn_gemm), and the head weight gradients accumulated into g_wkey / g_wquery (state_dict layouts [3200][64]).
+// eqd_tn_gemm), and the head weight gradients accumulated into g_wkey / g_wquery (state_dict layouts [64K][64]).
 extern "C" int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const float* h, const double* x,
                             const double* cov, const float* x_lig_in, const float* dcoors, const double* dkeypts,
                             const float* drot, const float* dtrans, void* workspace, size_t workspace_bytes, float* dh,
@@ -825,45 +843,47 @@ extern "C" int eqd_bwd_head_dropout(const eqd_graph* g, const eqd_head_params* h
                                     float* g_wkey, float* g_wquery, void* stream) {
   if (!g || !hp || !h || !x || !cov || !x_lig_in || !workspace || !dh || !dx || !dpre || !g_wkey || !g_wquery)
     return EQD_ERR_BAD_ARG;
-  if (workspace_bytes < eqd_bwd_head_workspace_bytes(g->n_nodes, g->n_node_tiles, g->n_pairs)) return EQD_ERR_WORKSPACE;
+  const int K = eqd_n_heads(hp);
+  if (!K) return EQD_ERR_UNSUPPORTED;
+  if (workspace_bytes < eqd_bwd_head_workspace_bytes_k(g->n_nodes, g->n_node_tiles, g->n_pairs, K)) return EQD_ERR_WORKSPACE;
   if (g->n_pairs <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;
   const size_t N = g->n_nodes, B = g->n_pairs;
   unsigned char* w = reinterpret_cast<unsigned char*>(workspace);
   size_t o = 0;
   auto take = [&](size_t bytes) { unsigned char* p = w + o; o += eqd_align256(bytes); return p; };
-  const size_t fwd_bytes = eqd_workspace_bytes(g->n_nodes, g->n_node_tiles, g->n_pairs);
+  const size_t fwd_bytes = eqd_workspace_bytes_k(g->n_nodes, g->n_node_tiles, g->n_pairs, K);
   unsigned char* fwd_ws = take(fwd_bytes);
-  double* keypts = reinterpret_cast<double*>(take(2 * B * EQD_HEADS * 3 * 8));
-  double* dY = reinterpret_cast<double*>(take(2 * B * EQD_HEADS * 3 * 8));
+  double* keypts = reinterpret_cast<double*>(take(2 * B * K * 3 * 8));
+  double* dY = reinterpret_cast<double*>(take(2 * B * K * 3 * 8));
   double* cov_scratch = reinterpret_cast<double*>(take(B * 9 * 8));
   double* ymean = reinterpret_cast<double*>(take(2 * B * 3 * 8));
   int* node_seg = reinterpret_cast<int*>(take(N * 4));
-  double* logits = reinterpret_cast<double*>(take(N * EQD_HEADS * 8));
-  double* stats = reinterpret_cast<double*>(take(2 * B * EQD_HEADS * 3 * 8));
-  double* du = reinterpret_cast<double*>(take(2 * B * EQD_HEADS * 64 * 8));
-  double* a = reinterpret_cast<double*>(take(2 * B * EQD_HEADS * 64 * 8));
+  double* logits = reinterpret_cast<double*>(take(N * K * 8));
+  double* stats = reinterpret_cast<double*>(take(2 * B * K * 3 * 8));
+  double* du = reinterpret_cast<double*>(take(2 * B * K * 64 * 8));
+  double* a = reinterpret_cast<double*>(take(2 * B * K * 64 * 8));
   double* dqbar = reinterpret_cast<double*>(take(2 * B * 64 * 8));
   // recompute qbar, u, keypoints and their means (cov_scratch is discarded: the caller's cov may carry the guard's noise)
   int rc = eqd_keypoints_dropout(g, hp, dropout, h, x, fwd_ws, fwd_bytes, keypts, ymean, cov_scratch, stream);
   if (rc) return rc;
   const double* qbar = reinterpret_cast<const double*>(fwd_ws + ws_part_bytes(g->n_node_tiles) + ws_tile_ptr_bytes(g->n_pairs));
   const double* u = reinterpret_cast<const double*>(reinterpret_cast<const unsigned char*>(qbar) + ws_qbar_bytes(g->n_pairs));
-  eqd::kabsch_bwd_kernel<<<g->n_pairs, 128, 0, st>>>(*g, cov, ymean, keypts, x_lig_in, dcoors, dkeypts, drot, dtrans, dY);
+  eqd::kabsch_bwd_kernel<<<g->n_pairs, 128, 0, st>>>(*g, K, cov, ymean, keypts, x_lig_in, dcoors, dkeypts, drot, dtrans, dY);
   EQD_CUDA_LAUNCH_CHECK();
   eqd::node_seg_kernel<<<2 * g->n_pairs, 128, 0, st>>>(*g, node_seg);
   EQD_CUDA_LAUNCH_CHECK();
-  eqd::kp_logits_kernel<<<(unsigned)((N * 32 + 255) / 256), 256, 0, st>>>(*g, node_seg, h, u, logits);
+  eqd::kp_logits_kernel<<<(unsigned)((N * 32 + 255) / 256), 256, 0, st>>>(*g, K, node_seg, h, u, logits);
   EQD_CUDA_LAUNCH_CHECK();
-  eqd::kp_stats_kernel<<<2 * g->n_pairs, 64, 0, st>>>(*g, logits, keypts, dY, stats);
+  eqd::kp_stats_kernel<<<2 * g->n_pairs, 64, 0, st>>>(*g, K, logits, keypts, dY, stats);
   EQD_CUDA_LAUNCH_CHECK();
-  eqd::kp_node_bwd_kernel<<<(unsigned)((N + 7) / 8), 256, 0, st>>>(*g, node_seg, x, u, dY, stats, logits, dx, dh);
+  eqd::kp_node_bwd_kernel<<<(unsigned)((N + 7) / 8), 256, 0, st>>>(*g, K, node_seg, x, u, dY, stats, logits, dx, dh);
   EQD_CUDA_LAUNCH_CHECK();
-  eqd::kp_du_kernel<<<2 * g->n_pairs, 256, 0, st>>>(*g, logits, h, du);
+  eqd::kp_du_kernel<<<2 * g->n_pairs, 256, 0, st>>>(*g, K, logits, h, du);
   EQD_CUDA_LAUNCH_CHECK();
-  eqd::head_weight_bwd_kernel<<<EQD_HEADS, 256, 0, st>>>(g->n_pairs, *hp, qbar, du, a, g_wkey, g_wquery);
+  eqd::head_weight_bwd_kernel<<<K, 256, 0, st>>>(g->n_pairs, K, *hp, qbar, du, a, g_wkey, g_wquery);
   EQD_CUDA_LAUNCH_CHECK();
-  eqd::head_dqbar_kernel<<<2 * g->n_pairs, 64, 0, st>>>(g->n_pairs, *hp, a, dqbar);
+  eqd::head_dqbar_kernel<<<2 * g->n_pairs, 64, 0, st>>>(g->n_pairs, K, *hp, a, dqbar);
   EQD_CUDA_LAUNCH_CHECK();
   const eqd_dropout dr = dropout ? *dropout : eqd_dropout{};
   if (dr.p > 0.f)

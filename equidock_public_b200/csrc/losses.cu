@@ -2,10 +2,10 @@
 //   * per-pair MSE of the predicted ligand C-alpha coordinates (nn.MSELoss, src/train.py:114)
 //   * body-intersection loss (src/train.py:41-49, 131-133): two n x m Gaussian log-sum reductions
 //   * pocket OT loss (src/train.py:125-129, src/utils/ot_utils.py:5-29): cost = |P_l - Y_l|^2 + |P_r - Y_r|^2 between the
-//     N_pocket pocket points and the 50 keypoints, EXACT earth mover's distance with uniform marginals.  The reference calls
+//     N_pocket pocket points and the K keypoints (num_att_heads, 1..64), EXACT earth mover's distance with uniform marginals.  The reference calls
 //     POT's network simplex on the CPU (ot.emd, a D2H/H2D round trip per pair); here the transport LP is solved on the SM
 //     by successive shortest augmenting paths with node potentials (primal-dual; Dijkstra on the dense bipartite residual
-//     graph, integer flows in units of 1/(N_pocket * 50)), which terminates at the LP optimum -- the unique optimal VALUE any
+//     graph, integer flows in units of 1/(N_pocket * K)), which terminates at the LP optimum -- the unique optimal VALUE any
 //     exact solver returns.  The plan is a constant for the gradient (ot_utils.py:27): dY = 2 sum_i T_ik (Y_k - P_i).
 // Everything in fp64; all reductions in a fixed order.  Restated in oracle/loss_oracle.py.
 #include "common.cuh"
@@ -89,8 +89,9 @@ loss_mse_intersection_kernel(eqd_graph g, const float* __restrict__ pred, const 
 }
 
 // Per-CTA state of the transport solver, carved from dynamic shared memory for a pocket capacity `cap` (the largest pocket
-// of the batch).  The cost matrix C (fp64, cap x 50) and the per-sink source lists (int16) live in shared memory when they
-// fit (cap <= 310: both; <= 370: C only; <= 870: lists only), else in global memory (L2); flows x_ik <= 50 are int8.
+// of the batch) and M = K keypoints.  The cost matrix C (fp64, cap x M) and the per-sink source lists (int16) live in shared
+// memory when they fit (M = 50: cap <= 310: both; <= 370: C only; <= 870: lists only), else in global memory (L2); flows
+// x_ik <= M <= 64 are int8.
 struct OtView {
   double *P, *Y, *u, *v, *base_v, *Cm;
   double *Wv, *dsink;          // sink graph: Wv[k][64] = min over the feeders i of sink k of C[i][.] - u[i]; settle distances
@@ -103,10 +104,10 @@ struct OtLayout {
   size_t bytes;
   int c_smem, fl_smem;
 };
-__host__ __device__ inline OtLayout ot_layout(int cap) {
-  const size_t fixed = (size_t)(cap * 6 + EQD_HEADS * 6 + cap + 2 * EQD_HEADS + EQD_HEADS * OT_WLD + OT_WLD) * 8 +
-                       (size_t)(4 * cap + 5 * EQD_HEADS + OT_WLD) * 4 + (size_t)EQD_HEADS * OT_WLD * 2 + (size_t)cap * EQD_HEADS + 256;
-  const size_t cbytes = (size_t)cap * EQD_HEADS * 8, fbytes = (size_t)cap * EQD_HEADS * 2;
+__host__ __device__ inline OtLayout ot_layout(int cap, int M) {
+  const size_t fixed = (size_t)(cap * 6 + M * 6 + cap + 2 * M + M * OT_WLD + OT_WLD) * 8 +
+                       (size_t)(4 * cap + 5 * M + OT_WLD) * 4 + (size_t)M * OT_WLD * 2 + (size_t)cap * M + 256;
+  const size_t cbytes = (size_t)cap * M * 8, fbytes = (size_t)cap * M * 2;
   const size_t lim = 227 * 1024 - 2048;      // static shared memory of the kernel is ~1.5 KB
   OtLayout L;
   L.c_smem = fixed + cbytes <= lim;
@@ -114,31 +115,31 @@ __host__ __device__ inline OtLayout ot_layout(int cap) {
   L.bytes = fixed + (L.c_smem ? cbytes : 0) + (L.fl_smem ? fbytes : 0);
   return L;
 }
-__device__ inline OtView ot_carve(unsigned char* base, int cap, const OtLayout& L, double* c_global, short* fl_global) {
+__device__ inline OtView ot_carve(unsigned char* base, int cap, int M, const OtLayout& L, double* c_global, short* fl_global) {
   OtView s;
   double* d = reinterpret_cast<double*>(base);
   s.P = d; d += cap * 6;
-  s.Y = d; d += EQD_HEADS * 6;
+  s.Y = d; d += M * 6;
   s.u = d; d += cap;
-  s.v = d; d += EQD_HEADS;
-  s.base_v = d; d += EQD_HEADS;
-  s.Wv = d; d += EQD_HEADS * OT_WLD;
+  s.v = d; d += M;
+  s.base_v = d; d += M;
+  s.Wv = d; d += M * OT_WLD;
   s.dsink = d; d += OT_WLD;
-  if (L.c_smem) { s.Cm = d; d += (size_t)cap * EQD_HEADS; } else s.Cm = c_global;
+  if (L.c_smem) { s.Cm = d; d += (size_t)cap * M; } else s.Cm = c_global;
   int* i = reinterpret_cast<int*>(d);
   s.excess = i; i += cap;
   s.exl = i; i += cap;
   s.exq = i; i += cap;
   s.stamp = i; i += cap;
-  s.deficit = i; i += EQD_HEADS;
-  s.par_k = i; i += EQD_HEADS;
-  s.par_via = i; i += EQD_HEADS;
-  s.fl_cnt = i; i += EQD_HEADS;
-  s.base_i = i; i += EQD_HEADS;
+  s.deficit = i; i += M;
+  s.par_k = i; i += M;
+  s.par_via = i; i += M;
+  s.fl_cnt = i; i += M;
+  s.base_i = i; i += M;
   s.ord = i; i += OT_WLD;
   short* h = reinterpret_cast<short*>(i);
-  s.Wi = h; h += EQD_HEADS * OT_WLD;
-  if (L.fl_smem) { s.fls = h; h += (size_t)cap * EQD_HEADS; } else s.fls = fl_global;
+  s.Wi = h; h += M * OT_WLD;
+  if (L.fl_smem) { s.fls = h; h += (size_t)cap * M; } else s.fls = fl_global;
   s.xs = reinterpret_cast<signed char*>(h);
   return s;
 }
@@ -156,11 +157,11 @@ __device__ __forceinline__ void warp_argmin(double& v, int& k) {
 }
 
 // One CTA per pair: successive shortest augmenting paths with node potentials on the transport problem scaled to integers
-// (supply 50 per pocket point, demand n per keypoint, n * 50 units in all).
+// (supply M = K per pocket point, demand n per keypoint, n * M units in all).
 //   * Forward arcs form a complete bipartite graph and backward arcs (k -> i, x_ik > 0) have reduced cost 0 (complementary
-//     slackness), so the search only has to SETTLE SINKS; it runs on the sink graph (50 nodes): a settled sink k reaches the
+//     slackness), so the search only has to SETTLE SINKS; it runs on the sink graph (M <= 64 nodes): a settled sink k reaches the
 //     sources that feed it for free, hence every sink k' at  W[k][k'] - v[k'],  W[k][k'] = min over the feeders i of k of
-//     (C[i][k'] - u[i]).  Every augmentation starts with all four warps rebuilding W (50 x 50 minima over the ~n + 50
+//     (C[i][k'] - u[i]).  Every augmentation starts with all four warps rebuilding W (M x M minima over the ~n + M
 //     non-zero flows, independent loads); the Dijkstra itself then runs in warp 0 out of registers -- lane l owns sinks l
 //     and l + 32 -- with one shared-memory row read per settled sink.  All unsettled sinks at the current minimum distance
 //     are settled in one round (arc lengths >= 0; with potentials most of the search happens at distance 0).
@@ -170,18 +171,17 @@ __device__ __forceinline__ void warp_argmin(double& v, int& k) {
 //     offset, so their contribution to the initial sink distances, base[k] = min_i (C_ik - u_i), changes only when the
 //     minimiser leaves the excess set.
 //   * All minima are lexicographic in (value, index): the plan does not depend on list or lane order.
-// The final flows are written to flow[(p0 + i) * 50 + k] (int32, global).
+// The final flows are written to flow[(p0 + i) * M + k] (int32, global).
 __global__ void __launch_bounds__(LOSS_THREADS)
-ot_emd_kernel(int n_pairs, int cap, const int* __restrict__ pocket_ptr, const float* __restrict__ pocket_lig,
+ot_emd_kernel(int n_pairs, int cap, int M, const int* __restrict__ pocket_ptr, const float* __restrict__ pocket_lig,
               const float* __restrict__ pocket_rec, const double* __restrict__ keypts, double w_ot,
               int* __restrict__ flow, short* __restrict__ lists_g, double* __restrict__ cost_g, double* __restrict__ parts,
               double* __restrict__ dkeypts, int* __restrict__ err) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int b = blockIdx.x, tid = threadIdx.x, B = n_pairs;
   const int p0 = pocket_ptr[b], n = pocket_ptr[b + 1] - p0;
-  constexpr int M = EQD_HEADS;
-  const OtLayout L = ot_layout(cap);
-  const OtView s = ot_carve(smem_raw, cap, L, cost_g + (long)p0 * M, lists_g + (long)p0 * M);
+  const OtLayout L = ot_layout(cap, M);
+  const OtView s = ot_carve(smem_raw, cap, M, L, cost_g + (long)p0 * M, lists_g + (long)p0 * M);
   __shared__ double red[LOSS_THREADS];
   __shared__ int redi[LOSS_THREADS];
   if (n <= 0 || n > cap) {
@@ -254,8 +254,8 @@ ot_emd_kernel(int n_pairs, int cap, const int* __restrict__ pocket_ptr, const fl
   __shared__ int sh_mass, sh_fail;
   {
     const int lane = tid & 31, warp = tid >> 5;
-    const int k0 = lane, k1 = lane + 32;               // the two sinks a lane owns (k1 valid iff < M)
-    const bool has1 = k1 < M;
+    const int k0 = lane, k1 = lane + 32;               // the two sinks a lane owns (each valid iff < M)
+    const bool has0 = k0 < M, has1 = k1 < M;
     int mass = n * M, nex = n, epoch = 0, fail = 0;    // solver state: warp 0
     double u_ex_off = 0.0;
     const long max_aug = 64L * (n + M) + 1024;
@@ -282,7 +282,7 @@ ot_emd_kernel(int n_pairs, int cap, const int* __restrict__ pocket_ptr, const fl
           for (int t = 0; t < 4; ++t) {
             ex[t] = s.excess[ii[t]];
             ui[t] = s.u[ii[t]];
-            c0[t] = s.Cm[ii[t] * M + k0];
+            c0[t] = has0 ? s.Cm[ii[t] * M + k0] : INFINITY;
             c1[t] = has1 ? s.Cm[ii[t] * M + k1] : INFINITY;
           }
 #pragma unroll
@@ -295,9 +295,9 @@ ot_emd_kernel(int n_pairs, int cap, const int* __restrict__ pocket_ptr, const fl
           }
         }
         // stored as arc lengths k -> k': W - v[k'] clamped at 0 (reduced costs are >= 0 up to rounding)
-        s.Wv[k * OT_WLD + k0] = fmax(w0 - s.v[k0], 0.0);
+        s.Wv[k * OT_WLD + k0] = has0 ? fmax(w0 - s.v[k0], 0.0) : INFINITY;
         s.Wv[k * OT_WLD + k1] = has1 ? fmax(w1 - s.v[k1], 0.0) : INFINITY;
-        s.Wi[k * OT_WLD + k0] = (short)(i0 == 0x7fffffff ? -1 : i0);
+        s.Wi[k * OT_WLD + k0] = (short)(i0 == 0x7fffffff || !has0 ? -1 : i0);
         s.Wi[k * OT_WLD + k1] = (short)(i1 == 0x7fffffff || !has1 ? -1 : i1);
       }
       __syncthreads();
@@ -305,12 +305,13 @@ ot_emd_kernel(int n_pairs, int cap, const int* __restrict__ pocket_ptr, const fl
         // ---- B: Dijkstra over the sinks (lane l owns sinks l and l + 32: distances and parents in registers).  All unsettled
         // sinks at the current minimum distance are settled in one round (arc lengths >= 0); a deficit among them ends the search.
         // (+ 0.0 turns a -0.0 into +0.0: warp_argmin orders distances by their bit patterns)
-        double d0 = fmax(s.base_v[k0] - u_ex_off - s.v[k0], 0.0) + 0.0, d1 = has1 ? fmax(s.base_v[k1] - u_ex_off - s.v[k1], 0.0) + 0.0 : INFINITY;
-        int p0_ = s.base_i[k0], p1_ = has1 ? s.base_i[k1] : -1;     // parent source ...
+        double d0 = has0 ? fmax(s.base_v[k0] - u_ex_off - s.v[k0], 0.0) + 0.0 : INFINITY,
+               d1 = has1 ? fmax(s.base_v[k1] - u_ex_off - s.v[k1], 0.0) + 0.0 : INFINITY;
+        int p0_ = has0 ? s.base_i[k0] : -1, p1_ = has1 ? s.base_i[k1] : -1;   // parent source ...
         int via0 = -1, via1 = -1;                                   // ... and the sink it was reached through (-1: it has excess)
-        const double v0 = s.v[k0], v1 = has1 ? s.v[k1] : 0.0;
-        const bool def0 = s.deficit[k0] > 0, def1 = has1 && s.deficit[k1] > 0;   // deficits do not change during a search
-        bool set0 = false, set1 = !has1;
+        const double v0 = has0 ? s.v[k0] : 0.0, v1 = has1 ? s.v[k1] : 0.0;
+        const bool def0 = has0 && s.deficit[k0] > 0, def1 = has1 && s.deficit[k1] > 0;   // deficits do not change during a search
+        bool set0 = !has0, set1 = !has1;                            // a lane's sinks past M never take part
         int target = -1, nord = 0;
         double D = 0.0;
         for (int round = 0; round <= M; ++round) {
@@ -353,12 +354,12 @@ ot_emd_kernel(int n_pairs, int cap, const int* __restrict__ pocket_ptr, const fl
         if (target < 0) fail |= 2;
         int left = -1;                                   // a source that just lost its last unit of excess
         if (!fail) {
-          if (set0 || k0 == target) { s.par_k[k0] = p0_; s.par_via[k0] = via0; }
+          if (has0 && (set0 || k0 == target)) { s.par_k[k0] = p0_; s.par_via[k0] = via0; }
           if (has1 && (set1 || k1 == target)) { s.par_k[k1] = p1_; s.par_via[k1] = via1; }
           // ---- C: potentials (kept modulo the common shift of an augmentation: u += D everywhere, v -= D everywhere leaves every
           // reduced cost unchanged).  Settled sinks: v -= D - d; a source without excess that feeds a settled sink was reached at
           // that sink's distance (the first one in settle order): u += D - d; the sources with excess share the lazy offset.
-          if (set0) s.v[k0] = v0 - (D - d0);
+          if (has0 && set0) s.v[k0] = v0 - (D - d0);
           if (has1 && set1) s.v[k1] = v1 - (D - d1);
           __syncwarp();
           for (int o = 0; o < nord; ++o) {
@@ -507,31 +508,49 @@ __global__ void loss_total_kernel(int n_pairs, const double* __restrict__ parts,
 
 }  // namespace eqd
 
-extern "C" size_t eqd_losses_workspace_bytes(int32_t n_rec_nodes, int32_t n_pocket_total) {
+extern "C" size_t eqd_losses_workspace_bytes_k(int32_t n_rec_nodes, int32_t n_pocket_total, int32_t n_heads) {
+  const int M = eqd_valid_heads(n_heads);
+  if (!M) return 0;
   const size_t a = ((size_t)(n_rec_nodes > 0 ? n_rec_nodes : 1) * 8 + 255) & ~(size_t)255;
-  const size_t f = ((size_t)(n_pocket_total > 0 ? n_pocket_total : 1) * EQD_HEADS * 4 + 255) & ~(size_t)255;
+  const size_t f = ((size_t)(n_pocket_total > 0 ? n_pocket_total : 1) * M * 4 + 255) & ~(size_t)255;
   return a + f + f / 2 + 256 + 2 * f + 256;      // flows (int32), per-sink source lists (int16), cost matrix (fp64)
 }
 
-// parts[B][4] = {mse, ot, intersection, -} per pair; total[4] = {loss, mean mse, mean ot, mean intersection};
-// dcoors [N_l][3] fp32 and dkeypts [2B][50][3] fp64 = gradients of `loss`; plan_flow (inside the workspace) keeps the
-// integer transport plans.  err_flags (device int, zeroed by the call) != 0 reports a pocket larger than 1024 or a solver
-// failure.
+extern "C" size_t eqd_losses_workspace_bytes(int32_t n_rec_nodes, int32_t n_pocket_total) {
+  return eqd_losses_workspace_bytes_k(n_rec_nodes, n_pocket_total, EQD_HEADS);
+}
+
 extern "C" int eqd_losses(const eqd_graph* g, const float* pred_lig, const float* bound_lig, const float* bound_rec,
                           const double* keypts, const int32_t* pocket_ptr, const float* pocket_lig,
                           const float* pocket_rec, int32_t n_pocket_total, int32_t max_pocket, float w_ot, float w_int, float sigma,
                           float surface_ct, void* workspace, size_t workspace_bytes, double* parts, double* total,
                           float* dcoors, double* dkeypts, int32_t* err_flags, void* stream) {
+  return eqd_losses_k(g, pred_lig, bound_lig, bound_rec, keypts, EQD_HEADS, pocket_ptr, pocket_lig, pocket_rec,
+                      n_pocket_total, max_pocket, w_ot, w_int, sigma, surface_ct, workspace, workspace_bytes, parts, total,
+                      dcoors, dkeypts, err_flags, stream);
+}
+
+// parts[B][4] = {mse, ot, intersection, -} per pair; total[4] = {loss, mean mse, mean ot, mean intersection};
+// dcoors [N_l][3] fp32 and dkeypts [2B][K][3] fp64 = gradients of `loss`; plan_flow (inside the workspace) keeps the
+// integer transport plans.  err_flags (device int, zeroed by the call) != 0 reports a pocket larger than 1024 or a solver
+// failure.
+extern "C" int eqd_losses_k(const eqd_graph* g, const float* pred_lig, const float* bound_lig, const float* bound_rec,
+                            const double* keypts, int32_t n_heads, const int32_t* pocket_ptr, const float* pocket_lig,
+                            const float* pocket_rec, int32_t n_pocket_total, int32_t max_pocket, float w_ot, float w_int,
+                            float sigma, float surface_ct, void* workspace, size_t workspace_bytes, double* parts,
+                            double* total, float* dcoors, double* dkeypts, int32_t* err_flags, void* stream) {
   if (!g || !pred_lig || !bound_lig || !bound_rec || !keypts || !pocket_ptr || !pocket_lig || !pocket_rec || !workspace ||
       !parts || !total || !dcoors || !dkeypts || !err_flags)
     return EQD_ERR_BAD_ARG;
+  const int M = eqd_valid_heads(n_heads);
+  if (!M) return EQD_ERR_UNSUPPORTED;
   const int n_rec = g->n_nodes - g->n_lig_nodes;
-  if (workspace_bytes < eqd_losses_workspace_bytes(n_rec, n_pocket_total)) return EQD_ERR_WORKSPACE;
+  if (workspace_bytes < eqd_losses_workspace_bytes_k(n_rec, n_pocket_total, M)) return EQD_ERR_WORKSPACE;
   if (g->n_pairs <= 0) return EQD_OK;
   cudaStream_t st = (cudaStream_t)stream;
   unsigned char* w = reinterpret_cast<unsigned char*>(workspace);
   double* wrec = reinterpret_cast<double*>(w);
-  const size_t fbytes = ((size_t)(n_pocket_total > 0 ? n_pocket_total : 1) * EQD_HEADS * 4 + 255) & ~(size_t)255;
+  const size_t fbytes = ((size_t)(n_pocket_total > 0 ? n_pocket_total : 1) * M * 4 + 255) & ~(size_t)255;
   int* flow = reinterpret_cast<int*>(w + (((size_t)(n_rec > 0 ? n_rec : 1) * 8 + 255) & ~(size_t)255));
   short* lists = reinterpret_cast<short*>(reinterpret_cast<unsigned char*>(flow) + fbytes);
   double* cost = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(lists) + fbytes / 2 + 256 - ((fbytes / 2) & 255));
@@ -543,9 +562,9 @@ extern "C" int eqd_losses(const eqd_graph* g, const float* pred_lig, const float
   EQD_CUDA_LAUNCH_CHECK();
   int cap = max_pocket > 0 ? max_pocket : 1;
   if (cap > OT_MAX_POCKET) cap = OT_MAX_POCKET;            // larger pockets are flagged by the kernel (err bit 1)
-  const size_t smem = eqd::ot_layout(cap).bytes;
+  const size_t smem = eqd::ot_layout(cap, M).bytes;
   EQD_SET_SMEM((eqd::ot_emd_kernel), smem);
-  eqd::ot_emd_kernel<<<g->n_pairs, LOSS_THREADS, smem, st>>>(g->n_pairs, cap, pocket_ptr, pocket_lig, pocket_rec, keypts,
+  eqd::ot_emd_kernel<<<g->n_pairs, LOSS_THREADS, smem, st>>>(g->n_pairs, cap, M, pocket_ptr, pocket_lig, pocket_rec, keypts,
                                                             (double)w_ot, flow, lists, cost, parts, dkeypts, err_flags);
   EQD_CUDA_LAUNCH_CHECK();
   eqd::loss_total_kernel<<<1, 32, 0, st>>>(g->n_pairs, parts, (double)w_ot, (double)w_int, total);

@@ -236,9 +236,9 @@ class PackedLayer:
 
 class PackedHead:
     """Head parameters for the kernels.  mlp_h_mean_ROT's weight is needed k-major (transposed, 64 x 64: one tiny copy); the
-    3200 x 64 key / query projections and the bias are used IN PLACE when they already are fp32, contiguous, 16-byte
-    aligned device tensors (the normal case: no 1.6 MB round trip through the host per parameter version), else
-    through one host-packed upload."""
+    64K x 64 key / query projections (K = num_att_heads keypoints, 1..MAX_HEADS) and the bias are used IN PLACE when they
+    already are fp32, contiguous, 16-byte aligned device tensors (the normal case: no 1.6 MB round trip through the host
+    per parameter version at K = 50), else through one host-packed upload."""
 
     def __init__(self, w_mean, b_mean, w_key, w_query, device, leaky_slope: float):
         dev = torch.device(device)
@@ -250,15 +250,18 @@ class PackedHead:
         else:
             self.t = _upload_blob({'w_mean': _host_f32(w_mean).t().contiguous(), 'b_mean': _host_f32(b_mean),
                                    'w_key': _host_f32(w_key), 'w_query': _host_f32(w_query)}, device)
-        assert self.t['w_key'].shape == (nat.HEADS * nat.HID, nat.HID)
+        self.n_heads = self.t['w_key'].shape[0] // nat.HID
+        assert 1 <= self.n_heads <= nat.MAX_HEADS and self.t['w_key'].shape == (self.n_heads * nat.HID, nat.HID)
+        assert self.t['w_query'].shape == self.t['w_key'].shape
         s = nat.EqdHeadParams()
         for k, v in self.t.items():
             if not k.startswith('_'):
                 setattr(s, k, v.data_ptr())
         s.leaky_slope = leaky_slope
+        s.n_heads = self.n_heads
         self.struct = s
-        # weights-only fold of the 50-head key / query projections (eqd_head_fold), done once per parameter version on the device
-        self.m_qk = torch.empty(nat.HEADS, nat.HID, nat.HID, dtype=torch.float64, device=device)
+        # weights-only fold of the K-head key / query projections (eqd_head_fold), done once per parameter version on the device
+        self.m_qk = torch.empty(self.n_heads, nat.HID, nat.HID, dtype=torch.float64, device=device)
         with torch.cuda.device(device):
             nat.check(nat.load().eqd_head_fold(C.byref(s), self.m_qk.data_ptr(), torch.cuda.current_stream().cuda_stream),
                       'eqd_head_fold')
@@ -330,7 +333,7 @@ class GraphPlan:
         ``n_lig_edges`` is the number of edges whose features are rows of ``he_l`` (the rest are rows of ``he_r``);
         ``unsorted`` = None: the edges are known to be grouped by destination."""
         self.n_pairs = len(n_lig)
-        self.forward_ws_bytes = None   # eqd_forward_workspace_bytes(), filled on first use
+        self.forward_ws_bytes = {}     # keypoint count K -> eqd_forward_workspace_bytes_k(), filled on first use
         self.n_lig_list, self.n_rec_list = [int(v) for v in n_lig], [int(v) for v in n_rec]
         self.N_l, self.N_r = sum(self.n_lig_list), sum(self.n_rec_list)
         self.N = self.N_l + self.N_r
@@ -573,14 +576,16 @@ class IEGMNEngine:
             res_l, res_r, mu_l, mu_r, x_l, x_r = map(cf, (res_l, res_r, mu_l, mu_r, x_l, x_r))
             assert x_l.shape == (plan.N_l, 3) and x_r.shape == (plan.N_r, 3)
             g = C.byref(plan.struct)
-            if plan.forward_ws_bytes is None:
-                plan.forward_ws_bytes = int(lib.eqd_forward_workspace_bytes(g))
-            ws = torch.empty(plan.forward_ws_bytes, dtype=torch.uint8, device=dev)
+            K = head.n_heads
+            if K not in plan.forward_ws_bytes:
+                plan.forward_ws_bytes[K] = int(lib.eqd_forward_workspace_bytes_k(g, K))
+            ws_bytes = plan.forward_ws_bytes[K]
+            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
             # outputs (separate allocations: the kernels assume 16-byte aligned rows)
             rot, trans = torch.empty(B, 3, 3, **f32), torch.empty(B, 1, 3, **f32)
             lig_out, h_fin = torch.empty(plan.N_l, 3, **f32), torch.empty(N, nat.HID, **f32)
             sing, x_fin = torch.empty(B, 3, **f64), torch.empty(N, 3, **f64)
-            keyp = torch.empty(2 * B, nat.HEADS, 3, **f64)
+            keyp = torch.empty(2 * B, K, 3, **f64)
             cov, ymean = torch.empty(B, 9, **f64), torch.empty(2 * B, 3, **f64)
             status = torch.empty(B + 1, dtype=torch.int32, device=dev)
             io = nat.EqdForwardIO()
@@ -596,7 +601,7 @@ class IEGMNEngine:
             descs = with_dropout([l.descriptor(mma_products) for l in layers], dropout)
             larr = (C.POINTER(nat.EqdLayer) * len(layers))(*[C.pointer(d) for d in descs])
             nat.check(lib.eqd_iegmn_forward(g, larr, len(layers), C.byref(head.struct), C.byref(io), nat.ptr(ws),
-                                            plan.forward_ws_bytes, st), 'eqd_iegmn_forward')
+                                            ws_bytes, st), 'eqd_iegmn_forward')
             kab = lambda mask: nat.check(lib.eqd_kabsch_apply(
                 g, nat.ptr(cov), nat.ptr(ymean), nat.ptr(x_l), nat.ptr(mask), nat.ptr(rot), nat.ptr(trans),
                 nat.ptr(lig_out), nat.ptr(sing), nat.ptr(status), st), 'eqd_kabsch_apply')

@@ -95,7 +95,7 @@ class GraphedPending:
 
     def raw_result(self) -> Dict:
         """Waits for the replay and returns the engine's raw output dict (batched tensors: ``ligand_coors`` (sum N_l, 3),
-        ``rotation`` (B, 3, 3), ``translation`` (B, 1, 3), ``keypts`` (2B, 50, 3) ...).  They are the graph's static
+        ``rotation`` (B, 3, 3), ``translation`` (B, 1, 3), ``keypts`` (2B, K, 3) ...).  They are the graph's static
         buffers: valid until this GraphedForward is launched again."""
         o = self.owner
         self.event.synchronize()

@@ -46,32 +46,33 @@ class PocketBatch:
 def device_losses(plan, pred_lig: torch.Tensor, keypts: torch.Tensor, tgt: PocketBatch, pocket_ot_loss_weight: float,
                   intersection_loss_weight: float, intersection_sigma: float, intersection_surface_ct: float) -> Dict:
     """-> {'total': (4,) f64 [loss, mse, ot, intersection], 'parts': (B,4) f64, 'dcoors': (N_l,3) f32,
-    'dkeypts': (2B,50,3) f64, 'plan': (n_pocket_total,50) i32, 'err': (1,) i32}.  'plan' is a view of the workspace
-    holding the integer transport plans (pair b: rows pocket_ptr[b]..pocket_ptr[b+1], units of 1/(N_pocket * 50); rows of
-    a pair the solver skipped are undefined).  check_loss_status(res) raises if a pocket exceeds the solver's capacity or
+    'dkeypts': (2B,K,3) f64, 'plan': (n_pocket_total,K) i32, 'err': (1,) i32}, K = keypts.shape[1] (the model's
+    num_att_heads).  'plan' is a view of the workspace holding the integer transport plans (pair b: rows
+    pocket_ptr[b]..pocket_ptr[b+1], units of 1/(N_pocket * K); rows of a pair the solver skipped are undefined).  check_loss_status(res) raises if a pocket exceeds the solver's capacity or
     the transport solve failed."""
     lib = nat.load()
     dev = pred_lig.device
-    B, N_l = plan.n_pairs, plan.N_l
+    B, N_l, K = plan.n_pairs, plan.N_l, int(keypts.shape[1])
     assert pred_lig.shape == (N_l, 3) and tgt.bound_lig.shape == (N_l, 3) and tgt.bound_rec.shape == (plan.N_r, 3)
+    assert keypts.shape == (2 * B, K, 3)
     with torch.cuda.device(dev):
         st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        ws_bytes = int(lib.eqd_losses_workspace_bytes(plan.N_r, tgt.n_pocket_total))
+        ws_bytes = int(lib.eqd_losses_workspace_bytes_k(plan.N_r, tgt.n_pocket_total, K))
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
         parts = torch.zeros(B, 4, dtype=torch.float64, device=dev)
         total = torch.zeros(4, dtype=torch.float64, device=dev)
         dco = torch.empty(N_l, 3, dtype=torch.float32, device=dev)
-        dkp = torch.empty(2 * B, nat.HEADS, 3, dtype=torch.float64, device=dev)
+        dkp = torch.empty(2 * B, K, 3, dtype=torch.float64, device=dev)
         err = torch.zeros(1, dtype=torch.int32, device=dev)
         pred = pred_lig.detach().to(torch.float32).contiguous()
         kp = keypts.detach().to(torch.float64).contiguous()
-        nat.check(lib.eqd_losses(C.byref(plan.struct), nat.ptr(pred), nat.ptr(tgt.bound_lig), nat.ptr(tgt.bound_rec), nat.ptr(kp),
-                                 nat.ptr(tgt.pocket_ptr), nat.ptr(tgt.pocket_lig), nat.ptr(tgt.pocket_rec), tgt.n_pocket_total,
+        nat.check(lib.eqd_losses_k(C.byref(plan.struct), nat.ptr(pred), nat.ptr(tgt.bound_lig), nat.ptr(tgt.bound_rec), nat.ptr(kp),
+                                 K, nat.ptr(tgt.pocket_ptr), nat.ptr(tgt.pocket_lig), nat.ptr(tgt.pocket_rec), tgt.n_pocket_total,
                                  tgt.max_pocket, float(pocket_ot_loss_weight), float(intersection_loss_weight), float(intersection_sigma),
                                  float(intersection_surface_ct), nat.ptr(ws), ws_bytes, nat.ptr(parts), nat.ptr(total),
-                                 nat.ptr(dco), nat.ptr(dkp), nat.ptr(err), st), 'eqd_losses')
+                                 nat.ptr(dco), nat.ptr(dkp), nat.ptr(err), st), 'eqd_losses_k')
     off = (max(plan.N_r, 1) * 8 + 255) // 256 * 256                     # plan_flow offset (eqd_iegmn.h)
-    flow = ws[off:off + tgt.n_pocket_total * nat.HEADS * 4].view(torch.int32).view(tgt.n_pocket_total, nat.HEADS)
+    flow = ws[off:off + tgt.n_pocket_total * K * 4].view(torch.int32).view(tgt.n_pocket_total, K)
     return {'total': total, 'parts': parts, 'dcoors': dco, 'dkeypts': dkp, 'plan': flow, 'err': err,
             '_keep': (ws, pred, kp)}
 

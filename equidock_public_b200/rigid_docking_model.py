@@ -32,6 +32,7 @@ one autograd node whose backward is the CUDA per-layer backward (``training.laye
 layers train like the reference's.
 """
 import math  # noqa: F401  (re-exported, see module docstring)
+import numbers
 import sys  # noqa: F401
 
 import torch
@@ -291,10 +292,12 @@ class IEGMN(nn.Module):
             for _ in range(1, n_lays):
                 self.iegmn_layers.append(IEGMN_Layer(in_dim, hid, hid, fine_tune, args, log))
 
-        self.num_att_heads = args['num_att_heads']
+        heads = args['num_att_heads']
         self.out_feats_dim = hid
-        if self.num_att_heads != nat.HEADS:
-            raise NotImplementedError(f'CUDA engine: num_att_heads must be {nat.HEADS}')
+        if isinstance(heads, bool) or not isinstance(heads, numbers.Integral) or not 1 <= heads <= nat.MAX_HEADS:
+            raise NotImplementedError(f'CUDA engine: num_att_heads must be an integer from 1 to {nat.MAX_HEADS} '
+                                      f'(the exact-EMD solver takes at most {nat.MAX_HEADS} keypoints), got {heads!r}')
+        self.num_att_heads = int(heads)
         self.att_mlp_key_ROT = nn.Sequential(nn.Linear(hid, self.num_att_heads * hid, bias=False))
         self.att_mlp_query_ROT = nn.Sequential(nn.Linear(hid, self.num_att_heads * hid, bias=False))
         self.mlp_h_mean_ROT = nn.Sequential(nn.Linear(hid, hid), nn.Dropout(args['dropout']),
@@ -420,7 +423,7 @@ class Rigid_Body_Docking_Net(nn.Module):
         class Pending:
             def raw_result(self_inner):
                 """The engine's batched output dict (``ligand_coors`` (sum N_l, 3), ``rotation`` (B, 3, 3),
-                ``translation`` (B, 1, 3), ``keypts`` (2B, 50, 3), ...) once the status words are resolved."""
+                ``translation`` (B, 1, 3), ``keypts`` (2B, K, 3), ...) once the status words are resolved."""
                 return net.iegmn_original.resolve(raw)
 
             def result(self_inner):

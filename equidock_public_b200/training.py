@@ -210,7 +210,7 @@ def tn_workspace_floats(N: int, E: int, dhps: Sequence[int] = (nat.H0_PAD, nat.H
 class BackwardWorkspace:
     """Device buffers of one backward, sized for a plan (reused across steps with the same sizes)."""
 
-    def __init__(self, plan: GraphPlan, device):
+    def __init__(self, plan: GraphPlan, device, n_heads: int = nat.HEADS):
         N, E, B = plan.N, plan.E, plan.n_pairs
         f = lambda *s: torch.empty(*s, dtype=_f32, device=device)
         d = lambda *s: torch.empty(*s, dtype=torch.float64, device=device)
@@ -227,7 +227,7 @@ class BackwardWorkspace:
         n_partial, n_colsum = tn_workspace_floats(N, E)
         self.partial, self.colsum = f(n_partial), f(n_colsum)
         self.vec = f(132 * VEC_FLOATS)   # per-CTA partial sums of bwd_node / bwd_edge (grid <= EQD_SMS)
-        self.head_ws_bytes = int(lib.eqd_bwd_head_workspace_bytes(N, plan.n_node_tiles, B))
+        self.head_ws_bytes = int(lib.eqd_bwd_head_workspace_bytes_k(N, plan.n_node_tiles, B, n_heads))
         self.head_ws = torch.empty(self.head_ws_bytes, dtype=torch.uint8, device=device)
         # edges grouped by SOURCE node (ascending edge id inside a group): the transpose index of the CSR-by-destination
         order = torch.sort(plan.col_src.long(), stable=True)
@@ -379,7 +379,7 @@ class TrainEngine:
                  on_bucket_done=None, capture: Optional[list] = None, d_x_out=None, d_h_out=None,
                  inputs_out: Optional[dict] = None) -> torch.Tensor:
         """Gradients of every parameter for upstream gradients w.r.t. the four raw outputs (ligand coordinates
-        (N_l,3) f32, keypoints (2B,50,3) f64, rotations (B,3,3) f32, translations (B,1,3) f32; any may be None) and
+        (N_l,3) f32, keypoints (2B,K,3) f64, rotations (B,3,3) f32, translations (B,1,3) f32; any may be None) and
         w.r.t. the last layer's coordinates and features (``d_x_out`` (N,3), ``d_h_out`` (N,64), global node order;
         None = no loss on them).
         Returns the flat gradient buffer (see ParamLayout).  ``on_bucket_done(label, lo, hi)`` is called on the host
@@ -396,7 +396,7 @@ class TrainEngine:
         with torch.cuda.device(dev):
             st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             if self._ws is None or self._ws.key != (N, E, B) or self._ws_plan is not plan:
-                self._ws = BackwardWorkspace(plan, dev)
+                self._ws = BackwardWorkspace(plan, dev, fwd['head'].n_heads)
                 self._ws_plan = plan
             ws = self._ws
             if flat is None:

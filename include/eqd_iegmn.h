@@ -40,7 +40,8 @@ extern "C" {
 #define EQD_H0 69             /* residue_emb_dim 64 + 5 surface features, :382-388 */
 #define EQD_H0_PAD 72         /* row stride of padded 69-wide tensors */
 #define EQD_N_RES_TYPES 21    /* nn.Embedding(21, 64), :382 */
-#define EQD_HEADS 50          /* num_att_heads */
+#define EQD_HEADS 50          /* num_att_heads of the shipped checkpoints; eqd_head_params.n_heads == 0 means this */
+#define EQD_MAX_HEADS 64      /* largest num_att_heads K: the transport solver's one-warp search owns sinks l and l + 32 */
 #define EQD_TILE_ROWS 128     /* rows (edges / nodes) per CTA tile */
 
 enum {
@@ -200,15 +201,22 @@ typedef struct eqd_layer {
   eqd_layer_norms norms;
 } eqd_layer;
 
-/* ---- keypoint read-out parameters (IEGMN.__init__ :427-438), reference layouts ------------- */
+/* ---- keypoint read-out parameters (IEGMN.__init__ :427-438), reference layouts -------------
+ * K = the head's keypoint count (num_att_heads): n_heads, or EQD_HEADS (50) when n_heads is 0.  Every keypoint-shaped
+ * array of the head, Kabsch and loss entry points is K wide: w_key / w_query [64K][64], m_qk [K][64][64], keypoints and
+ * their gradients [2B][K][3], the transport plans [n_pocket_total][K].  The head entry points refuse K outside
+ * [1, EQD_MAX_HEADS] with EQD_ERR_UNSUPPORTED.  With K <= 3 the keypoint covariance has rank < 3 and the Kabsch guard
+ * fires for every pair, as in the reference.                                                                           */
 typedef struct eqd_head_params {
   const float* w_mean;        /* [64][64] mlp_h_mean_ROT.0.weight^T (k-major) */
   const float* b_mean;        /* [64] */
-  const float* w_key;         /* [3200][64] att_mlp_key_ROT.0.weight, as in the state_dict */
-  const float* w_query;       /* [3200][64] att_mlp_query_ROT.0.weight, as in the state_dict */
-  const double* m_qk;         /* [50][64][64] fp64, written once per model by eqd_head_fold() from w_key / w_query:
+  const float* w_key;         /* [64K][64] att_mlp_key_ROT.0.weight, as in the state_dict */
+  const float* w_query;       /* [64K][64] att_mlp_query_ROT.0.weight, as in the state_dict */
+  const double* m_qk;         /* [K][64][64] fp64, written once per model by eqd_head_fold() from w_key / w_query:
                                  m_qk[k][d'][d] = sum_e w_query[64k+e][d'] w_key[64k+e][d] / 8.  Device memory, 16-byte aligned. */
   float leaky_slope;
+  int32_t n_heads;            /* K, 1..EQD_MAX_HEADS; 0 = EQD_HEADS.  It fills what was tail padding: sizeof and every
+                                 other offset are unchanged. */
 } eqd_head_params;
 
 int eqd_abi_version(void);
@@ -219,9 +227,11 @@ int eqd_abi_version(void);
  *   0                                              float part[T][64]   per node tile column sums of LeakyReLU(W_m h + b_m)
  *   round_up(T*256)                                int tile_ptr[2B+1]  first node tile of every protein
  *   q = round_up(T*256) + round_up((2B+1)*4)       double qbar[2B][64] mean-pooled queries (:525, :529), segment order
- *   q + round_up(2B*64*8)                          double u[2B][50][64] u[s][k] = m_qk[k]^T qbar[partner of s]
- * so the fp64 stages of the head can be checked one at a time.                                                      */
+ *   q + round_up(2B*64*8)                          double u[2B][K][64]  u[s][k] = m_qk[k]^T qbar[partner of s]
+ * so the fp64 stages of the head can be checked one at a time.  eqd_workspace_bytes is the size for K = 50,
+ * eqd_workspace_bytes_k for a head of n_heads keypoints (0 bytes for n_heads outside [1, EQD_MAX_HEADS]).             */
 size_t eqd_workspace_bytes(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs);
+size_t eqd_workspace_bytes_k(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs, int32_t n_heads);
 
 /* Input stage, IEGMN.forward :452-471.
  *   h0[n][72]  = [Embedding(res_feat.long()) (64) | log(mu_r_norm) (5) | 0 0 0]
@@ -322,14 +332,15 @@ int eqd_iegmn_layer_forward(const eqd_graph* g, const eqd_layer* p, const eqd_la
                             float* proj, float* proj_next, float* aggr, float* mu,
                             float* h_out, double* x_out, int32_t* status, void* stream);
 
-/* Weights-only fold of the 50-head key / query projections (att_mlp_key_ROT, att_mlp_query_ROT :427-438) into
+/* Weights-only fold of the K-head key / query projections (att_mlp_key_ROT, att_mlp_query_ROT :427-438) into
  * m_qk (see eqd_head_params), so that the per-protein logits are h_j . (m_qk[k]^T qbar) (:544-546, :555-557).
  * Call once after loading a checkpoint; eqd_keypoints() reads hp->m_qk.                                       */
-int eqd_head_fold(const eqd_head_params* hp, double* m_qk /*[50][64][64]*/, void* stream);
+int eqd_head_fold(const eqd_head_params* hp, double* m_qk /*[K][64][64]*/, void* stream);
 
-/* Keypoint read-out (IEGMN.forward :521-567): mean-pooled queries, 50-head attention over each
- * protein's nodes, keypoints Y (fp64 [2B][50][3], segment order), their means and the 3x3
- * covariance A = (Y_rec - mean)^T (Y_lig - mean) per pair (cov[B][9], ymean[2B][3]).        */
+/* Keypoint read-out (IEGMN.forward :521-567): mean-pooled queries, K-head attention over each
+ * protein's nodes, keypoints Y (fp64 [2B][K][3], segment order), their means over the K keypoints and the 3x3
+ * covariance A = (Y_rec - mean)^T (Y_lig - mean) per pair (cov[B][9], ymean[2B][3]).  The workspace is
+ * eqd_workspace_bytes_k(.., K) bytes.                                                       */
 int eqd_keypoints(const eqd_graph* g, const eqd_head_params* hp, const float* h /*[n][64]*/,
                   const double* x /*[n][3] last-layer coords*/, void* workspace, size_t workspace_bytes,
                   double* keypts, double* ymean, double* cov, void* stream);
@@ -372,7 +383,7 @@ typedef struct eqd_forward_io {
   int32_t* status;            /* [B+1] EQD_STATUS_* bits, zeroed by the call */
   float* h_out;               /* [n][64] last layer's node features  (ndata['hv_iegmn_out']) */
   double* x_out;              /* [n][3]  last layer's coordinates    (ndata['x_iegmn_out'])  */
-  double* keypts;             /* [2B][50][3] or NULL */
+  double* keypts;             /* [2B][K][3] or NULL (K = the head's keypoint count) */
   double* cov;                /* [B][9] Kabsch covariances (eqd_kabsch_apply can be replayed on them) or NULL */
   double* ymean;              /* [2B][3] keypoint means (needed for such a replay) or NULL */
   /* optional: HOST array of 4*n_layers cudaEvent_t handles (edge begin, edge end, node begin, node end per layer) recorded
@@ -384,7 +395,10 @@ typedef struct eqd_forward_io {
   size_t train_stash_bytes;
 } eqd_forward_io;
 
+/* eqd_forward_workspace_bytes: for a head of K = 50 keypoints; eqd_forward_workspace_bytes_k: of n_heads keypoints (0 for
+ * n_heads outside [1, EQD_MAX_HEADS]).  eqd_iegmn_forward needs the size for its head's K.                            */
 size_t eqd_forward_workspace_bytes(const eqd_graph* g);
+size_t eqd_forward_workspace_bytes_k(const eqd_graph* g, int32_t n_heads);
 size_t eqd_forward_stash_bytes(const eqd_graph* g, int32_t n_layers);
 /* out[9] = byte offsets / strides inside the stash: h0 [n][72] f32 | x[l] [n][3] f64 (offset, stride per layer; x[0] = the
  * input coordinates) | h[l] [n][64] f32, l >= 1 (offset, stride) | aggr[l] [n][64] f32 (offset, stride) | mu[l] f32, row
@@ -457,8 +471,10 @@ int eqd_bwd_project(const eqd_graph* g, const eqd_layer* p, const float* w_projT
 int eqd_bwd_embed(const eqd_graph* g, const float* res_lig, const float* res_rec, const float* dh0_acc,
                   const float* dh_layer0, float* demb, void* stream);
 /* Keypoint read-out + Kabsch backward (:521-589, 657-665), fp64, incl. the 3x3 SVD backward (torch's svd_backward with
- * the guard's gap as denominator).  See csrc/head.cu for the argument semantics.                                      */
+ * the guard's gap as denominator).  See csrc/head.cu for the argument semantics; dkeypts is [2B][K][3], and the
+ * workspace eqd_bwd_head_workspace_bytes_k(.., K) bytes (eqd_bwd_head_workspace_bytes: K = 50).                       */
 size_t eqd_bwd_head_workspace_bytes(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs);
+size_t eqd_bwd_head_workspace_bytes_k(int32_t n_nodes, int32_t n_node_tiles, int32_t n_pairs, int32_t n_heads);
 int eqd_bwd_head(const eqd_graph* g, const eqd_head_params* hp, const float* h, const double* x, const double* cov,
                  const float* x_lig_in, const float* dcoors, const double* dkeypts, const float* drot,
                  const float* dtrans, void* workspace, size_t workspace_bytes, float* dh, double* dx, float* dpre,
@@ -494,11 +510,14 @@ int eqd_bwd_inputs(const eqd_graph* g, const float* dh0_acc, const float* dh_lay
  * Per pair: MSE of the predicted ligand coordinates, body-intersection loss, pocket OT loss with the EXACT earth mover's
  * distance (uniform marginals; successive shortest paths with potentials instead of POT's CPU network simplex), batch
  * means combined with the reference's weights; plus the gradients w.r.t. the predicted coordinates and the keypoints.
- * After the call the workspace holds the integer transport plans: int32 plan_flow[n_pocket_total][50] at byte offset
+ * After the call the workspace holds the integer transport plans: int32 plan_flow[n_pocket_total][K] at byte offset
  * round_up(max(N_r, 1) * 8, 256), N_r = n_nodes - n_lig_nodes; pair b owns rows pocket_ptr[b] .. pocket_ptr[b+1] in units
- * of 1 / (N_pocket * 50) (every row sums to 50, every column to N_pocket).  Rows of a pair that err_flags reports as too
- * large are not written. */
+ * of 1 / (N_pocket * K) (every row sums to K, every column to N_pocket).  Rows of a pair that err_flags reports as too
+ * large are not written.  eqd_losses and eqd_losses_workspace_bytes are for K = 50 keypoints per protein;
+ * eqd_losses_k / eqd_losses_workspace_bytes_k take K = n_heads (1..EQD_MAX_HEADS; else EQD_ERR_UNSUPPORTED / 0 bytes)
+ * and the same arguments otherwise, with keypts and dkeypts [2B][K][3]. */
 size_t eqd_losses_workspace_bytes(int32_t n_rec_nodes, int32_t n_pocket_total);
+size_t eqd_losses_workspace_bytes_k(int32_t n_rec_nodes, int32_t n_pocket_total, int32_t n_heads);
 int eqd_losses(const eqd_graph* g, const float* pred_lig /*[N_l][3]*/, const float* bound_lig /*[N_l][3]*/,
                const float* bound_rec /*[N_r][3]*/, const double* keypts /*[2B][50][3]*/,
                const int32_t* pocket_ptr /*[B+1]*/, const float* pocket_lig, const float* pocket_rec /*[sum P][3]*/,
@@ -507,6 +526,12 @@ int eqd_losses(const eqd_graph* g, const float* pred_lig /*[N_l][3]*/, const flo
                float intersection_sigma, float intersection_surface_ct, void* workspace, size_t workspace_bytes,
                double* parts /*[B][4] mse, ot, intersection, -*/, double* total /*[4] loss, mse, ot, intersection*/,
                float* dcoors /*[N_l][3]*/, double* dkeypts /*[2B][50][3]*/, int32_t* err_flags, void* stream);
+int eqd_losses_k(const eqd_graph* g, const float* pred_lig, const float* bound_lig, const float* bound_rec,
+                 const double* keypts /*[2B][K][3]*/, int32_t n_heads /* K */, const int32_t* pocket_ptr,
+                 const float* pocket_lig, const float* pocket_rec, int32_t n_pocket_total, int32_t max_pocket,
+                 float pocket_ot_loss_weight, float intersection_loss_weight, float intersection_sigma,
+                 float intersection_surface_ct, void* workspace, size_t workspace_bytes, double* parts, double* total,
+                 float* dcoors, double* dkeypts /*[2B][K][3]*/, int32_t* err_flags, void* stream);
 
 /* ---- residue k-NN graph construction on the device (src/utils/protein_utils.py:212-397, RBFs :71-86) ------------------
  * Proteins of a batch in engine order (ligand proteins of all pairs, then receptor proteins): seg_ptr [n_prot+1] residue
