@@ -303,10 +303,12 @@ __global__ void kabsch_apply_kernel(eqd_graph g, const double* __restrict__ cov,
     svd3(A, U, S, V);
     int st = 0;
     if (nan) st |= EQD_STATUS_NAN;
-    // guard of :574, evaluated on the fp32-rounded singular values like the reference's fp32 S
+    // guard of :574, evaluated on the fp32-rounded singular values like the reference's fp32 S.  The squares are rounded
+    // on their own (__fmul_rn is never contracted): fmaf(s0, s0, -q1) would leave the rounding residual of q1, up to
+    // ulp(S^2) / 2, where the reference's difference of two rounded squares is 0, and so miss near-equal large S.
     {
       float s0 = (float)S[0], s1 = (float)S[1], s2 = (float)S[2];
-      float q0 = s0 * s0, q1 = s1 * s1, q2 = s2 * s2;
+      float q0 = __fmul_rn(s0, s0), q1 = __fmul_rn(s1, s1), q2 = __fmul_rn(s2, s2);
       float gap = fminf(fminf(fabsf(q0 - q1), fabsf(q0 - q2)), fabsf(q1 - q2));
       if (fminf(fminf(s0, s1), s2) < 1e-3f || gap < 1e-2f) st |= EQD_STATUS_SVD_DEGENERATE;
     }

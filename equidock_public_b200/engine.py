@@ -647,6 +647,7 @@ class IEGMNEngine:
                 f'a node has more than max_in_degree={plan.struct.max_in_degree} in-edges; '
                 'pass the true bound (args["graph_max_neighbor"])')
         pair_st = st_host[:plan.n_pairs]
+        draws = out['guard_draws'] = [0] * plan.n_pairs     # perturbations each pair's covariance took
         if not bool(pair_st.any()):
             return
         if bool((pair_st & nat.STATUS_NAN).any()):
@@ -657,10 +658,15 @@ class IEGMNEngine:
             mask[b] = 1
             num_it = 0
             while True:
-                noise = torch.rand(3, 3)  # same CPU-generator draw as the reference (:578)
+                # the reference's torch.rand(3, 3) of :578 from the default CPU generator.  A training forward with
+                # dropout has drawn its mask seed from that generator first (draw_dropout), which the reference's
+                # nn.Dropout on the GPU does not, so from the same torch seed the noise matches the reference's only
+                # without dropout.
+                noise = torch.rand(3, 3)
                 out['cov'][b, eye_idx] += torch.diagonal(noise).to(self.device, torch.float64)
                 kab(mask)
                 num_it += 1
+                draws[b] = num_it
                 if num_it > 10:  # the reference gives up before re-testing the 11th attempt (:582-584)
                     if log is not None:
                         log('SVD consistently numerically unstable! Exitting ... ')

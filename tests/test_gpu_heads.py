@@ -1,10 +1,13 @@
-"""GPU (H100): models with num_att_heads = K keypoints per protein (K = 4, 25, 32, 33, 64 at the kernels; 25 and 64 end to
-end) against fp64.
+"""GPU (H100): models with num_att_heads = K keypoints per protein (K = 1, 2, 3, 4, 25, 32, 33, 64 at the kernels; 25 and
+64 end to end) against fp64.
 
   - eqd_head_fold, eqd_keypoints and eqd_kabsch_apply: every fp64 stage from the kernel's own inputs, at the bounds of
-    tests/test_gpu_forward_kernels.py, then the keypoints and the rigid transform against oracle/iegmn_oracle.py.  K = 32 /
-    33 end the last warp's heads at a lane boundary / one past it, 33 and 64 leave a partial last group of 25 heads.
-  - eqd_bwd_head against oracle/backward_manual.py at the 1e-5 of tests/test_gpu_backward_kernels.py.
+    tests/test_gpu_forward_kernels.py, then the keypoints and the rigid transform against oracle/iegmn_oracle.py, the
+    pairs the SVD guard flags (every pair at K <= 3, whose centred keypoints have rank <= K - 1) after the engine's host
+    loop with the oracle's loop replaying its draws.  K = 1 .. 3 run the kernels' one- to three-head groups, K = 32 / 33
+    end the last warp's heads at a lane boundary / one past it, 33 and 64 leave a partial last group of 25 heads.
+  - eqd_bwd_head against oracle/backward_manual.py at the 1e-5 of tests/test_gpu_backward_kernels.py (K >= 4: the manual
+    backward has no guard branch; the backward through the guard is tests/test_gpu_svd_guard.py's).
   - eqd_losses_k: the exact-EMD value against the HiGHS optimum (1e-9), every plan certified optimal by
     loss_oracle.ot_certify, at pocket sizes 4 .. 398 and one past the largest pocket whose cost matrix still fits in
     shared memory for that K (1024, the solver's capacity, where it always fits).
@@ -37,7 +40,8 @@ from test_gpu_losses import _plan
 
 pytestmark = pytest.mark.gpu
 F64 = torch.float64
-KS = [4, 25, 32, 33, 64]
+KS = [1, 2, 3, 4, 25, 32, 33, 64]
+KS_UNGUARDED = [4, 25, 32, 33, 64]     # K >= 4: the guard need not fire
 
 
 def _pairs(kind):
@@ -69,6 +73,27 @@ def _sd_np(model):
 def _cfg(args):
     return orc.OracleConfig(args['iegmn_n_lays'], args['skip_weight_h'], args['x_connection_init'],
                             args['leakyrelu_neg_slope'], args['num_att_heads'])
+
+
+def _guard_loop(dev, plan, cov, status, kab, seed):
+    """IEGMNEngine.resolve_status over a hand-launched eqd_kabsch_apply (``kab(mask)``) from torch.manual_seed(seed):
+    perturbs ``cov`` of the flagged pairs and re-solves them.  Returns the draws per pair."""
+    from equidock_public_b200.engine import IEGMNEngine
+    torch.cuda.synchronize()
+    ev = torch.cuda.Event()
+    ev.record()
+    out = {'cov': cov, 'status': status, 'status_event': ev,
+           'status_host': torch.cat([status.cpu(), torch.zeros(2, dtype=torch.int32)])}
+    torch.manual_seed(seed)
+    IEGMNEngine(dev).resolve_status(plan, out, kab)
+    return out['guard_draws']
+
+
+def _counted(rand_diag, used):
+    """The oracle's iterator of noise diagonals over a replay callable, counting the draws in ``used``."""
+    while True:
+        used.append(1)
+        yield rand_diag().numpy()
 
 
 # ---- forward kernels --------------------------------------------------------------------------------------------------
@@ -107,14 +132,18 @@ def test_head_forward_kernels_vs_fp64(K, kind, cuda_device):
         lig = torch.full((NL, 3), float('nan'), device=dev)
         sing = torch.full((B, 3), float('nan'), dtype=F64, device=dev)
         status = torch.zeros(B, dtype=torch.int32, device=dev)
-        nat.check(lib.eqd_kabsch_apply(C.byref(plan.struct), nat.ptr(cov), nat.ptr(ym), nat.ptr(xl), None, nat.ptr(rot),
-                                       nat.ptr(trans), nat.ptr(lig), nat.ptr(sing), nat.ptr(status), None),
-                  'eqd_kabsch_apply')
+        kab = lambda mask: nat.check(lib.eqd_kabsch_apply(C.byref(plan.struct), nat.ptr(cov), nat.ptr(ym), nat.ptr(xl),
+                                                          nat.ptr(mask), nat.ptr(rot), nat.ptr(trans), nat.ptr(lig),
+                                                          nat.ptr(sing), nat.ptr(status), None), 'eqd_kabsch_apply')
+        kab(None)
         qbar = ws[q_off:q_off + 2 * B * 512].view(F64).view(2 * B, 64).clone()
         u = ws[u_off:u_off + 2 * B * K * 512].view(F64).view(2 * B, K, 64).clone()
-        return m, qbar, u, kp, ym, cov, rot, trans, lig, sing, status
+        cov0, status0 = cov.clone(), status.clone()
+        draws = torch.tensor(_guard_loop(dev, plan, cov, status, kab, 100 + K))     # perturbs cov, re-solves
+        return m, qbar, u, kp, ym, cov0, status0, cov, draws, rot, trans, lig, sing, status
 
-    m, qbar, u, kp, ym, cov, rot, trans, lig, sing, status = _twice(run)
+    m, qbar, u, kp, ym, cov, status, cov_p, draws, rot, trans, lig, sing, status_p = _twice(run)
+    assert not bool((status_p & nat.STATUS_SVD_DEGENERATE).any())
     wq = net.att_mlp_query_ROT[0].weight.detach().to(F64).view(K, 64, 64)
     wk = net.att_mlp_key_ROT[0].weight.detach().to(F64).view(K, 64, 64)
     seg = [int(v) for v in plan.seg_ptr_host]
@@ -130,24 +159,38 @@ def test_head_forward_kernels_vs_fp64(K, kind, cuda_device):
     print(f'\nhead K={K} {kind}: ' + ', '.join(f'{k} {e:.1e}' for k, (e, _) in errs.items()))
     assert all(e <= tol for e, tol in errs.values()), errs
     # end to end against the numpy fp64 oracle (iegmn_oracle.keypoints_and_kabsch): keypoints from the fp32 qbar GEMM
-    # (1e-5), the rotation within 2e-4 and the ligand within the coordinate bound where the oracle's guard does not fire
+    # (1e-5), the rotation within 2e-4 and the ligand within the coordinate bound.  Where the guard fires, the oracle's
+    # loop takes the engine's draws (hr.replay_draws, pairs in order): the same number per pair and the same perturbed
+    # covariance; the pose is then checked against Kabsch of the kernel's own perturbed covariance, because with K = 2 / 3
+    # trained heads the noise-set rotation amplifies the keypoints' fp32-level error by S_max / S_min
     sd, cfg = _sd_np(model), _cfg(hr.args_with('dips', K))
     hn, xn = h64.cpu().numpy(), x.cpu().numpy()
+    _, rand_diag = hr.replay_draws(100 + K)
     for b in range(B):
         (la, lb), (ra, rb) = (seg[b], seg[b + 1]), (seg[B + b], seg[B + b + 1])
         c = bm.head_forward(sd, cfg, hn[la:lb], xn[la:lb], hn[ra:rb], xn[ra:rb])
         assert _rel(kp[b], c['Y'][0]) <= 1e-5 and _rel(kp[B + b], c['Y'][1]) <= 1e-5, b
-        try:
-            T, t, _, _, info = orc.keypoints_and_kabsch(sd, cfg, hn[la:lb], xn[la:lb], hn[ra:rb], xn[ra:rb], np.float64)
-        except RuntimeError:                   # the guard fired (a one-node protein: all K keypoints coincide)
-            assert int(status[b]) & nat.STATUS_SVD_DEGENERATE, b
-            continue
-        assert not int(status[b]) & nat.STATUS_SVD_DEGENERATE, (b, info['S'])
+        used = []
+        T, t, _, _, info = orc.keypoints_and_kabsch(sd, cfg, hn[la:lb], xn[la:lb], hn[ra:rb], xn[ra:rb], np.float64,
+                                                    rand_diag=_counted(rand_diag, used))
+        flagged = bool(int(status[b]) & nat.STATUS_SVD_DEGENERATE)
+        assert info['flagged'] == flagged and len(used) == int(draws[b]), (b, info['S'], len(used), int(draws[b]))
+        assert flagged or int(draws[b]) == 0
+        if flagged:
+            A = cov_p[b].cpu().numpy().reshape(3, 3)
+            assert np.abs(A - info['A']).max() <= 1e-5 * np.abs(info['A']).max(), b
+            U, _, Vt = np.linalg.svd(A)
+            T = U @ np.diag([1., 1., np.sign(np.linalg.det(A))]) @ Vt
+            yl_m, yr_m = kp[b].mean(0).cpu().numpy(), kp[B + b].mean(0).cpu().numpy()
+            t = yr_m - T @ yl_m
         assert float(np.abs(rot[b].cpu().numpy().reshape(3, 3) - T).max()) <= 2e-4, b
         ref = xl[la:lb].double().cpu().numpy() @ T.T + t
         assert float(np.abs(lig[la:lb].cpu().numpy() - ref).max()) <= 2e-3 * max(1.0, np.abs(ref).max() / 100), b
+    print(f'head K={K} {kind}: guard draws {draws.tolist()}')
     if kind == 'sizes':
         assert int(status[0]) & nat.STATUS_SVD_DEGENERATE and int(status[2]) & nat.STATUS_SVD_DEGENERATE
+    if K <= 3:
+        assert all(int(v) & nat.STATUS_SVD_DEGENERATE for v in status.tolist())
 
 
 def test_head_entry_points_refuse_keypoint_counts_out_of_range(cuda_device):
@@ -162,7 +205,7 @@ def test_head_entry_points_refuse_keypoint_counts_out_of_range(cuda_device):
 
 # ---- backward kernel --------------------------------------------------------------------------------------------------
 
-@pytest.mark.parametrize('K', KS)
+@pytest.mark.parametrize('K', KS_UNGUARDED)
 def test_bwd_head_vs_manual_oracle(K, cuda_device):
     dev, lib = cuda_device, nat.load()
     model = hr.build_model('dips', dev, K, seed=K)
@@ -298,7 +341,7 @@ def test_module_forward_graph_replay_and_training_vs_fp64(ds, K, cuda_device):
     assert kp_l[0].shape == (K, 3) and kp_r[-1].shape == (K, 3)
     got = torch.cat(coors)
     plan = model.iegmn_original.last_outputs['plan']
-    co_ref, Y, R, _ = hr.model_forward(_fp64_state(model), args, _oracle_inputs(g, plan))
+    co_ref, Y, R, _, _ = hr.model_forward(_fp64_state(model), args, _oracle_inputs(g, plan))
     cr = co_ref.numpy()
     err = float(np.abs(got.cpu().double().numpy() - cr).max())
     print(f'\nforward {ds} K={K}: max |coors - fp64| = {err:.3e}')
@@ -316,7 +359,7 @@ def test_module_forward_graph_replay_and_training_vs_fp64(ds, K, cuda_device):
     _, _, loss2, coors2, grads2 = _run_module(model, pairs, tg, dev, 11)
     assert torch.equal(loss, loss2) and torch.equal(coors, coors2) and all(torch.equal(grads[n], grads2[n]) for n in grads)
     sd = _fp64_state(model, requires_grad=True)
-    co_ref, Y, _, _ = hr.model_forward(sd, args, _oracle_inputs(g, fwd['plan']))
+    co_ref, Y, _, _, _ = hr.model_forward(sd, args, _oracle_inputs(g, fwd['plan']))
     B = fwd['plan'].n_pairs
     loss_ref = _loss(co_ref, (Y[:B], Y[B:]), tg, fwd['plan'].n_lig_list)
     loss_ref.backward()
@@ -371,7 +414,7 @@ def test_training_with_dropout_vs_fp64_under_the_same_masks(cuda_device):
     plan, d0 = fwd['plan'], fwd['dropout_layers'][0].dropout
     masks = dm.BatchMasks(p, d0.seed, 0, plan.N, plan.E, int(args['iegmn_n_lays']))
     sd = _fp64_state(model, requires_grad=True)
-    co_ref, Y, _, _ = hr.model_forward(sd, args, _oracle_inputs(g, plan), masks)
+    co_ref, Y, _, _, _ = hr.model_forward(sd, args, _oracle_inputs(g, plan), masks)
     B = plan.n_pairs
     loss_ref = _loss(co_ref, (Y[:B], Y[B:]), tg, plan.n_lig_list)
     loss_ref.backward()
