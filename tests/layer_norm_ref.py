@@ -66,16 +66,23 @@ def args_with(ds, layer_norm_coors='LN', dropout=0.0, final_h_layer_norm='0'):
     return a
 
 
-def build_model(ds, device, args, seed=0, gamma_zero=False):
+def build_model(ds, device, args, seed=0, gamma_zero=False, heads=None):
     """The shipped checkpoint of ``ds`` in a model built with ``args``; the optional LayerNorms the checkpoint lacks get
     seeded gamma ~ 1 + U(-0.5, 0.5) (gamma_zero: the coordinate LayerNorm's gamma is 0, what reset_parameters leaves; a
     final LayerNorm with gamma 0 would give every node the same features and a degenerate keypoint covariance) and
     beta ~ U(-0.2, 0.2), one draw per
-    layer module (weight-shared layers share it).  Loads the completed state dict with strict=True."""
+    layer module (weight-shared layers share it).  ``heads`` = K: num_att_heads K with heads_ref.head_weights' K-head
+    key / query projections.  Loads the completed state dict with strict=True."""
     from equidock_public_b200.rigid_docking_model import Rigid_Body_Docking_Net
     args = dict(args, device=device)
+    if heads is not None:
+        args['num_att_heads'] = heads
     model = Rigid_Body_Docking_Net(args)
-    sd = {k: torch.from_numpy(np.asarray(v)) for k, v in gio.load_checkpoint(ds).items()}
+    ck = gio.load_checkpoint(ds)
+    sd = {k: torch.from_numpy(np.asarray(v)) for k, v in ck.items()}
+    if heads is not None:
+        import heads_ref
+        sd.update(heads_ref.head_weights(ck, heads, np.random.default_rng(seed)))
     rng = np.random.default_rng(seed)
     drawn = {}
     for li, lay in enumerate(model.iegmn_original.iegmn_layers):

@@ -129,8 +129,8 @@ def _engine_loss(model, g, tgts):
                   nr['hv_iegmn_out'])
 
 
-def _report(got_in, ref_in, model, ref_p):
-    """Prints every tensor's error; returns the ones out of bound."""
+def _report(got_in, ref_in, model, ref_p, amp=1.0):
+    """Prints every tensor's error; returns the ones out of bound (``amp`` times the bound)."""
     rows = [(grp, f'd {n}', _np(a).reshape(r.shape), r)
             for n, grp, a, r in zip(INPUTS, ('x', 'x', 'mu', 'mu', 'he', 'he'), got_in, ref_in) if a is not None]
     rows += [('param', n.replace('iegmn_original.', ''), _np(p.grad).reshape(ref_p[n].shape) if p.grad is not None
@@ -139,7 +139,7 @@ def _report(got_in, ref_in, model, ref_p):
     bad = []
     for grp, tag, got, ref in rows:
         err, rmax = float(np.abs(got - ref).max()), float(np.abs(ref).max())
-        ok = err <= 3e-3 * rmax + 2e-6 * G[grp]
+        ok = err <= amp * (3e-3 * rmax + 2e-6 * G[grp])
         line = f'{"ok  " if ok else "BAD "}{tag:52s} abs {err:.2e}  rel {err / max(rmax, 1e-30):.2e}  max|ref| {rmax:.3e}'
         print(line)
         if not ok:

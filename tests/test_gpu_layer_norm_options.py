@@ -1,6 +1,8 @@
 """GPU (H100): models with the reference's coordinate LayerNorm (layer_norm_coors='LN', coors_mlp.3) and final feature
 LayerNorm (final_h_layer_norm='LN', final_h_layernorm_layer), alone and together, on the tensor-core and fp32 edge and node
-stages and in the CUDA backward, against the fp64 restatement of tests/layer_norm_ref.py.
+stages and in the CUDA backward, against the fp64 restatement of tests/layer_norm_ref.py.  These are whole-model and
+whole-layer checks; tests/test_gpu_layer_norm_kernels.py holds each kernel with a layer-norm option to 1e-5 against fp64
+on batches where CTAs run several tiles, and the graph-input gradients of these models.
 
 Bounds.  Those of the shipped configuration: tests/test_gpu_edge_stage.py's 1e-5 relative for the edge-stage kernels and
 tests/test_gpu_dropout.py's 2e-3 on coordinates scaled by max(1, |x|/100) and 3e-3 relative per parameter gradient for
