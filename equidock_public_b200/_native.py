@@ -25,7 +25,7 @@ class EqdGraph(C.Structure):
                 ('n_lig_edges', _i32), ('max_in_degree', _i32),
                 ('seg_ptr', _vp), ('row_ptr', _vp), ('col_src', _vp), ('edge_dst', _vp),
                 ('he_lig', _vp), ('he_rec', _vp),
-                ('n_node_tiles', _i32), ('node_tiles', _vp)]
+                ('n_node_tiles', _i32), ('max_segment_nodes', _i32), ('node_tiles', _vp)]
 
 
 class EqdLayerParams(C.Structure):

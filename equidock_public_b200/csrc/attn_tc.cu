@@ -473,14 +473,224 @@ attention64_tc_kernel(eqd_graph g, const float* __restrict__ proj, const unsigne
   cp_async_wait<0>();
 }
 
+// ---- the 64-wide layers, partner K / V resident in shared memory ------------------------------------------------------
+// For batches whose partner proteins all fit (eqd_graph.max_segment_nodes <= AT_RES_MAX_NODES): the unit of work is one
+// query protein.  Its partner's K / V chunks (the same 8-block chunks from the partner's first block that
+// attention64_tc_kernel streams for every 64-row query tile) are copied once into six resident planes, K and V x 3
+// splits, and every query tile of the protein reads them from there: the per-tile chunk stream, its mbarrier waits and
+// the chain barriers that protected its refills are gone.  The GEMMs, masks and sums are those of attention64_tc_kernel
+// on the same B bytes, so mu is bitwise the same.
+//   K split 0 (all that pass 1's hi-only S GEMMs read) lands first under res_k0; the other five planes follow per chunk,
+//   chunk c under res_kv[c].  Both chains take the protein's non-empty 64-row halves (chain c: halves c, c + 2, ...); the
+//   planes are refilled for the CTA's next protein after a CTA barrier that follows both chains' last tile, so each
+//   mbarrier is re-armed only after every thread has observed its previous phase.
+#define AT_RES_CHUNKS 4
+#define AT_RES_BLOCKS (AT_RES_CHUNKS * 8)
+#define AT_RES_PLANE (AT_RES_CHUNKS * AT_CHUNK_BYTES)
+// largest partner whose chunk walk fits: a segment that starts mid-block spans ceil(n / 8) + 1 blocks
+#define AT_RES_MAX_NODES (8 * (AT_RES_BLOCKS - 1))
+
+struct __align__(128) AtResSmem {
+  unsigned char k[3][AT_RES_PLANE];   // resident K chunks, one plane per split
+  unsigned char v[3][AT_RES_PLANE];
+  float qs[AT_CHAINS][64 * 64];       // per chain: Q rows of its next tile
+  unsigned long long res_k0, res_kv[AT_RES_CHUNKS];
+};
+static_assert(sizeof(AtResSmem) <= 227 * 1024, "resident K / V planes + Q staging exceed the 227 KB of shared memory per CTA");
+
+template <int P>
+__global__ void __launch_bounds__(AT_CHAINS * 128, 1)
+attention64_res_kernel(eqd_graph g, const float* __restrict__ proj, const unsigned char* __restrict__ kv,
+                       long kv_split_stride, float* __restrict__ mu) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  AtResSmem& R = *reinterpret_cast<AtResSmem*>(smem_raw);
+  const int tid = threadIdx.x, wgi = tid >> 7, t = tid & 127, lane = t & 31;
+  const int bar = 1 + wgi;   // this chain's named barrier
+  float* const qs = R.qs[wgi];
+  if (tid == 0) {
+    mbar_init(&R.res_k0, 1);
+    for (int c = 0; c < AT_RES_CHUNKS; ++c) mbar_init(&R.res_kv[c], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  const unsigned k_saddr = smem_u32(R.k), v_saddr = smem_u32(R.v);
+  const int B = g.n_pairs, nseg = 2 * B;
+  const unsigned char* k_g = kv;                              // which = 0
+  const unsigned char* v_g = kv + 3 * kv_split_stride;        // which = 1
+
+  // The chain's tiles in order: (segment, half), segments blockIdx.x + i gridDim.x, halves wgi, wgi + 2, ... of each.
+  // next_tile: the first one from (seg, h) on; seg = -1 if none.
+  auto next_tile = [&](int& seg, int& h) {
+    for (; seg < nseg; seg += gridDim.x, h = wgi)
+      if (64 * h < __ldg(g.seg_ptr + seg + 1) - __ldg(g.seg_ptr + seg)) return;
+    seg = -1;
+  };
+  auto stage_q = [&](int seg, int h) {
+    const int node0 = __ldg(g.seg_ptr + seg) + 64 * h;
+    stage_rows64(qs, proj, 320, 128, node0, min(64, __ldg(g.seg_ptr + seg + 1) - node0), t);
+  };
+  int qseg = blockIdx.x, qh = wgi;   // the chain's next tile to stage
+  next_tile(qseg, qh);
+  if (qseg >= 0) stage_q(qseg, qh);
+
+  const int fr0 = (t >> 5) * 16 + (lane >> 2), fc = 2 * (lane & 3);
+  unsigned phase = 0;   // of every resident-plane mbarrier: one completed phase per loaded segment
+  for (int seg = blockIdx.x; seg < nseg; seg += gridDim.x) {
+    const int i0 = __ldg(g.seg_ptr + seg), i1 = __ldg(g.seg_ptr + seg + 1);
+    if (i1 <= i0) continue;
+    const int pseg = seg < B ? seg + B : seg - B;
+    const int j0 = __ldg(g.seg_ptr + pseg), j1 = __ldg(g.seg_ptr + pseg + 1);
+    const int blk_lo = j0 >> 3, nchunks = (((j1 + 7) >> 3) - blk_lo + 7) >> 3;
+    const bool fits = nchunks <= AT_RES_CHUNKS;
+    if (tid == 0 && fits) {
+      // every mbarrier completes one phase per segment: chunks the partner does not have are plain arrivals
+      mbar_expect_tx(&R.res_k0, nchunks * AT_CHUNK_BYTES);
+      if (nchunks > 0) bulk_g2s(R.k[0], k_g + (long)blk_lo * 1024, nchunks * AT_CHUNK_BYTES, &R.res_k0);
+      for (int c = 0; c < AT_RES_CHUNKS; ++c) {
+        unsigned long long* b = &R.res_kv[c];
+        if (c >= nchunks) {
+          mbar_expect_tx(b, 0);
+          continue;
+        }
+        mbar_expect_tx(b, 5 * AT_CHUNK_BYTES);
+        const long off = (long)(blk_lo + 8 * c) * 1024;
+#pragma unroll
+        for (int s = 0; s < 3; ++s) {
+          if (s > 0) bulk_g2s(R.k[s] + c * AT_CHUNK_BYTES, k_g + s * kv_split_stride + off, AT_CHUNK_BYTES, b);
+          bulk_g2s(R.v[s] + c * AT_CHUNK_BYTES, v_g + s * kv_split_stride + off, AT_CHUNK_BYTES, b);
+        }
+      }
+    }
+    for (int h = wgi; 64 * h < i1 - i0; h += 2) {
+      const int node0 = i0 + 64 * h, nvalid = min(64, i1 - node0);
+      // this tile's Q rows have landed (every thread's own copies, then the barrier for the others')
+      cp_async_wait<0>();
+      wg_barrier(bar);
+      unsigned qf[3][4][4];
+      staged_rows_to_a_split3<P>(qs, t, qf);
+      wg_barrier(bar);   // the staging buffer is free: the chain's next tile
+      qh += 2;
+      next_tile(qseg, qh);
+      if (qseg >= 0) stage_q(qseg, qh);
+      if (!fits) {   // only reachable if max_segment_nodes understated the batch: no overrun, and NaN marks the rows
+        for (int i = t; i < nvalid * EQD_HID; i += 128) mu[(long)node0 * EQD_HID + i] = __int_as_float(0x7fc00000);
+        continue;
+      }
+      auto k_desc = [&](int c) {
+        return [&, c](int sp, int kk) { return b_desc_ex(k_saddr + sp * AT_RES_PLANE + c * AT_CHUNK_BYTES + kk * 256, 128, 1024); };
+      };
+      // ---------------- pass 1: row maxima (hi-only S) --------------------------------------------------------------
+      float mx[2] = {-INFINITY, -INFINITY};
+      if (nchunks > 0) mbar_wait(&R.res_k0, phase);
+      for (int c = 0; c < nchunks; ++c) {
+        float s[32];
+        wg_gemm6_rs_issue<64, 4, 0, true>(s, qf, k_desc(c), false);
+        wg_mma_wait(s);
+        const int key0 = (blk_lo + 8 * c) * 8 + fc;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int kn = key0 + 8 * j + e;
+            const bool ok = kn >= j0 && kn < j1;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) mx[hh] = fmaxf(mx[hh], ok ? s[4 * j + 2 * hh + e] : -INFINITY);
+          }
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+      }
+      // ---------------- pass 2: P = exp(S - max), O += P V ----------------------------------------------------------
+      float lh[2][2] = {{0.f, 0.f}, {0.f, 0.f}};   // [fragment row][32-key half]: the row-per-thread code's per-half sums
+      float o_acc[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o_acc[i] = 0.f;
+      for (int c = 0; c < nchunks; ++c) {
+        mbar_wait(&R.res_kv[c], phase);
+        float s[32];
+        wg_gemm6_rs_issue<64, 4, 0, false, P>(s, qf, k_desc(c), false);
+        wg_mma_wait(s);
+        const int key0 = (blk_lo + 8 * c) * 8 + fc;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int kn = key0 + 8 * j + e;
+            const bool ok = kn >= j0 && kn < j1;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
+              float& x = s[4 * j + 2 * hh + e];
+              x = ok ? expf(x - mx[hh]) : 0.f;
+            }
+          }
+        {  // l: four chains per 32-key half, (l0 + l1) + (l2 + l3), added to the half's running sum
+          float ps[32];
+#pragma unroll
+          for (int i = 0; i < 32; ++i) ps[i] = __shfl_xor_sync(0xffffffffu, s[i], 2);
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+            for (int ch = 0; ch < 2; ++ch) {
+              float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+              for (int c4 = 0; c4 < 8; ++c4) {
+                s0 = __fadd_rn(s0, chain_val(s, ps, hh, ch, c4, 0));
+                s1 = __fadd_rn(s1, chain_val(s, ps, hh, ch, c4, 1));
+              }
+              const float sp = __fadd_rn(s0, s1);
+              lh[hh][ch] = __fadd_rn(lh[hh][ch], __fadd_rn(sp, __shfl_xor_sync(0xffffffffu, sp, 1)));
+            }
+        }
+        unsigned pf[3][4][4];
+        acc_to_a_split3<4, P>(s, pf);
+        float o[32];
+        wg_gemm6_rs_issue<64, 4, 1, false, P>(o, pf, [&](int sp, int kk) {
+          return b_desc_ex(v_saddr + sp * AT_RES_PLANE + c * AT_CHUNK_BYTES + kk * 2048, 1024, 128); }, false);
+        wg_mma_wait(o);
+        // chunks summed with round-to-nearest FADDs, as in attention64_tc_kernel
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o_acc[i] = __fadd_rn(o_acc[i], o[i]);
+      }
+      // ---------------- mu = O / l ------------------------------------------------------------------------------------
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const float l = __fadd_rn(lh[hh][0], lh[hh][1]);
+        const float inv = l > 0.f ? 1.f / l : 0.f;
+        const int row = fr0 + 8 * hh;
+        if (row < nvalid) {
+          float* dst = mu + (long)(node0 + row) * EQD_HID + fc;
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o_acc[4 * j + 2 * hh] * inv, o_acc[4 * j + 2 * hh + 1] * inv);
+        }
+      }
+    }
+    // both chains' MMAs on the planes are complete and every thread has observed this segment's phases: refill
+    __syncthreads();
+    if (fits) phase ^= 1;
+  }
+  cp_async_wait<0>();
+}
+
 template <int P>
 static int launch_attention64_tc(const eqd_graph* g, const float* proj, const void* kv, float* mu, void* stream) {
+  const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
+  if (g->max_segment_nodes > 0 && g->max_segment_nodes <= AT_RES_MAX_NODES) {
+    const size_t smem = sizeof(AtResSmem);
+    EQD_SET_SMEM(attention64_res_kernel<P>, smem);
+    const int grid = 2 * g->n_pairs < EQD_SMS ? 2 * g->n_pairs : EQD_SMS;
+    attention64_res_kernel<P><<<grid, AT_CHAINS * 128, smem, (cudaStream_t)stream>>>(
+        *g, proj, reinterpret_cast<const unsigned char*>(kv), split_stride, mu);
+    EQD_CUDA_LAUNCH_CHECK();
+    return EQD_OK;
+  }
   const size_t smem = AT_CHAINS * sizeof(AtChainSmem);
   EQD_SET_SMEM(attention64_tc_kernel<P>, smem);
   const int nht = 2 * g->n_node_tiles;
   int grid = (nht + AT_CHAINS - 1) / AT_CHAINS;
   if (grid > EQD_SMS) grid = EQD_SMS;
-  const long split_stride = (long)((g->n_nodes + 7) / 8 + 8) * 1024;
   attention64_tc_kernel<P><<<grid, AT_CHAINS * 128, smem, (cudaStream_t)stream>>>(
       *g, proj, reinterpret_cast<const unsigned char*>(kv), split_stride, mu);
   EQD_CUDA_LAUNCH_CHECK();

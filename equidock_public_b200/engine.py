@@ -355,13 +355,17 @@ class GraphPlan:
         g.col_src, g.edge_dst = col_src.data_ptr(), edge_dst.data_ptr()
         g.he_lig, g.he_rec = he_l.data_ptr(), he_r.data_ptr()
         g.n_node_tiles, g.node_tiles = self.n_node_tiles, node_tiles.data_ptr()
+        # lets the 64-wide attention keep each partner protein's K / V resident in shared memory when all of them fit
+        g.max_segment_nodes = max(self.n_lig_list + self.n_rec_list)
         self.struct = g
 
     def refresh(self, graph) -> bool:
         """Re-derives the topology arrays IN PLACE from a graph object whose tensors were overwritten with a new batch
         of the same shape signature (same per-pair node counts and edge totals): every device pointer of the plan stays
         valid, which is what a captured CUDA graph of the forward needs.  Returns False when the shapes differ (the
-        caller must build a new plan).  A handful of index ops on the current stream, no host sync."""
+        caller must build a new plan).  A handful of index ops on the current stream, no host sync.  The descriptor's
+        ``max_segment_nodes`` (the largest protein, which selects the attention kernel) is left as it is: the per-protein
+        node counts are part of the shape signature, so it stays exact for every batch the plan serves."""
         n_l = [int(v) for v in graph.batch_num_nodes(LIGAND).tolist()]
         n_r = [int(v) for v in graph.batch_num_nodes(RECEPTOR).tolist()]
         src_l, dst_l = graph.edges(etype=LL)

@@ -73,6 +73,10 @@ typedef struct eqd_graph {
   const float* he_lig;        /* [n_lig_edges][27] edges['ll'].data['he'] */
   const float* he_rec;        /* [n_edges-n_lig_edges][27] edges['rr'].data['he'] */
   int32_t n_node_tiles;       /* number of (segment, first node) tiles of <=128 nodes */
+  int32_t max_segment_nodes;  /* upper bound on the nodes of any segment, 0 = unknown.  A bound of at most 248 lets the
+                                 64-wide attention copy each partner protein's K/V into shared memory once instead of
+                                 once per query tile; it must hold for every segment.  Sits in what was the padding
+                                 before node_tiles, so every other field keeps its offset */
   const int32_t* node_tiles;  /* [n_node_tiles][2] = {segment, first global node} */
 } eqd_graph;
 
