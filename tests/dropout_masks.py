@@ -7,6 +7,7 @@ keep(seed, rank, layer, site, row, col) = philox4x32_10(counter = (row, col >> 2
 """
 from __future__ import annotations
 
+import functools
 import math
 
 import numpy as np
@@ -49,9 +50,18 @@ def keep(seed, rank, layer, site, rows, cols, p):
     return word >= np.uint32(threshold(p))
 
 
+@functools.lru_cache(maxsize=64)
+def _keep_all(seed, rank, layer, site, n_rows, n_cols, p):
+    """keep over every row and column, cached: the masks of a 400 k-edge batch take seconds in numpy, and the forward
+    and backward tests of a stage draw the same ones."""
+    k = keep(seed, rank, layer, site, np.arange(n_rows), np.arange(n_cols), p)
+    k.setflags(write=False)
+    return k
+
+
 def mask(seed, rank, layer, site, n_rows, n_cols, p):
     """keep * scale as an fp64 torch tensor [n_rows][n_cols] (the factor the engine multiplies the site by)."""
-    k = keep(seed, rank, layer, site, np.arange(n_rows), np.arange(n_cols), p)
+    k = _keep_all(int(seed), int(rank), int(layer), int(site), int(n_rows), int(n_cols), float(p))
     return torch.from_numpy(k.astype(np.float64) * scale(p))
 
 

@@ -1,6 +1,8 @@
 """GPU (H100): every backward entry point (csrc/bwd_*.cu and the backward half of head.cu) called directly on seeded
 inputs and compared with a torch fp64 autograd of the forward formula of its stage -- independent of
-oracle/backward_manual.py, except for the head, whose reference is that file's kabsch_bwd / keypoints_bwd.
+oracle/backward_manual.py, except for the head, whose reference is that file's kabsch_bwd / keypoints_bwd.  The
+graph-input gradient kernels (eqd_bwd_layer_inputs, eqd_bwd_inputs) are compared with their fp64 formulas; the dropout
+variants of the edge and node kernels are in test_gpu_dropout_backward_kernels.py.
 
 The tile kernels are persistent (grid = min(tiles, 132), a CTA walks tile, tile + 132, ...).  The `bulk` batch (the
 ragged pairs of test_gpu_node_stage.py plus 100 pairs of 200 + 200 nodes, 41 510 nodes, 415 k edges) gives every CTA
@@ -17,7 +19,12 @@ cases of each test):
   edge       ein 5.9e-9, n1 4.3e-7, msg 1.0e-6, dz3 8.0e-8, dmsg 5.3e-7, dz1 5.2e-7, dxrel 1.6e-7,
              dgamma 1.5e-7, dbeta 3.4e-7, dw4 5.3e-7, db4 4.6e-7
   gather     dPsrc 3.6e-7, dPdst 2.9e-7, dx 2.8e-9;  project dh 1.9e-7;  embed demb 5.2e-7;  head dh 3.0e-7, dx 2.5e-7
+  inputs     layer inputs dhe 1.1e-7 (dx_orig exact);  d mu_r_norm within 1.47 fp32 ulp, dx 7.0e-17 (700 W power limit)
 (the printed report of `pytest -s` lists every value).
+
+The graph-input gradient kernels have their own bounds: eqd_bwd_layer_inputs' dhe 1e-5, its dx_orig += eta dx_out exact
+(one fp64 rounding, or none through an FMA); eqd_bwd_inputs' d mu_r_norm within 2 fp32 ulp (a sum and a quotient in
+fp32) and its dx within 1e-14 (products of fp32 values are exact in fp64, leaving three fp64 additions).
 
 The LeakyReLU kink: the kernels recompute z1, z3 (edge) and u5 (node) in fp32.  Where an fp64 pre-activation lies
 within the fp32 error of its dot product of 0, the kernel may take the other branch and its derivative differs by
@@ -334,12 +341,23 @@ def test_bwd_edge_vs_fp64_autograd(kind, li, cuda_device):
         return (*outs, dxrel, sums)
 
     ein, n1, msg, dz3, dmsg, dz1, dxrel, sums = _twice(run)
+    ref = _bwd_edge_ref(mod, plan, proj, x_in, daggr, dx_out)
+    _bwd_edge_report(Report(f'edge[{kind}, L{li}]'), ref, ein, n1, msg, dz3, dmsg, dz1, dxrel, sums).check()
 
-    # fp64 autograd of the edge stage (:204-237, 263-292)
+
+def _bwd_edge_ref(mod, plan, proj, x_in, daggr, dx_out, m0=None, m1=None):
+    """fp64 autograd of the edge stage (:204-237, 263-292), with the dropout factors m0 / m1 [E][64] (site 0 on z1,
+    site 1 on z3) when given.  Returns the reference tensors, the rows outside the LeakyReLU kink band (`ok`) and the
+    slack of d gamma / d beta for the z3 elements inside it."""
     lin1, ln, lin2 = mod.edge_mlp[0], mod.edge_mlp[3], mod.edge_mlp[4]
     lin3, lin4 = mod.coors_mlp[0], mod.coors_mlp[4]
-    slope, dh = float(mod.leakyrelu_neg_slope), tp.dh
+    slope, dh = float(mod.leakyrelu_neg_slope), int(mod.att_mlp_Q[0].weight.shape[0])
+    N, E, dev = plan.N, plan.E, x_in.device
+    ones = torch.ones(E, 64, dtype=F64, device=dev)
+    m0 = ones if m0 is None else m0
+    m1 = ones if m1 is None else m1
     src, dst = plan.col_src.long(), plan.edge_dst.long()
+    deg = (plan.row_ptr[1:] - plan.row_ptr[:-1]).long()
     he = torch.cat([plan.he_l, plan.he_r]).to(F64)
     xrel = (x_in[src] - x_in[dst]).requires_grad_(True)
     d2 = (xrel ** 2).sum(1, keepdim=True)
@@ -350,46 +368,55 @@ def test_bwd_edge_vs_fp64_autograd(kind, li, cuda_device):
     z1 = P[src, 0:64] + P[dst, 64:128] + ein_ref @ w1e.t()
     gamma, beta, w4, b4 = _leaf(ln.weight), _leaf(ln.bias), _leaf(lin4.weight), _leaf(lin4.bias)
     z1.retain_grad()
-    n1_ref = F.layer_norm(F.leaky_relu(z1, slope), (64,), gamma, beta, ln.eps)
-    nhat = F.layer_norm(F.leaky_relu(z1, slope), (64,)).detach()
+    a1 = F.leaky_relu(z1 * m0, slope)
+    n1_ref = F.layer_norm(a1, (64,), gamma, beta, ln.eps)
+    nhat = F.layer_norm(a1, (64,)).detach()
     msg_ref = n1_ref @ _d(lin2.weight).t() + _d(lin2.bias)
     msg_ref.retain_grad()
     z3 = msg_ref @ _d(lin3.weight).t() + _d(lin3.bias)
     z3.retain_grad()
-    phi = F.leaky_relu(z3, slope) @ w4.t() + b4
+    c3 = F.leaky_relu(z3 * m1, slope)
+    c3.retain_grad()
+    phi = c3 @ w4.t() + b4
     inv = 1.0 / deg.clamp(min=1).to(F64)[:, None]
     aggr = torch.zeros(N, 64, dtype=F64, device=dev).index_add_(0, dst, msg_ref) * inv
     xupd = torch.zeros(N, 3, dtype=F64, device=dev).index_add_(0, dst, xrel * phi) * inv
     ((aggr * _d(daggr)).sum() + (xupd * dx_out).sum()).backward()
 
-    t1 = P[src, 0:64].abs() + P[dst, 64:128].abs() + ein_ref.detach().abs() @ w1e.abs().t()
-    t3 = msg_ref.detach().abs() @ _d(lin3.weight).abs().t() + _d(lin3.bias).abs()
-    near3 = z3.detach().abs() < KINK_BAND * t3
-    ok = ~(_kink_rows(z1.detach(), t1, 'z1') | _kink_rows(z3.detach(), t3, 'z3'))
-    # dgamma / dbeta sum over every edge: a z3 element inside the band can move them by (1 - slope) |dphi w4_j| times
-    # row j of |W3 W2| (times |n-hat| for dgamma)
+    # the kink test over the elements the masks keep (a dropped element enters the LeakyReLU as an exact 0)
+    t1 = (P[src, 0:64].abs() + P[dst, 64:128].abs() + ein_ref.detach().abs() @ w1e.abs().t()) * m0
+    t3 = (msg_ref.detach().abs() @ _d(lin3.weight).abs().t() + _d(lin3.bias).abs()) * m1
+    pre1, pre3 = z1.detach() * m0, z3.detach() * m1
+    near3 = (pre3.abs() < KINK_BAND * t3) & (m1 != 0)
+    ok = ~(_kink_rows(torch.where(m0 != 0, pre1, torch.inf), t1, 'z1')
+           | _kink_rows(torch.where(m1 != 0, pre3, torch.inf), t3, 'z3'))
+    # dgamma / dbeta sum over every edge: a z3 element inside the band can move them by (1 - slope) |dc3_j m1_j| (dc3 =
+    # the gradient w.r.t. LeakyReLU(z3 m1) = dphi w4_j) times row j of |W3 W2| (times |n-hat| for dgamma)
     rows, cols = near3.nonzero(as_tuple=True)
-    dphi = (xrel.detach() * (_d(dx_out) * inv)[dst]).sum(1)
-    mag = (1.0 - slope) * (dphi[rows] * _d(lin4.weight)[0, cols]).abs()
+    mag = (1.0 - slope) * (c3.grad[rows, cols] * m1[rows, cols]).abs()
     w32 = (_d(lin3.weight) @ _d(lin2.weight)).abs()               # [j][c]: dn_c per unit dz3_j
-    slack_b = (mag[:, None] * w32[cols]).sum(0)
-    slack_g = (mag[:, None] * w32[cols] * nhat[rows].abs()).sum(0)
+    return {'ein': ein_ref.detach(), 'n1': n1_ref.detach(), 'msg': msg_ref.detach(), 'dz3': z3.grad,
+            'dmsg': msg_ref.grad, 'dz1': z1.grad, 'dxrel': xrel.grad, 'dgamma': gamma.grad, 'dbeta': beta.grad,
+            'dw4': w4.grad[0], 'db4': b4.grad, 'ok': ok, 'n_band3': rows.numel(),
+            'slack_b': (mag[:, None] * w32[cols]).sum(0), 'slack_g': (mag[:, None] * w32[cols] * nhat[rows].abs()).sum(0)}
 
-    rep = Report(f'edge[{kind}, L{li}]')
-    rep.rel('ein', ein[:, :42], ein_ref.detach())
+
+def _bwd_edge_report(rep, ref, ein, n1, msg, dz3, dmsg, dz1, dxrel, sums):
+    """eqd_bwd_edge's per-edge outputs and its reduced 193 per-CTA sums against _bwd_edge_ref."""
+    ok = ref['ok']
+    rep.rel('ein', ein[:, :42], ref['ein'])
     assert float(ein[:, 42:].abs().max()) == 0.0
-    rep.rel('n1', n1, n1_ref.detach())
-    rep.rel('msg', msg, msg_ref.detach())
-    rep.rel('dz3', dz3, z3.grad, ok)
-    rep.rel('dmsg', dmsg, msg_ref.grad, ok)
-    rep.rel('dz1', dz1, z1.grad, ok)
-    rep.rel('dxrel', dxrel, xrel.grad, ok)
-    rep.rel(f'dgamma ({rows.numel()} z3 in band)', sums[0:64], gamma.grad, slack=slack_g)
-    rep.rel('dbeta', sums[64:128], beta.grad, slack=slack_b)
-    rep.rel('dw4', sums[128:192], w4.grad[0])
-    rep.rel('db4', sums[192:193], b4.grad)
-    rep.check()
-
+    rep.rel('n1', n1, ref['n1'])
+    rep.rel('msg', msg, ref['msg'])
+    rep.rel('dz3', dz3, ref['dz3'], ok)
+    rep.rel('dmsg', dmsg, ref['dmsg'], ok)
+    rep.rel('dz1', dz1, ref['dz1'], ok)
+    rep.rel('dxrel', dxrel, ref['dxrel'], ok)
+    rep.rel(f'dgamma ({ref["n_band3"]} z3 in band)', sums[0:64], ref['dgamma'], slack=ref['slack_g'])
+    rep.rel('dbeta', sums[64:128], ref['dbeta'], slack=ref['slack_b'])
+    rep.rel('dw4', sums[128:192], ref['dw4'])
+    rep.rel('db4', sums[192:193], ref['db4'])
+    return rep
 
 # ---- gather, projections, embedding -------------------------------------------------------------------------------
 
@@ -485,6 +512,124 @@ def test_bwd_embed_vs_fp64(cuda_device):
     ((emb[res] * (_d(dh0) + _d(dhl0))[:, :64]).sum()).backward()
     rep = Report('embed[bulk]')
     rep.rel('demb (accumulated)', out, _d(demb0) + emb.grad)
+    rep.check()
+
+
+# ---- graph-input gradients ----------------------------------------------------------------------------------------
+
+def _fma_or_two_roundings(got, a, b, c):
+    """True where got == fl(a + fl(b c)) or == fma(b, c, a) (the compiler may contract the update), in fp64."""
+    got, a, b, c = (t.cpu().numpy().ravel() for t in (got, a, b, c))
+    ok = got == a + b * c
+    from fractions import Fraction
+    for i in np.flatnonzero(~ok):
+        ok[i] = float(got[i]) == float(Fraction(float(a[i])) + Fraction(float(b[i])) * Fraction(float(c[i])))
+    return bool(ok.all())
+
+
+@pytest.mark.parametrize('li,eta', [(1, 0.0), (1, 0.3), (0, 0.0), (0, 0.3)])
+def test_bwd_layer_inputs_vs_fp64(li, eta, cuda_device):
+    """eqd_bwd_layer_inputs on the bulk batch: dhe += dz1 . W1[:, 2 dh : 2 dh + 27]^T (edge_mlp.0.weight's he block,
+    69 + 69 columns in front of it in layer 0), accumulated into a non-zero dhe, and dx_orig += eta dx_out, exact (eta =
+    0: bitwise unchanged).  The grid is min(max(edge tiles, 3N / 128), 4 x 132) = 528 CTAs: each walks about 6 edge
+    tiles (the last one short) and takes two passes over the 3N coordinates."""
+    dev, lib = cuda_device, nat.load()
+    _, plan = _batch('bulk', dev)
+    mod, lay, _ = _layer(li, dev)
+    N, E, dh = plan.N, plan.E, int(mod.att_mlp_Q[0].weight.shape[0])
+    grid = min(max((E + 127) // 128, (3 * N + 127) // 128), 4 * SMS)
+    assert (E + 127) // 128 >= 2 * grid and 3 * N > grid * 128 and E % 128 != 0
+    desc = nat.EqdLayer.from_buffer_copy(lay.struct)
+    desc.dev.x_connection_init = eta
+    eta32 = float(np.float32(eta))
+    r = _gen(650 + li, dev)
+    dz1 = r(E, 64, s=0.1)
+    dx_out = r(N, 3).double()
+    dhe0, dxo0 = r(E + 3, 27), r(N + 1, 3).double()
+    sentinel = -777.25
+    dhe0[E:], dxo0[N:] = sentinel, sentinel
+
+    def run():
+        dhe, dxo = dhe0.clone(), dxo0.clone()
+        nat.check(lib.eqd_bwd_layer_inputs(C.byref(plan.struct), C.byref(desc), nat.ptr(dz1), nat.ptr(dx_out),
+                                           nat.ptr(dhe), nat.ptr(dxo), None), 'eqd_bwd_layer_inputs')
+        return dhe, dxo
+
+    dhe, dxo = _twice(run)
+    assert bool((dhe[E:] == sentinel).all()) and bool((dxo[N:] == sentinel).all()), 'rows past the end were written'
+    w_he = _d(mod.edge_mlp[0].weight)[:, 2 * dh:2 * dh + 27]
+    rep = Report(f'layer inputs[bulk, L{li}, eta {eta}]')
+    rep.rel('dhe (accumulated)', dhe[:E], _d(dhe0[:E]) + _d(dz1) @ w_he)
+    rep.check()
+    if eta == 0.0:
+        assert torch.equal(dxo, dxo0), 'eta = 0: dx_orig must be bitwise unchanged'
+    else:
+        assert _fma_or_two_roundings(dxo[:N], dxo0[:N], torch.full_like(dx_out, eta32), dx_out), \
+            'dx_orig += eta dx_out is not exact'
+
+
+def _pair_of_node(n_lig):
+    """[N_l] pair index of every ligand node (ligands in pair order, n_lig[b] nodes each)."""
+    return torch.repeat_interleave(torch.arange(len(n_lig)), torch.tensor(n_lig))
+
+
+@pytest.mark.parametrize('kind,with_dcoors', [('bench', True), ('bench', False), ('ragged', True), ('ragged', False)])
+def test_bwd_inputs_vs_fp64(kind, with_dcoors, cuda_device):
+    """eqd_bwd_inputs (one thread per node, each ligand node finding its pair by a binary search over seg_ptr): on the
+    bench batch's 330 ligands and the ragged batch's ligands of 1 .. 200 nodes, with a distinct rotation per pair.
+    d mu_r_norm = (dh0_acc + dh_layer0)[64:69] / mu_r_norm within 2 fp32 ulp; dx = dx_layer0 + dx_orig (+ T_b^T dcoors
+    on ligand rows) within 1e-14 (the fp32 products are exact in fp64); receptor rows, and every row without dcoors,
+    bitwise equal to dx_layer0 + dx_orig; the first and the last node of every ligand checked on their own."""
+    from test_gpu_forward_kernels import _fbatch
+    dev, lib = cuda_device, nat.load()
+    _, plan = _fbatch(kind, dev)
+    N, NL, B = plan.N, plan.N_l, plan.n_pairs
+    seg = [int(v) for v in plan.seg_ptr_host]
+    n_lig = [seg[b + 1] - seg[b] for b in range(B)]
+    if kind == 'bench':
+        assert B == 330
+    else:
+        assert min(n_lig) == 1 and max(n_lig) >= 129
+    r = _gen(660, dev)
+    dh0, dhl0 = r(N, nat.H0_PAD), r(N, nat.H0_PAD)
+    mu = torch.exp(r(N, 5, s=0.5))
+    mu_l, mu_r = mu[:NL].contiguous(), mu[NL:].contiguous()
+    dx_l0, dx_orig = r(N, 3).double(), r(N, 3).double()
+    rot = torch.linalg.qr(r(B, 3, 3).double())[0].float().contiguous()    # a distinct rotation per pair
+    dcoors = r(NL, 3, s=0.05) if with_dcoors else None
+
+    def run():
+        dmu = torch.full((N + 2, 5), -777.25, device=dev)
+        dx = torch.full((N + 2, 3), -777.25, dtype=F64, device=dev)
+        nat.check(lib.eqd_bwd_inputs(C.byref(plan.struct), nat.ptr(dh0), nat.ptr(dhl0), nat.ptr(mu_l), nat.ptr(mu_r),
+                                     nat.ptr(dx_l0), nat.ptr(dx_orig), nat.ptr(rot),
+                                     nat.ptr(dcoors) if dcoors is not None else None, nat.ptr(dmu), nat.ptr(dx), None),
+                  'eqd_bwd_inputs')
+        return dmu, dx
+
+    dmu, dx = _twice(run)
+    assert bool((dmu[N:] == -777.25).all()) and bool((dx[N:] == -777.25).all()), 'rows past the end were written'
+    dmu, dx = dmu[:N], dx[:N]
+    dmu_ref = (_d(dh0) + _d(dhl0))[:, 64:69] / _d(mu)
+    ulp = torch.from_numpy(np.spacing(np.abs(dmu_ref.cpu().numpy()).astype(np.float32)).astype(np.float64)).to(dev)
+    worst = float(((_d(dmu) - dmu_ref).abs() / ulp).max())
+    print(f'\nbwd inputs[{kind}, dcoors {with_dcoors}]: dmu {worst:.2f} fp32 ulp')
+    assert worst <= 2.0, f'dmu: {worst:.2f} ulp'
+    base = dx_l0 + dx_orig
+    assert torch.equal(dx[NL:], base[NL:]), 'receptor rows must be dx_layer0 + dx_orig, bitwise'
+    if dcoors is None:
+        assert torch.equal(dx[:NL], base[:NL]), 'without dcoors every row must be dx_layer0 + dx_orig, bitwise'
+        return
+    pair = _pair_of_node(n_lig).to(dev)
+    ref = base[:NL] + torch.einsum('nrc,nr->nc', _d(rot).view(B, 3, 3)[pair], _d(dcoors))
+    firsts = torch.tensor(seg[:B], device=dev)
+    lasts = torch.tensor(seg[1:B + 1], device=dev) - 1
+    rep = Report(f'bwd inputs[{kind}]', 1e-14)
+    rep.rel('dx ligand rows', dx[:NL], ref)
+    for tag, rows in (('first', firsts), ('last', lasts)):
+        err = (dx[rows] - ref[rows]).abs().max(1).values / float(ref.abs().max())
+        rep.rel(f'dx {tag} node of every ligand', dx[rows], ref[rows])
+        assert bool((err <= 1e-14).all()), f'{tag} nodes of pairs {torch.nonzero(err > 1e-14).flatten().tolist()}'
     rep.check()
 
 

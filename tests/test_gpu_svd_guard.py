@@ -46,7 +46,18 @@ def _min_gap(covs):
 
 HEAD_CASES = ([(K, kind, 0.0, False) for K in (1, 2, 3, 4, 50) for kind in ('single', 'ragged3', 'sizes')]
               + [(K, 'ragged3', 0.25, False) for K in (1, 2, 3, 4, 50)]
-              + [(K, 'ragged3', 0.0, True) for K in (4, 50)])
+              + [(K, 'ragged3', 0.0, True) for K in (4, 50)]
+              + [(K, 'bulk', 0.25, False) for K in (25, 50, 64)])
+
+
+def _head_batch(kind, dev):
+    """(graph, plan) of a head case: test_gpu_heads' pairs, or test_gpu_backward_kernels' bulk batch (109 pairs,
+    41 510 nodes, 422 node tiles)."""
+    if kind == 'bulk':
+        from test_gpu_backward_kernels import _batch
+        return _batch('bulk', dev)
+    g = gio.make_batch(_pairs(kind), dev)
+    return g, GraphPlan.from_graph(g, dev, 10)
 
 
 @pytest.mark.parametrize('K,kind,p,small', HEAD_CASES)
@@ -58,7 +69,9 @@ def test_head_kernels_through_the_perturbed_covariance_vs_fp64(K, kind, p, small
     them would not show here: the means themselves are checked against fp64 by test_gpu_heads.py's forward-kernel test
     (qbar), and their gradient path (dpre) here.  Trained weights (the shipped checkpoint with seeded K-head key / query
     projections), and ``small``: key / query weights scaled by 1e-3, so that the keypoints collapse onto their centroid as
-    at initialisation and the guard fires on every pair.
+    at initialisation and the guard fires on every pair.  `bulk` (p = 0.25, K = 25, 50, 64): the dropout backward over
+    109 pairs, its site-3 mask replayed on 41 510 nodes, after a re-run of the forward's mean kernel (422 node tiles on
+    264 CTAs: 158 of them walk a second tile).
 
     K = 2 and 3 with trained weights are tested here, at the head level, only: after the noise the perturbed A has one
     large singular value next to two of size ~1 (e.g. S = (7.1e3, 0.68, 0.57)), so the rotation about the two small axes
@@ -66,8 +79,9 @@ def test_head_kernels_through_the_perturbed_covariance_vs_fp64(K, kind, p, small
     kernels' own h / x / means the fp64 tail sees delta at fp64 level; a whole-model comparison would see the fp32-level
     delta of the layers, amplified by ~1e4."""
     dev, lib = cuda_device, nat.load()
-    g = gio.make_batch(_pairs(kind), dev)
-    plan = GraphPlan.from_graph(g, dev, 10)
+    g, plan = _head_batch(kind, dev)
+    if kind == 'bulk':      # the mean kernel that eqd_bwd_head_dropout re-runs (grid 264) walks a second tile
+        assert plan.n_node_tiles > 264 and plan.n_pairs > 100
     model = hr.build_model('dips', dev, K, seed=K)
     net = model.iegmn_original
     if small:
