@@ -217,7 +217,9 @@ extern "C" int eqd_sqnorm_partials(const float* g, int64_t n, double* partial, i
 extern "C" int eqd_clip_adam(float* w, float* g, float* m, float* v, int64_t n, const double* sq_partial,
                              int32_t n_partial, float max_norm, float lr, float beta1, float beta2, float eps,
                              float weight_decay, int32_t step, float scale_extra, float* norm_out, void* stream) {
-  if (!w || !g || !m || !v || !sq_partial || n < 0 || step < 1) return EQD_ERR_BAD_ARG;
+  // the partial count is that of eqd_sqnorm_partials: with 0 the norm would read as 0 and clipping would silently not run
+  if (!w || !g || !m || !v || !sq_partial || n < 0 || step < 1 || n_partial <= 0 || n_partial > 1024)
+    return EQD_ERR_BAD_ARG;
   if (n == 0) return EQD_OK;
   const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
   eqd::clip_adam_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(

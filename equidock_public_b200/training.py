@@ -675,7 +675,9 @@ class DataParallelTrainer:
         self.layout = self.engine.layout
         dev = self.engine.device
         self.device, self.world, self.group = dev, int(world), group
-        self.flat_w = torch.empty(self.layout.total, dtype=_f32, device=dev)
+        # zeroed: the alignment padding between parameters must stay 0, or Adam's weight decay would carry whatever it
+        # held into m and v, and flat_w would differ between ranks there
+        self.flat_w = torch.zeros(self.layout.total, dtype=_f32, device=dev)
         with torch.no_grad():
             for p, v in zip(self.layout.params, self.layout.views(self.flat_w)):
                 v.copy_(p.detach().to(_f32))

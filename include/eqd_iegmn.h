@@ -631,7 +631,8 @@ int eqd_rmsd_meter(const eqd_graph* g, const float* lig_pred, const float* rec_p
                    const float* rec_true, double* out /*[B][3]*/, void* stream);
 
 /* ---- optimiser side on the flat fp32 parameter / gradient buffers (src/train.py:156, 165, 302) -----------------------
- * eqd_sqnorm_partials: partial[i] = sum of squares of slice i (n_partial <= 1024 doubles).  eqd_clip_adam: g *= scale_extra;
+ * eqd_sqnorm_partials: partial[i] = sum of squares of slice i (1 <= n_partial <= 1024 doubles, for both calls; other
+ * counts are refused).  eqd_clip_adam: g *= scale_extra;
  * clip_grad_norm_(max_norm) with the global norm sqrt(sum partial) * |scale_extra|; torch.optim.Adam step (L2 weight decay,
  * bias correction at `step` >= 1); norm_out (device float, may be NULL) receives the pre-clip norm.                     */
 int eqd_sqnorm_partials(const float* g, int64_t n, double* partial, int32_t n_partial, void* stream);
