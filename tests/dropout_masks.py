@@ -80,8 +80,9 @@ SIGMAS = [1.5 ** s for s in range(15)]
 
 
 def _segmean(v, idx, n):
-    out = torch.zeros((n,) + tuple(v.shape[1:]), dtype=v.dtype).index_add_(0, idx, v)
-    deg = torch.zeros(n, dtype=v.dtype).index_add_(0, idx, torch.ones(idx.shape[0], dtype=v.dtype))
+    out = torch.zeros((n,) + tuple(v.shape[1:]), dtype=v.dtype, device=v.device).index_add_(0, idx, v)
+    deg = torch.zeros(n, dtype=v.dtype, device=v.device).index_add_(0, idx, torch.ones(idx.shape[0], dtype=v.dtype,
+                                                                                      device=v.device))
     return out / deg.clamp(min=1).unsqueeze(1)
 
 

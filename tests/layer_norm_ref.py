@@ -14,8 +14,10 @@ import dropout_masks as dm
 import golden_io as gio
 
 
-def layer_forward(p, x, h, x0, h0, src, dst, he, seg, B, slope, skip, eta, masks=None, li=0):
-    """dropout_masks.layer_forward with the coordinate LayerNorm when p has coors_mlp.3.weight."""
+def layer_forward(p, x, h, x0, h0, src, dst, he, seg, B, slope, skip, eta, masks=None, li=0, taps=None):
+    """dropout_masks.layer_forward with the coordinate LayerNorm when p has coors_mlp.3.weight.  A dict ``taps``
+    receives the two node-MLP inputs the engine stashes for its backward: 'aggr' (the mean message) and 'mu' (the
+    cross-attention output)."""
     lr = lambda t: F.leaky_relu(t, slope)
     N = x.shape[0]
     m = (lambda site, dh=64: masks(li, site, dh)) if masks is not None else (lambda site, dh=64: 1.0)
@@ -39,7 +41,10 @@ def layer_forward(p, x, h, x0, h0, src, dst, he, seg, B, slope, skip, eta, masks
         c3 = F.layer_norm(c3, (c3.shape[1],), p['coors_mlp.3.weight'], p['coors_mlp.3.bias'])
     coef = F.linear(c3, p['coors_mlp.4.weight'], p['coors_mlp.4.bias'])
     x_new = eta * x0 + (1. - eta) * x + dm._segmean(x_rel * coef, dst, N)
-    u5 = F.linear(torch.cat([h, dm._segmean(msg, dst, N), mu, h0], dim=-1), p['node_mlp.0.weight'], p['node_mlp.0.bias'])
+    aggr = dm._segmean(msg, dst, N)
+    if taps is not None:
+        taps.update(aggr=aggr, mu=mu)
+    u5 = F.linear(torch.cat([h, aggr, mu, h0], dim=-1), p['node_mlp.0.weight'], p['node_mlp.0.bias'])
     hid = F.layer_norm(lr(u5 * m(2, u5.shape[1])), (u5.shape[1],), p['node_mlp.3.weight'], p['node_mlp.3.bias'])
     h_new = F.linear(hid, p['node_mlp.4.weight'], p['node_mlp.4.bias'])
     if h_new.shape[1] == h.shape[1]:

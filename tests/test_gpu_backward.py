@@ -255,32 +255,6 @@ def test_ragged_batch_gradient_is_the_sum_of_pair_gradients(cuda_device):
     assert not bad, bad
 
 
-def test_tn_gemm_and_reduce_vs_torch(cuda_device):
-    lib = nat.load()
-    torch.manual_seed(0)
-    # the last five: the training shapes of 100 pairs of 200 + 200 nodes (E = 400 000 edge rows, N = 40 000 node rows)
-    for rows, K, nc, ldx, ldd in ((1000, 64, 64, 64, 64), (37, 44, 64, 44, 64), (5000, 72, 344, 72, 344), (300, 72, 72, 72, 72),
-                                  (400000, 64, 64, 64, 64), (400000, 44, 64, 44, 64), (40000, 64, 320, 64, 320),
-                                  (40000, 72, 344, 72, 344), (40000, 64, 72, 64, 72)):
-        X = torch.randn(rows, ldx, device=cuda_device)
-        D = torch.randn(rows, ldd, device=cuda_device)
-        need = int(lib.eqd_tn_partial_floats(rows, K, nc, None, None))
-        part = torch.empty(need, device=cuda_device)
-        cs = torch.empty(4096 * nc, device=cuda_device)
-        nch = C.c_int32(0)
-        st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        nat.check(lib.eqd_tn_gemm(nat.ptr(X), ldx, K, nat.ptr(D), ldd, nc, rows, 0.5, nat.ptr(part), nat.ptr(cs), C.byref(nch), st), 'tn')
-        grad = torch.zeros(K * nc + nc, device=cuda_device)
-        idx = torch.arange(K * nc, dtype=torch.int32, device=cuda_device)
-        nat.check(lib.eqd_grad_reduce(nat.ptr(part), nch.value, K * nc, nat.ptr(idx), nat.ptr(idx), K * nc, nat.ptr(grad), st), 'red')
-        idc = torch.arange(nc, dtype=torch.int32, device=cuda_device)
-        dst = (idc + K * nc).contiguous()
-        nat.check(lib.eqd_grad_reduce(nat.ptr(cs), nch.value, nc, nat.ptr(idc), nat.ptr(dst), nc, nat.ptr(grad), st), 'red')
-        ref = 0.5 * (X[:, :K].double().t() @ D[:, :nc].double())
-        assert (grad[:K * nc].view(K, nc).double() - ref).abs().max() < 1e-3 * ref.abs().max()
-        assert (grad[K * nc:].double() - 0.5 * D[:, :nc].double().sum(0)).abs().max() < 1e-3 * rows ** 0.5
-
-
 def test_clip_adam_kernel_vs_torch_adam(cuda_device):
     lib = nat.load()
     torch.manual_seed(1)
