@@ -387,6 +387,7 @@ class GraphPlan:
         for own, new in ((self.he_l, graph.edges[LL].data['he']), (self.he_r, graph.edges[RR].data['he'])):
             if own.data_ptr() != new.data_ptr():
                 own.copy_(new)
+        self.edge_perm = None     # the arrays now hold the graph's edges in its own order (sorted copies of them or not)
         return True
 
     @classmethod

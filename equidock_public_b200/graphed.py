@@ -5,17 +5,19 @@ Captured once into a CUDA graph, a step costs the host ONE ``cudaGraphLaunch`` -
 process that shares its cores with seven other ranks (round-1 SCALE run: 7 ms of GPU idle per 4 ms of kernels).
 
 ``GraphedForward(model, device_batch)`` owns the captured graph together with everything it points at: the batch's
-device tensors, its ``GraphPlan`` (topology arrays), the workspace, the outputs and one pinned status buffer.  A new
-batch of the SAME shape signature is served by overwriting the batch tensors in place and calling ``refresh()``
-(``GraphPlan.refresh`` re-derives the CSR in place); ``launch()`` replays the graph and returns a handle whose
-``result()`` waits for the replay, inspects the per-pair status words and -- only if the SVD guard, a NaN, an unsorted
-edge list or a bad residue index was flagged -- falls back to the eager path, which replays the reference's host-side
-control flow (rigid_docking_model.py:570-584).  The captured work is exactly the eager path's: same kernels, same
-order, same buffers.
+device tensors, its ``GraphPlan`` (topology arrays), the packed layer and head weights, the workspace, the outputs and
+one pinned status buffer.  A new batch of the SAME shape signature is served by overwriting the batch tensors in place
+and calling ``refresh()`` (``GraphPlan.refresh`` re-derives the CSR in place); ``launch()`` replays the graph and
+returns a handle whose ``result()`` waits for the replay, inspects the per-pair status words and -- only if the SVD
+guard, a NaN, an unsorted edge list or a bad residue index was flagged -- falls back to the eager path, which replays
+the reference's host-side control flow (rigid_docking_model.py:570-584).  The captured work is exactly the eager
+path's: same kernels, same order, same buffers.
 
 The graph is tied to the parameter version and the precision (``IEGMN.precision``) it was captured with (kernel
 parameter banks hold small per-layer vectors and the product count selects the kernels): ``launch()`` re-captures when
-either changed.
+either changed.  Every weight update moves a parameter's version: optimizer steps and ``load_state_dict`` write the
+parameters in place, and ``training.DataParallelTrainer.step``, whose fused Adam writes them through a raw pointer,
+bumps the versions itself.
 """
 from __future__ import annotations
 
@@ -68,6 +70,9 @@ class GraphedForward:
             self.stream.synchronize()
             self.plan = self.batch._eqd_plan
             self.key = self._param_key()
+            # the packed weights the warm-up cached and the capture records: the graph reads their device buffers
+            self.packed = ([lay.packed(self.device) for lay in self.iegmn.iegmn_layers],
+                           self.iegmn.packed_head(self.device))
             self.graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self.graph, stream=self.stream):
                 self.before_forward()
@@ -76,8 +81,13 @@ class GraphedForward:
 
     def refresh(self) -> bool:
         """Call after overwriting the batch's device tensors in place with a new same-shaped batch (on the current
-        stream).  False = the shapes changed: build a new GraphedForward."""
-        return self.plan.refresh(self.batch)
+        stream).  False = the shapes changed: build a new GraphedForward.  The refreshed plan becomes the batch's plan
+        again, so that the eager fallback of a flagged replay runs on this batch's topology, not on a destination-sorted
+        copy an earlier batch's fallback left on the batch object."""
+        if not self.plan.refresh(self.batch):
+            return False
+        self.batch._eqd_plan = self.plan
+        return True
 
     def launch(self) -> 'GraphedPending':
         if self._param_key() != self.key:

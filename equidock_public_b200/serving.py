@@ -4,7 +4,7 @@ stream and batch k-1's status words / results are read back -- so end-to-end thr
 instead of their sum.  Every batch still goes through ``Rigid_Body_Docking_Net.forward_async`` (same kernels, same
 status handling as ``model(graph, epoch)``).
 
-Device input buffers and pinned result buffers live in two reusable slots (keyed by the batch's tensor shapes), so a
+Device input buffers and pinned result buffers live in three reusable slots (keyed by the batch's tensor shapes), so a
 steady stream of same-shaped batches performs no allocation at all; the copy stream waits for a slot's previous
 consumer before overwriting it.  With ``use_cuda_graph=True`` (default) every slot also owns a captured CUDA graph of the
 forward (``graphed.GraphedForward``): a same-shaped batch is served by refreshing the slot's plan in place and ONE graph

@@ -697,10 +697,12 @@ class DataParallelTrainer:
         self.lib = nat.load()
 
     def invalidate_packed(self):
-        for lay in self.model.iegmn_original.iegmn_layers:
-            lay._packed = None
-        self.model.iegmn_original._head = None
-        self.engine._packs.clear()
+        """Tells every cache of the weights that they changed.  eqd_clip_adam writes flat_w through a raw pointer, which
+        moves neither a parameter's data_ptr nor its version counter; bumping the versions reaches every cache keyed on
+        them: the packed layers and head (IEGMN_Layer.packed, IEGMN.packed_head), the training packs built on those
+        (TrainEngine.layer_pack) and the CUDA graphs of the model's forward (graphed.GraphedForward), which re-capture
+        at their next launch."""
+        torch.autograd.graph.increment_version(self.layout.params)
 
     def step(self, graph, targets) -> Dict:
         from .losses import device_losses
