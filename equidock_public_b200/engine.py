@@ -620,7 +620,8 @@ class IEGMNEngine:
                 status_event.record()
             out = {'status_lease': lease, 'ligand_coors': lig_out, 'keypts': keyp, 'rotation': rot,
                    'translation': trans, 'h': h_fin, 'x64': x_fin, 'cov': cov, 'sing': sing, 'status': status,
-                   'unsorted': plan.unsorted, 'kabsch': kab, 'status_host': status_host, 'status_event': status_event, '_keep': (ws, ymean, x_l)}
+                   'unsorted': plan.unsorted, 'kabsch': kab, 'status_host': status_host, 'status_event': status_event,
+                   'stream': torch.cuda.current_stream(dev), '_keep': (ws, ymean, x_l)}
             if dropout is not None:
                 out.update(dropout_layers=descs, dropout_head=head_dropout(dropout, len(layers)))
             if check_status:
@@ -629,8 +630,11 @@ class IEGMNEngine:
 
     def resolve_status(self, plan: GraphPlan, out, kab, log=None):
         """The ONE host sync of a forward: reads the status words and replays the reference's
-        host-side control flow for flagged pairs (rigid_docking_model.py:570-584)."""
-        with torch.cuda.device(self.device):
+        host-side control flow for flagged pairs (rigid_docking_model.py:570-584).  The SVD guard's loop runs on the
+        forward's stream (``out['stream']``; None = the current one), where ``kab`` relaunches the Kabsch kernel: its
+        covariance perturbation, mask and status read are then ordered with that launch whichever stream is current
+        when the forward is resolved."""
+        with torch.cuda.device(self.device), torch.cuda.stream(out.get('stream')):
             try:
                 self._resolve_status(plan, out, kab, log)
             finally:

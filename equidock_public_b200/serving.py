@@ -124,6 +124,6 @@ class PipelinedInference:
             hbuf.copy_(t, non_blocking=True)
             out[key] = hbuf
         done = torch.cuda.Event()
-        done.record()
+        done.record(torch.cuda.current_stream(self.device))    # the copies' stream, also when another device is current
         out['_event'] = done
         return out
