@@ -18,6 +18,34 @@ namespace eqd {
 // and post == 0 exactly when pre <= 0 for slope == 0.
 __device__ __forceinline__ float lrelu_grad_from_post(float post, float slope) { return post > 0.f ? 1.f : slope; }
 
+// nn.LayerNorm backward of one row held by its 8 lanes: dnh = dL/d(output) * gamma and nhat = the normalised input at
+// this lane's 8 columns (with EXTRA also column 64 + tx in dnhx / nhx, 0 for a column past the row's width), rstd of the
+// row (ln_row_stats), inv_n = 1 / channel count.  Overwrites dnh (dnhx) with dL/d(input) = rstd (dnh - m1 - nhat m2),
+// m1 = mean(dnh), m2 = mean(dnh nhat); the caller multiplies in the activation's derivative afterwards.
+template <bool EXTRA>
+__device__ __forceinline__ void layernorm_bwd_row(float (&dnh)[8], float& dnhx, const float (&nhat)[8], float nhx,
+                                                  float rstd, float inv_n) {
+  float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    s1 += dnh[j];
+    s2 = fmaf(dnh[j], nhat[j], s2);
+  }
+  if (EXTRA) {
+    s1 += dnhx;
+    s2 = fmaf(dnhx, nhx, s2);
+  }
+  const float m1 = row_sum8(s1) * inv_n, m2 = row_sum8(s2) * inv_n;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) dnh[j] = rstd * (dnh[j] - m1 - nhat[j] * m2);
+  if (EXTRA) dnhx = rstd * (dnhx - m1 - nhx * m2);
+}
+// The same for a 64-wide row.
+__device__ __forceinline__ void layernorm_bwd_row(float (&dnh)[8], const float (&nhat)[8], float rstd) {
+  float unused = 0.f;
+  layernorm_bwd_row<false>(dnh, unused, nhat, 0.f, rstd, 1.f / 64.f);
+}
+
 // Adds this thread's 8 rows of an 8x8 micro-tile into per-thread column accumulators (column map col_nn).
 __device__ __forceinline__ void colacc8(float (&s)[8], const float (&v)[8][8]) {
 #pragma unroll

@@ -13,30 +13,19 @@
 // over IN-edges, dx = (1 - eta) dx' + sum_out dx_rel - sum_in dx_rel: fixed summation order, no atomics.
 // Restated in oracle/backward_manual.py::edge_bwd / edge_gather.
 #include "bwd_common.cuh"
-#include "philox.cuh"
+#include "edge_tile.cuh"
 
 namespace eqd {
 
-#define BE_K1 44
-#define BE_LD1 48
-#define BE_LD 68
-
-struct EdgeBwdSmem {
-  float w1[BE_K1 * 64];        // k-major [he|rbf feature][out]
-  float w2[64 * 64];           // k-major edge_mlp.4
-  float w3[64 * 64];           // k-major coors_mlp.0
+struct EdgeBwdSmem : EdgeTileSmem {
   float w2lin[64 * 64];        // edge_mlp.4.weight [out][in]   (k-major for dn = dmsg . W2)
   float w3lin[64 * 64];        // coors_mlp.0.weight [out][in]  (k-major for dmsg += dz3 . W3)
-  float ln_g[64], ln_b[64], b2[64], b3[64], w4[64];
-  float bufE[EQD_TM * BE_LD1];  // [he | rbf]
-  float bufA[EQD_TM * BE_LD];   // current A operand
-  float bufH[EQD_TM * BE_LD];   // n-hat
+  float bufE[EQD_TM * EDGE_LD1];  // [he | rbf]
+  float bufA[EQD_TM * EDGE_LD];   // current A operand
+  float bufH[EQD_TM * EDGE_LD];   // n-hat
   float scratch[16 * 64];
-  double xrel[EQD_TM * 3];
   double dxm[EQD_TM * 3];
   float phi[EQD_TM], dphi[EQD_TM], rstd[EQD_TM], invdeg[EQD_TM];
-  int src[EQD_TM], dst[EQD_TM];
-  float cln_g[64], cln_b[64];   // coors_mlp.3 (CLN only)
 };
 
 // DROP: the forward applied dropout sites 0 / 1 of `dr` to z1 / z3; the same masks and scale enter the chain rule
@@ -57,24 +46,10 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
   const int tid = threadIdx.x, ty = tid >> 3, tx = tid & 7;
   const int pw = 128 + 3 * p.dhp;
   const float slope = p.leaky_slope;
-  for (int i = tid; i < BE_K1 * 64 / 4; i += EQD_THREADS)
-    reinterpret_cast<float4*>(s.w1)[i] = reinterpret_cast<const float4*>(p.w_edge1)[i];
+  edge_tile_weights<CLN>(s, p, nm, tid);
   for (int i = tid; i < 64 * 64 / 4; i += EQD_THREADS) {
-    reinterpret_cast<float4*>(s.w2)[i] = reinterpret_cast<const float4*>(p.w_edge2)[i];
-    reinterpret_cast<float4*>(s.w3)[i] = reinterpret_cast<const float4*>(p.w_coor1)[i];
     reinterpret_cast<float4*>(s.w2lin)[i] = reinterpret_cast<const float4*>(w2lin)[i];
     reinterpret_cast<float4*>(s.w3lin)[i] = reinterpret_cast<const float4*>(w3lin)[i];
-  }
-  if (tid < 64) {
-    s.ln_g[tid] = p.edge_ln_g[tid];
-    s.ln_b[tid] = p.edge_ln_b[tid];
-    s.b2[tid] = p.b_edge2[tid];
-    s.b3[tid] = p.b_coor1[tid];
-    s.w4[tid] = p.w_coor2[tid];
-  }
-  if (CLN && tid < 64) {
-    s.cln_g[tid] = nm.coors_ln_g[tid];
-    s.cln_b[tid] = nm.coors_ln_b[tid];
   }
   __syncthreads();
   float gsum[8], bsum[8], w4sum[8], b4sum = 0.f;
@@ -88,122 +63,65 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
     const int e0 = tile * EQD_TM;
     const int ne = min(EQD_TM, E - e0);
     // ---- per-edge geometry and the gradient of the two mean aggregations: thread t <-> edge e0 + t ----
-    {
-      float* row = s.bufE + tid * BE_LD1;
-      if (tid < ne) {
-        const int e = e0 + tid;
-        const int sn = g.col_src[e], dn = g.edge_dst[e];
-        s.src[tid] = sn;
-        s.dst[tid] = dn;
-        const double rx = x_in[(long)sn * 3 + 0] - x_in[(long)dn * 3 + 0];
-        const double ry = x_in[(long)sn * 3 + 1] - x_in[(long)dn * 3 + 1];
-        const double rz = x_in[(long)sn * 3 + 2] - x_in[(long)dn * 3 + 2];
-        s.xrel[tid * 3 + 0] = rx; s.xrel[tid * 3 + 1] = ry; s.xrel[tid * 3 + 2] = rz;
-        const float d2 = (float)(rx * rx + ry * ry + rz * rz);
-        float sigma = 1.f;
-#pragma unroll
-        for (int q = 0; q < EQD_N_RBF; ++q) {
-          row[EQD_EDGE_FEATS + q] = expf(-d2 / sigma);
-          sigma *= 1.5f;
-        }
-        const int deg = g.row_ptr[dn + 1] - g.row_ptr[dn];
-        const double inv = deg > 0 ? 1.0 / (double)deg : 0.0;
-        s.invdeg[tid] = (float)inv;
-        const double mx = dx_out[(long)dn * 3 + 0] * inv, my = dx_out[(long)dn * 3 + 1] * inv, mz = dx_out[(long)dn * 3 + 2] * inv;
-        s.dxm[tid * 3 + 0] = mx; s.dxm[tid * 3 + 1] = my; s.dxm[tid * 3 + 2] = mz;
-        const float dph = (float)(rx * mx + ry * my + rz * mz);
-        s.dphi[tid] = dph;
-        b4sum += dph;
-      } else {
-        s.src[tid] = -1;
-        s.dst[tid] = -1;
-        s.invdeg[tid] = 0.f;
-        s.dphi[tid] = 0.f;
-#pragma unroll
-        for (int q = 0; q < EQD_N_RBF; ++q) row[EQD_EDGE_FEATS + q] = 0.f;
-      }
-      row[42] = 0.f;
-      row[43] = 0.f;
-    }
-    for (int idx = tid; idx < EQD_TM * EQD_EDGE_FEATS; idx += EQD_THREADS) {
-      int r = idx / EQD_EDGE_FEATS, k = idx - r * EQD_EDGE_FEATS;
-      float v = 0.f;
-      if (r < ne) {
-        int e = e0 + r;
-        v = e < g.n_lig_edges ? g.he_lig[(long)e * EQD_EDGE_FEATS + k]
-                              : g.he_rec[(long)(e - g.n_lig_edges) * EQD_EDGE_FEATS + k];
-      }
-      s.bufE[r * BE_LD1 + k] = v;
+    edge_tile_inputs(s, s.bufE, g, x_in, e0, ne, tid);
+    if (tid < ne) {
+      const int dn = s.dst[tid];
+      const double rx = s.xrel[tid * 3 + 0], ry = s.xrel[tid * 3 + 1], rz = s.xrel[tid * 3 + 2];
+      const int deg = g.row_ptr[dn + 1] - g.row_ptr[dn];
+      const double inv = deg > 0 ? 1.0 / (double)deg : 0.0;
+      s.invdeg[tid] = (float)inv;
+      const double mx = dx_out[(long)dn * 3 + 0] * inv, my = dx_out[(long)dn * 3 + 1] * inv, mz = dx_out[(long)dn * 3 + 2] * inv;
+      s.dxm[tid * 3 + 0] = mx; s.dxm[tid * 3 + 1] = my; s.dxm[tid * 3 + 2] = mz;
+      const float dph = (float)(rx * mx + ry * my + rz * mz);
+      s.dphi[tid] = dph;
+      b4sum += dph;
+    } else {
+      s.invdeg[tid] = 0.f;
+      s.dphi[tid] = 0.f;
     }
     __syncthreads();
     // ein = [he | rbf | 0 0] -> global (X operand of dW1e)
-    for (int idx = tid; idx < ne * (BE_K1 / 4); idx += EQD_THREADS) {
-      int r = idx / (BE_K1 / 4), c4 = idx - r * (BE_K1 / 4);
-      *reinterpret_cast<float4*>(ein_out + (long)(e0 + r) * BE_K1 + c4 * 4) =
-          *reinterpret_cast<const float4*>(s.bufE + r * BE_LD1 + c4 * 4);
+    for (int idx = tid; idx < ne * (EDGE_K1 / 4); idx += EQD_THREADS) {
+      int r = idx / (EDGE_K1 / 4), c4 = idx - r * (EDGE_K1 / 4);
+      *reinterpret_cast<float4*>(ein_out + (long)(e0 + r) * EDGE_K1 + c4 * 4) =
+          *reinterpret_cast<const float4*>(s.bufE + r * EDGE_LD1 + c4 * 4);
     }
     // ---- z1, LeakyReLU, LayerNorm: keep n-hat (smem), rstd (smem), sign(z1) (registers) ----
     float acc[8][8], accx[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      int r = ty * 8 + i;
-      int sn = s.src[r], dn = s.dst[r];
-      if (sn >= 0) {
-        const float* ps = proj + (long)sn * pw + tx * 4;
-        const float* pd = proj + (long)dn * pw + 64 + tx * 4;
-        float4 a0 = *reinterpret_cast<const float4*>(ps), a1 = *reinterpret_cast<const float4*>(ps + 32);
-        float4 b0 = *reinterpret_cast<const float4*>(pd), b1 = *reinterpret_cast<const float4*>(pd + 32);
-        acc[i][0] = a0.x + b0.x; acc[i][1] = a0.y + b0.y; acc[i][2] = a0.z + b0.z; acc[i][3] = a0.w + b0.w;
-        acc[i][4] = a1.x + b1.x; acc[i][5] = a1.y + b1.y; acc[i][6] = a1.z + b1.z; acc[i][7] = a1.w + b1.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-      }
-    }
-    gemm_nn<false>(acc, accx, s.bufE + ty * 8 * BE_LD1, BE_LD1, s.w1, 64, BE_K1, tx);
-    if (DROP) dropout_tile<false>(acc, accx, dr, 0, e0 + ty * 8, tx);
+    edge_tile_z1<DROP>(acc, accx, s, s.bufE, proj, pw, dr, e0, ty, tx);
     unsigned pos_lo = 0, pos_hi = 0;
     float nrm[8][8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      float sum = 0.f;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         float a = lrelu(acc[i][j], slope);
         if (a > 0.f) { if (i < 4) pos_lo |= 1u << (i * 8 + j); else pos_hi |= 1u << ((i - 4) * 8 + j); }
         acc[i][j] = a;
-        sum += a;
       }
-      const float mean = row_sum8(sum) * (1.f / 64.f);
-      float q = 0.f;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float d = acc[i][j] - mean;
-        q = fmaf(d, d, q);
-      }
-      const float rstd = 1.f / sqrtf(row_sum8(q) * (1.f / 64.f) + 1e-5f);
-      if (tx == 0) s.rstd[ty * 8 + i] = rstd;
+      const LnRow st = ln_row_stats(acc[i], 1.f / 64.f);
+      if (tx == 0) s.rstd[ty * 8 + i] = st.rstd;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int c = col_nn(tx, j);
-        acc[i][j] = (acc[i][j] - mean) * rstd;                 // n-hat
+        acc[i][j] = (acc[i][j] - st.mean) * st.rstd;           // n-hat
         nrm[i][j] = acc[i][j] * s.ln_g[c] + s.ln_b[c];          // n1
       }
     }
-    store_tile_smem<false>(s.bufH, BE_LD, acc, accx, ty, tx);
-    store_tile_smem<false>(s.bufA, BE_LD, nrm, accx, ty, tx);
+    store_tile_smem<false>(s.bufH, EDGE_LD, acc, accx, ty, tx);
+    store_tile_smem<false>(s.bufA, EDGE_LD, nrm, accx, ty, tx);
     store_tile_global(n1_out, e0, 64, ne, nrm, ty, tx);
     __syncthreads();
     // ---- msg = W2 n1 + b2 ----
     acc_set_bias(acc, s.b2, tx);
-    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * BE_LD, BE_LD, s.w2, 64, 64, tx);
+    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * EDGE_LD, EDGE_LD, s.w2, 64, 64, tx);
     __syncthreads();
-    store_tile_smem<false>(s.bufA, BE_LD, acc, accx, ty, tx);
+    store_tile_smem<false>(s.bufA, EDGE_LD, acc, accx, ty, tx);
     store_tile_global(msg_out, e0, 64, ne, acc, ty, tx);
     __syncthreads();
     // ---- z3 = W3 msg + b3, c3 = lrelu(z3), phi; dz3 = dphi w4 lrelu'(z3); dw4 += c3 dphi ----
     acc_set_bias(acc, s.b3, tx);
-    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * BE_LD, BE_LD, s.w3, 64, 64, tx);
+    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * EDGE_LD, EDGE_LD, s.w3, 64, 64, tx);
     float keep[8][8];   // DROP: mask * scale of z3 (the same factor then carries dz3 back through the dropout)
     if (DROP) {
 #pragma unroll
@@ -225,26 +143,16 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
         const int r = ty * 8 + i;
         const float dph = s.dphi[r];
         float v = 0.f;
-        if (CLN) {   // LayerNorm statistics in the order of the forward's lrelu_layernorm
-          float c3[8], sum = 0.f;
+        if (CLN) {
+          float c3[8];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            c3[j] = lrelu(acc[i][j], slope);
-            sum += c3[j];
-          }
-          const float mean = row_sum8(sum) * (1.f / 64.f);
-          float q = 0.f;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float d = c3[j] - mean;
-            q = fmaf(d, d, q);
-          }
-          const float rstd = 1.f / sqrtf(row_sum8(q) * (1.f / 64.f) + 1e-5f);
-          float nhat[8], dnh[8], s1 = 0.f, s2 = 0.f;
+          for (int j = 0; j < 8; ++j) c3[j] = lrelu(acc[i][j], slope);
+          const LnRow st = ln_row_stats(c3, 1.f / 64.f);
+          float nhat[8], dnh[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             const int c = col_nn(tx, j);
-            nhat[j] = (c3[j] - mean) * rstd;
+            nhat[j] = (c3[j] - st.mean) * st.rstd;
             const float n3 = nhat[j] * s.cln_g[c] + s.cln_b[c];
             v = fmaf(n3, w4r[j], v);
             w4sum[j] = fmaf(n3, dph, w4sum[j]);
@@ -252,13 +160,11 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
             cgsum[j] = fmaf(dn3, nhat[j], cgsum[j]);
             cbsum[j] += dn3;
             dnh[j] = dn3 * s.cln_g[c];
-            s1 += dnh[j];
-            s2 = fmaf(dnh[j], nhat[j], s2);
           }
-          const float m1 = row_sum8(s1) * (1.f / 64.f), m2 = row_sum8(s2) * (1.f / 64.f);
+          layernorm_bwd_row(dnh, nhat, st.rstd);
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            acc[i][j] = rstd * (dnh[j] - m1 - nhat[j] * m2) * lrelu_grad_from_post(c3[j], slope);   // dz3
+            acc[i][j] = dnh[j] * lrelu_grad_from_post(c3[j], slope);   // dz3
             if (DROP) acc[i][j] *= keep[i][j];
           }
         } else {
@@ -276,7 +182,7 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
       }
     }
     __syncthreads();   // bufA (msg) no longer read
-    store_tile_smem<false>(s.bufA, BE_LD, acc, accx, ty, tx);
+    store_tile_smem<false>(s.bufA, EDGE_LD, acc, accx, ty, tx);
     store_tile_global(dz3_out, e0, 64, ne, acc, ty, tx);
     __syncthreads();
     // ---- dmsg = daggr[dst] / deg + dz3 . W3 ----
@@ -295,9 +201,9 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
         for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
       }
     }
-    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * BE_LD, BE_LD, s.w3lin, 64, 64, tx);
+    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * EDGE_LD, EDGE_LD, s.w3lin, 64, 64, tx);
     __syncthreads();
-    store_tile_smem<false>(s.bufA, BE_LD, acc, accx, ty, tx);
+    store_tile_smem<false>(s.bufA, EDGE_LD, acc, accx, ty, tx);
     store_tile_global(dmsg_out, e0, 64, ne, acc, ty, tx);
     __syncthreads();
     // ---- dn = dmsg . W2; LayerNorm backward; dz1 = da lrelu'(z1) ----
@@ -305,12 +211,12 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
     for (int i = 0; i < 8; ++i)
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * BE_LD, BE_LD, s.w2lin, 64, 64, tx);
+    gemm_nn<false>(acc, accx, s.bufA + ty * 8 * EDGE_LD, EDGE_LD, s.w2lin, 64, 64, tx);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int r = ty * 8 + i;
-      const float* nh = s.bufH + r * BE_LD;
-      float nhat[8], s1 = 0.f, s2 = 0.f;
+      const float* nh = s.bufH + r * EDGE_LD;
+      float nhat[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int c = col_nn(tx, j);
@@ -318,26 +224,23 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
         const float dn = acc[i][j];
         gsum[j] = fmaf(dn, nhat[j], gsum[j]);
         bsum[j] += dn;
-        const float dnh = dn * s.ln_g[c];
-        acc[i][j] = dnh;
-        s1 += dnh;
-        s2 = fmaf(dnh, nhat[j], s2);
+        acc[i][j] = dn * s.ln_g[c];
       }
-      const float m1 = row_sum8(s1) * (1.f / 64.f), m2 = row_sum8(s2) * (1.f / 64.f), rstd = s.rstd[r];
+      layernorm_bwd_row(acc[i], nhat, s.rstd[r]);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const bool pos = i < 4 ? (pos_lo >> (i * 8 + j)) & 1u : (pos_hi >> ((i - 4) * 8 + j)) & 1u;
-        acc[i][j] = rstd * (acc[i][j] - m1 - nhat[j] * m2) * (pos ? 1.f : slope);
+        acc[i][j] *= pos ? 1.f : slope;
       }
     }
     if (DROP) dropout_tile<false>(acc, accx, dr, 0, e0 + ty * 8, tx);   // dz1 = d(dropout output) * mask * scale
     __syncthreads();   // bufA (dmsg) no longer read
-    store_tile_smem<false>(s.bufA, BE_LD, acc, accx, ty, tx);
+    store_tile_smem<false>(s.bufA, EDGE_LD, acc, accx, ty, tx);
     store_tile_global(dz1_out, e0, 64, ne, acc, ty, tx);
     __syncthreads();
     // ---- coordinates: thread t <-> edge.  drbf = dz1 . W1e[rbf rows]; d(d^2); dx_rel ----
     if (tid < ne) {
-      const float* dz = s.bufA + tid * BE_LD;
+      const float* dz = s.bufA + tid * EDGE_LD;
       float drbf[EQD_N_RBF];
 #pragma unroll
       for (int q = 0; q < EQD_N_RBF; ++q) drbf[q] = 0.f;
@@ -353,7 +256,7 @@ bwd_edge_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ w2lin
       double dd2 = 0.0, sigma = 1.0;
 #pragma unroll
       for (int q = 0; q < EQD_N_RBF; ++q) {
-        dd2 -= (double)drbf[q] * (double)s.bufE[tid * BE_LD1 + EQD_EDGE_FEATS + q] / sigma;
+        dd2 -= (double)drbf[q] * (double)s.bufE[tid * EDGE_LD1 + EQD_EDGE_FEATS + q] / sigma;
         sigma *= 1.5;
       }
       const double ph = (double)s.phi[tid];

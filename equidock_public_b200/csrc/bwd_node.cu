@@ -94,36 +94,22 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
     const float inv_n = 1.f / (float)p.dh;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      float s = 0.f;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         float a = lrelu(acc[i][j], slope);
         if (a > 0.f) { if (i < 4) pos_lo |= 1u << (i * 8 + j); else pos_hi |= 1u << ((i - 4) * 8 + j); }
         acc[i][j] = a;
-        s += a;
       }
       if (EXTRA) {
         float a = xvalid ? lrelu(accx[i], slope) : 0.f;
         if (a > 0.f) pos_x |= 1u << i;
         accx[i] = a;
-        s += a;
       }
-      float mean = row_sum8(s) * inv_n;
-      float q = 0.f;
+      const LnRow st = ln_row_stats<EXTRA>(acc[i], inv_n, accx[i], xvalid);
+      if (tx == 0) rstd_s[ty * 8 + i] = st.rstd;
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float d = acc[i][j] - mean;
-        q = fmaf(d, d, q);
-      }
-      if (EXTRA && xvalid) {
-        float d = accx[i] - mean;
-        q = fmaf(d, d, q);
-      }
-      float rstd = 1.f / sqrtf(row_sum8(q) * inv_n + 1e-5f);
-      if (tx == 0) rstd_s[ty * 8 + i] = rstd;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[i][j] = (acc[i][j] - mean) * rstd;      // n-hat
-      if (EXTRA) accx[i] = xvalid ? (accx[i] - mean) * rstd : 0.f;
+      for (int j = 0; j < 8; ++j) acc[i][j] = (acc[i][j] - st.mean) * st.rstd;      // n-hat
+      if (EXTRA) accx[i] = xvalid ? (accx[i] - st.mean) * st.rstd : 0.f;
     }
     store_tile_smem<EXTRA>(bufH, LD, acc, accx, ty, tx);
     if (HLN) {   // n5 of every row -> bufB: A operand of the recomputed node_mlp.4 product
@@ -164,51 +150,27 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int r = ty * 8 + i;
-        if (skip && r < nvalid) {
-          const float* hr = h_in + (long)(node0 + r) * ldh + tx * 4;
-          const float4 a = *reinterpret_cast<const float4*>(hr), b = *reinterpret_cast<const float4*>(hr + 32);
-          const float s1 = 1.f - p.skip_weight_h, s0 = p.skip_weight_h;
-          y[i][0] = s0 * y[i][0] + s1 * a.x; y[i][1] = s0 * y[i][1] + s1 * a.y;
-          y[i][2] = s0 * y[i][2] + s1 * a.z; y[i][3] = s0 * y[i][3] + s1 * a.w;
-          y[i][4] = s0 * y[i][4] + s1 * b.x; y[i][5] = s0 * y[i][5] + s1 * b.y;
-          y[i][6] = s0 * y[i][6] + s1 * b.z; y[i][7] = s0 * y[i][7] + s1 * b.w;
-        }
-        float s = 0.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s += y[i][j];
-        const float mean = row_sum8(s) * (1.f / 64.f);
-        float q = 0.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float dv = y[i][j] - mean;
-          q = fmaf(dv, dv, q);
-        }
-        const float rstd = 1.f / sqrtf(row_sum8(q) * (1.f / 64.f) + 1e-5f);
+        if (skip && r < nvalid) skip_row(y[i], h_in + (long)(node0 + r) * ldh + tx * 4, p.skip_weight_h);
+        const LnRow st = ln_row_stats(y[i], 1.f / 64.f);
         float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         if (r < nvalid) {
           const float* gr = dy_io + (long)(node0 + r) * 64 + tx * 4;
           const float4 a = *reinterpret_cast<const float4*>(gr), b = *reinterpret_cast<const float4*>(gr + 32);
           g[0] = a.x; g[1] = a.y; g[2] = a.z; g[3] = a.w; g[4] = b.x; g[5] = b.y; g[6] = b.z; g[7] = b.w;
         }
-        float s1 = 0.f, s2 = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int c = col_nn(tx, j);
-          y[i][j] = (y[i][j] - mean) * rstd;                   // y-hat
+          y[i][j] = (y[i][j] - st.mean) * st.rstd;             // y-hat
           fgsum[j] = fmaf(g[j], y[i][j], fgsum[j]);
           fbsum[j] += g[j];
           g[j] *= nm.final_ln_g[c];
-          s1 += g[j];
-          s2 = fmaf(g[j], y[i][j], s2);
         }
-        const float m1 = row_sum8(s1) * (1.f / 64.f), m2 = row_sum8(s2) * (1.f / 64.f);
+        layernorm_bwd_row(g, y[i], st.rstd);                   // dy
         if (r < nvalid) {
-          float dy[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) dy[j] = rstd * (g[j] - m1 - y[i][j] * m2);
           float* o = dy_io + (long)(node0 + r) * 64 + tx * 4;
-          *reinterpret_cast<float4*>(o) = make_float4(dy[0], dy[1], dy[2], dy[3]);
-          *reinterpret_cast<float4*>(o + 32) = make_float4(dy[4], dy[5], dy[6], dy[7]);
+          *reinterpret_cast<float4*>(o) = make_float4(g[0], g[1], g[2], g[3]);
+          *reinterpret_cast<float4*>(o + 32) = make_float4(g[4], g[5], g[6], g[7]);
         }
       }
       __syncthreads();   // dy of the tile is in dy_io for the loads below
@@ -226,6 +188,8 @@ bwd_node_mlp_kernel(int n_nodes, eqd_layer_params p, const float* __restrict__ w
     }
     gemm_nn_stream<EXTRA>(acc, accx, bufA + ty * 8 * LD, LD, 64, w_node2_lin, DHP, DHP, wbuf, tid);
     // ---------------- LayerNorm backward, LeakyReLU backward -> du ----------------
+    // Not layernorm_bwd_row: through it ptxas contracts other products by inv_n = 1/69 into FFMAs in the 69-wide
+    // instantiations, which would change layer 0's gradients in the last bits.
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const int r = ty * 8 + i;

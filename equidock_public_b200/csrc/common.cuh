@@ -210,7 +210,33 @@ __device__ __forceinline__ float row_max8(float v) {
   return v;
 }
 
-// LeakyReLU then nn.LayerNorm (biased variance, eps 1e-5) over `dh` real channels of each row.
+// nn.LayerNorm statistics (biased variance, eps 1e-5) of one row held by its 8 lanes: this lane's 8 values v and, with
+// EXTRA, its channel 64 + tx in vx (0 unless xvalid); inv_n = 1 / channel count.  The one definition of the statistics
+// for every fp32 forward LayerNorm and every backward recompute of one, so both see the same mean and rstd bits.
+struct LnRow {
+  float mean, rstd;
+};
+template <bool EXTRA = false>
+__device__ __forceinline__ LnRow ln_row_stats(const float (&v)[8], float inv_n, float vx = 0.f, bool xvalid = false) {
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) s += v[j];
+  if (EXTRA) s += vx;
+  const float mean = row_sum8(s) * inv_n;
+  float q = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const float d = v[j] - mean;
+    q = fmaf(d, d, q);
+  }
+  if (EXTRA && xvalid) {
+    const float d = vx - mean;
+    q = fmaf(d, d, q);
+  }
+  return {mean, 1.f / sqrtf(row_sum8(q) * inv_n + 1e-5f)};
+}
+
+// LeakyReLU then nn.LayerNorm over `dh` real channels of each row.
 // EXTRA: channels 64..64+7 live in accx (valid iff 64+tx < dh).  gamma/beta indexed by channel.
 template <bool EXTRA>
 __device__ __forceinline__ void lrelu_layernorm(float (&acc)[8][8], float (&accx)[8], const float* __restrict__ gamma,
@@ -219,61 +245,43 @@ __device__ __forceinline__ void lrelu_layernorm(float (&acc)[8][8], float (&accx
   const bool xvalid = EXTRA && (64 + tx < dh);
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    float s = 0.f;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      acc[i][j] = lrelu(acc[i][j], slope);
-      s += acc[i][j];
-    }
-    if (EXTRA) {
-      accx[i] = xvalid ? lrelu(accx[i], slope) : 0.f;
-      s += accx[i];
-    }
-    float mean = row_sum8(s) * inv_n;
-    float q = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float d = acc[i][j] - mean;
-      q = fmaf(d, d, q);
-    }
-    if (EXTRA && xvalid) {
-      float d = accx[i] - mean;
-      q = fmaf(d, d, q);
-    }
-    float var = row_sum8(q) * inv_n;
-    float rstd = 1.f / sqrtf(var + 1e-5f);
+    for (int j = 0; j < 8; ++j) acc[i][j] = lrelu(acc[i][j], slope);
+    if (EXTRA) accx[i] = xvalid ? lrelu(accx[i], slope) : 0.f;
+    const LnRow st = ln_row_stats<EXTRA>(acc[i], inv_n, accx[i], xvalid);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       int c = col_nn(tx, j);
-      acc[i][j] = (acc[i][j] - mean) * rstd * gamma[c] + beta[c];
+      acc[i][j] = (acc[i][j] - st.mean) * st.rstd * gamma[c] + beta[c];
     }
-    if (EXTRA) accx[i] = xvalid ? (accx[i] - mean) * rstd * gamma[64 + tx] + beta[64 + tx] : 0.f;
+    if (EXTRA) accx[i] = xvalid ? (accx[i] - st.mean) * st.rstd * gamma[64 + tx] + beta[64 + tx] : 0.f;
   }
 }
 
-// nn.LayerNorm(64) (biased variance, eps 1e-5) of each row of a 64-wide micro-tile, with the statistics code of
-// lrelu_layernorm.  gamma/beta indexed by channel.
+// nn.LayerNorm(64) of each row of a 64-wide micro-tile.  gamma/beta indexed by channel.
 __device__ __forceinline__ void layernorm64(float (&acc)[8][8], const float* __restrict__ gamma,
                                             const float* __restrict__ beta, int tx) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s += acc[i][j];
-    const float mean = row_sum8(s) * (1.f / 64.f);
-    float q = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float d = acc[i][j] - mean;
-      q = fmaf(d, d, q);
-    }
-    const float rstd = 1.f / sqrtf(row_sum8(q) * (1.f / 64.f) + 1e-5f);
+    const LnRow st = ln_row_stats(acc[i], 1.f / 64.f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int c = col_nn(tx, j);
-      acc[i][j] = (acc[i][j] - mean) * rstd * gamma[c] + beta[c];
+      acc[i][j] = (acc[i][j] - st.mean) * st.rstd * gamma[c] + beta[c];
     }
   }
+}
+
+// Skip connection of the node update (rigid_docking_model.py:332-334) on one row of a 64-wide micro-tile:
+// v = sk * v + (1 - sk) * h, hr = the row's h at this lane's first column (tx * 4).  The fmaf pairing is explicit because
+// the compiler's own contraction of this expression depends on the surrounding code; this is the one the kernels use.
+__device__ __forceinline__ void skip_row(float (&v)[8], const float* __restrict__ hr, float sk) {
+  const float4 a = *reinterpret_cast<const float4*>(hr), b = *reinterpret_cast<const float4*>(hr + 32);
+  const float sk1 = 1.f - sk;
+  v[0] = fmaf(sk, v[0], sk1 * a.x); v[1] = fmaf(sk1, a.y, sk * v[1]);
+  v[2] = fmaf(sk1, a.z, sk * v[2]); v[3] = fmaf(sk1, a.w, sk * v[3]);
+  v[4] = fmaf(sk1, b.x, sk * v[4]); v[5] = fmaf(sk1, b.y, sk * v[5]);
+  v[6] = fmaf(sk1, b.z, sk * v[6]); v[7] = fmaf(sk1, b.w, sk * v[7]);
 }
 
 // Store the micro-tile (NN column map) row-major into shared memory (row stride ld).

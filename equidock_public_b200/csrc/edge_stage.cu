@@ -5,27 +5,14 @@
 // The first Linear of the edge MLP is split: its [h_src | h_dst] columns were applied per NODE
 // by the projection stage (Psrc, Pdst(+bias)); only the 27+15 per-edge columns are a GEMM here.
 // Per-edge activations never leave the SM.
-#include "common.cuh"
-#include "philox.cuh"
+#include "edge_tile.cuh"
 
 namespace eqd {
 
-#define EDGE_K1 44    // 27 he + 15 rbf + 2 zero
-#define EDGE_LD1 48   // smem row stride of the [he|rbf] operand
-#define EDGE_LD 68    // smem row stride of 64-wide operands
-
-struct EdgeSmem {
-  float w1[EDGE_K1 * 64];
-  float w2[64 * 64];
-  float w3[64 * 64];
-  float ln_g[64], ln_b[64], b2[64], b3[64], w4[64];
+struct EdgeSmem : EdgeTileSmem {
   float buf[EQD_TM * EDGE_LD];
-  double xrel[EQD_TM * 3];
   float phi[EQD_TM];
-  int src[EQD_TM];
-  int dst[EQD_TM];
   int rp[EQD_TM + 1];
-  float cln_g[64], cln_b[64];   // coors_mlp.3 (CLN only)
 };
 
 // DROP: training-mode dropout sites 0 (z1) and 1 (z3) of eqd_dropout `dr`, applied before their LeakyReLU.
@@ -41,24 +28,7 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
   const int tid = threadIdx.x, ty = tid >> 3, tx = tid & 7;
   const int pw = 128 + 3 * p.dhp;
 
-  // layer weights -> shared memory, once per CTA
-  for (int i = tid; i < EDGE_K1 * 64 / 4; i += EQD_THREADS)
-    reinterpret_cast<float4*>(s.w1)[i] = reinterpret_cast<const float4*>(p.w_edge1)[i];
-  for (int i = tid; i < 64 * 64 / 4; i += EQD_THREADS) {
-    reinterpret_cast<float4*>(s.w2)[i] = reinterpret_cast<const float4*>(p.w_edge2)[i];
-    reinterpret_cast<float4*>(s.w3)[i] = reinterpret_cast<const float4*>(p.w_coor1)[i];
-  }
-  if (tid < 64) {
-    s.ln_g[tid] = p.edge_ln_g[tid];
-    s.ln_b[tid] = p.edge_ln_b[tid];
-    s.b2[tid] = p.b_edge2[tid];
-    s.b3[tid] = p.b_coor1[tid];
-    s.w4[tid] = p.w_coor2[tid];
-  }
-  if (CLN && tid < 64) {
-    s.cln_g[tid] = nm.coors_ln_g[tid];
-    s.cln_b[tid] = nm.coors_ln_b[tid];
-  }
+  edge_tile_weights<CLN>(s, p, nm, tid);  // once per CTA
   __syncthreads();
 
   const int ntiles = (g.n_nodes + tn - 1) / tn;
@@ -75,69 +45,12 @@ edge_stage_kernel(eqd_graph g, eqd_layer_params p, const float* __restrict__ pro
       continue;
     }
 
-    // ---- per-edge geometry: thread t <-> edge e0+t ------------------------------------------
-    {
-      float* row = s.buf + tid * EDGE_LD1;
-      if (tid < ne) {
-        int e = e0 + tid;
-        int sn = g.col_src[e], dn = g.edge_dst[e];
-        s.src[tid] = sn;
-        s.dst[tid] = dn;
-        double rx = x_in[(long)sn * 3 + 0] - x_in[(long)dn * 3 + 0];  // u_sub_v :204-205
-        double ry = x_in[(long)sn * 3 + 1] - x_in[(long)dn * 3 + 1];
-        double rz = x_in[(long)sn * 3 + 2] - x_in[(long)dn * 3 + 2];
-        s.xrel[tid * 3 + 0] = rx;
-        s.xrel[tid * 3 + 1] = ry;
-        s.xrel[tid * 3 + 2] = rz;
-        float d2 = (float)(rx * rx + ry * ry + rz * rz);  // :208-209
-        float sigma = 1.f;
-#pragma unroll
-        for (int q = 0; q < EQD_N_RBF; ++q) {  // exp(-d^2 / 1.5^q) :210
-          row[EQD_EDGE_FEATS + q] = expf(-d2 / sigma);
-          sigma *= 1.5f;
-        }
-      } else {
-        s.src[tid] = -1;
-        s.dst[tid] = -1;
-#pragma unroll
-        for (int q = 0; q < EQD_N_RBF; ++q) row[EQD_EDGE_FEATS + q] = 0.f;
-      }
-      row[42] = 0.f;
-      row[43] = 0.f;
-    }
-    // original edge features he (E,27): the tile's rows are contiguous in one of the two arrays
-    for (int idx = tid; idx < EQD_TM * EQD_EDGE_FEATS; idx += EQD_THREADS) {
-      int r = idx / EQD_EDGE_FEATS, k = idx - r * EQD_EDGE_FEATS;
-      float v = 0.f;
-      if (r < ne) {
-        int e = e0 + r;
-        v = e < g.n_lig_edges ? g.he_lig[(long)e * EQD_EDGE_FEATS + k]
-                              : g.he_rec[(long)(e - g.n_lig_edges) * EQD_EDGE_FEATS + k];
-      }
-      s.buf[r * EDGE_LD1 + k] = v;
-    }
+    edge_tile_inputs(s, s.buf, g, x_in, e0, ne, tid);
     __syncthreads();
 
     // ---- edge_mlp.0: gathered node projections + [he|rbf] GEMM -------------------------------
     float acc[8][8], accx[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      int r = ty * 8 + i;
-      int sn = s.src[r], dn = s.dst[r];
-      if (sn >= 0) {
-        const float* ps = proj + (long)sn * pw + tx * 4;       // Psrc row
-        const float* pd = proj + (long)dn * pw + 64 + tx * 4;  // Pdst row (+bias)
-        float4 a0 = *reinterpret_cast<const float4*>(ps), a1 = *reinterpret_cast<const float4*>(ps + 32);
-        float4 b0 = *reinterpret_cast<const float4*>(pd), b1 = *reinterpret_cast<const float4*>(pd + 32);
-        acc[i][0] = a0.x + b0.x; acc[i][1] = a0.y + b0.y; acc[i][2] = a0.z + b0.z; acc[i][3] = a0.w + b0.w;
-        acc[i][4] = a1.x + b1.x; acc[i][5] = a1.y + b1.y; acc[i][6] = a1.z + b1.z; acc[i][7] = a1.w + b1.w;
-      } else {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-      }
-    }
-    gemm_nn<false>(acc, accx, s.buf + ty * 8 * EDGE_LD1, EDGE_LD1, s.w1, 64, EDGE_K1, tx);
-    if (DROP) dropout_tile<false>(acc, accx, dr, 0, e0 + ty * 8, tx);
+    edge_tile_z1<DROP>(acc, accx, s, s.buf, proj, pw, dr, e0, ty, tx);
     lrelu_layernorm<false>(acc, accx, s.ln_g, s.ln_b, 64, p.leaky_slope, tx);  // edge_mlp.2-3
     __syncthreads();  // everyone is done reading the [he|rbf] operand
     store_tile_smem<false>(s.buf, EDGE_LD, acc, accx, ty, tx);

@@ -170,15 +170,7 @@ node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const int r = ty * 8 + i;
-        if (skip && r < nvalid) {
-          const float* hr = h_in + (long)(node0 + r) * ldh + tx * 4;
-          float4 a = *reinterpret_cast<const float4*>(hr), b = *reinterpret_cast<const float4*>(hr + 32);
-          const float sk = p.skip_weight_h, sk1 = 1.f - p.skip_weight_h;
-          acc[i][0] = sk * acc[i][0] + sk1 * a.x; acc[i][1] = sk * acc[i][1] + sk1 * a.y;
-          acc[i][2] = sk * acc[i][2] + sk1 * a.z; acc[i][3] = sk * acc[i][3] + sk1 * a.w;
-          acc[i][4] = sk * acc[i][4] + sk1 * b.x; acc[i][5] = sk * acc[i][5] + sk1 * b.y;
-          acc[i][6] = sk * acc[i][6] + sk1 * b.z; acc[i][7] = sk * acc[i][7] + sk1 * b.w;
-        }
+        if (skip && r < nvalid) skip_row(acc[i], h_in + (long)(node0 + r) * ldh + tx * 4, p.skip_weight_h);
       }
       layernorm64(acc, nm.final_ln_g, nm.final_ln_b, tx);   // final_h_layernorm_layer
 #pragma unroll
@@ -195,15 +187,7 @@ node_stage_kernel(eqd_graph g, eqd_layer_params p, eqd_layer_params pn, int has_
     for (int i = 0; i < 8; ++i) {
       int r = ty * 8 + i;
       if (r < nvalid) {
-        if (skip) {
-          const float* hr = h_in + (long)(node0 + r) * ldh + tx * 4;
-          float4 a = *reinterpret_cast<const float4*>(hr), b = *reinterpret_cast<const float4*>(hr + 32);
-          const float sk = p.skip_weight_h, sk1 = 1.f - p.skip_weight_h;
-          acc[i][0] = sk * acc[i][0] + sk1 * a.x; acc[i][1] = sk * acc[i][1] + sk1 * a.y;
-          acc[i][2] = sk * acc[i][2] + sk1 * a.z; acc[i][3] = sk * acc[i][3] + sk1 * a.w;
-          acc[i][4] = sk * acc[i][4] + sk1 * b.x; acc[i][5] = sk * acc[i][5] + sk1 * b.y;
-          acc[i][6] = sk * acc[i][6] + sk1 * b.z; acc[i][7] = sk * acc[i][7] + sk1 * b.w;
-        }
+        if (skip) skip_row(acc[i], h_in + (long)(node0 + r) * ldh + tx * 4, p.skip_weight_h);
         float* orow = h_out + (long)(node0 + r) * EQD_HID + tx * 4;
         *reinterpret_cast<float4*>(orow) = make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]);
         *reinterpret_cast<float4*>(orow + 32) = make_float4(acc[i][4], acc[i][5], acc[i][6], acc[i][7]);
